@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — SVD UNet train-step frames/sec on B200 (BASELINE.json metric), one JSON line on rank 0.
+"""bench.py — SVD UNet train-step frames/sec on H100 (BASELINE.json metric), one JSON line on rank 0.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 2|4|5]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 2|4|5] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -18,6 +18,11 @@ sample of the same workload (fewer frames of the same 40x64 latents per step).
 
 --config selects the BASELINE.json configuration (default 2, the one the metric is quoted on; 4 = 25 frames 576x1024 with
 gradient checkpointing, 5 = rank-64 LoRA): same step, same JSON line, `config.workload` names it.
+
+--dump-outputs DIR writes what the last timed step computed, as a caller of the step receives it, to DIR/<name>.npy
+(float32): the loss, the UNet prediction, and a fixed seeded sample of the updated fp32 master weights and of their
+gradients. Weights, inputs and the sample are seeded, so two builds run with the same arguments can be compared array by
+array.
 
 Only the baseline legs (`cpu_baseline`, `--impl reference`, `gpu_eager_baseline`) import `oracle/`; the product arm takes
 its synthetic batches and the EDM loss from svd_xtend_b200.workload.
@@ -62,7 +67,10 @@ def parse():
     ap.add_argument("--no-families", action="store_true", help="skip the per-family ablation rooflines")
     ap.add_argument("--no-script-path", action="store_true", help="skip the unchanged-script (eager, torch.optim.AdamW) timing")
     ap.add_argument("--no-graph", action="store_true", help="do not capture the step in a CUDA graph")
-    ap.add_argument("--profile-one", action="store_true", help="run warm-up + one eager step only (for ncu)")
+    ap.add_argument("--profile-one", action="store_true", help="run warm-up + one eager step only (for a profiler)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's loss, prediction and a seeded sample of the updated weights / gradients "
+                         "to DIR/<name>.npy (float32)")
     return ap.parse_args()
 
 
@@ -70,8 +78,9 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1400.0), d.get("bf16_tflops", 1590.0), d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json)"
-    return 1400.0, 1590.0, 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("bf16_tflops", 989.0), d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json)"
+    # NVIDIA H100 SXM data sheet (700 W card): dense BF16 989 TFLOP/s, HBM3 3.35 TB/s; a power-limited card reaches less
+    return 989.0, 989.0, 3350.0, "H100 SXM data sheet (dense BF16, HBM3), not a measurement"
 
 
 # ----------------------------------------------------------------------------- CPU reference arm
@@ -299,6 +308,24 @@ def gpu_eager_baseline(dev, cfg, steps=3, warmup=2):
 
 
 # ----------------------------------------------------------------------------- our arm
+DUMP_SAMPLE = 1 << 20     # elements of the weight / gradient arenas written by --dump-outputs (4 MB each)
+
+
+def dump_outputs(out_dir, loss, pred, arena):
+    """the last timed step's results as float32 .npy files (see --dump-outputs); the arena sample is a fixed seeded index set"""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    g = torch.Generator().manual_seed(20261015)
+    n = min(DUMP_SAMPLE, arena.numel)
+    idx = torch.randperm(arena.numel, generator=g)[:n].sort().values.to(arena.data.device)
+    arrays = {"loss": loss.detach().float().reshape(1), "pred": pred.detach().float(),
+              "weights_sample": arena.data[idx], "grads_sample": arena.grad[idx]}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.cpu().numpy().astype(np.float32))
+
+
+
 FAMILY_BOUND = {"linear": "tensor", "conv": "tensor", "attention": "tensor", "groupnorm": "hbm", "layernorm": "hbm", "adamw": "hbm",
                 "elementwise": "hbm"}
 
@@ -401,9 +428,14 @@ def main():
     devb = {k: v.to(dev) for k, v in host.items()}
     h2d_bytes = sum(v.numel() * v.element_size() for v in host.values())
 
+    # the prediction of the latest step (inside a captured graph: its static output buffer); detached, so that no warm-up
+    # autograd graph outlives its step (GraphedStep relies on that)
+    last = {}
+
     def step(b):
         arena.zero_grad()
         pred = unet(b["sample"], b["timestep"], b["encoder_hidden_states"], added_time_ids=b["added_time_ids"]).sample
+        last["pred"] = pred.detach()
         loss = edm_loss(pred.float(), b["noisy"], b["latents"], b["sigmas"])
         loss.backward()
         if reducer is not None:
@@ -441,7 +473,7 @@ def main():
             raw.SHAPE_LOG = []
         step(devb)
         torch.cuda.synchronize()
-        if raw.SHAPE_LOG is not None:     # the tapgemm launches of the LAST step, in launch order (scripts/join_shapes.py)
+        if raw.SHAPE_LOG is not None:     # the tapgemm launches of the LAST step, in launch order
             with open(os.environ["SVDX_SHAPE_LOG"], "w") as fh:
                 json.dump(raw.SHAPE_LOG, fh)
         return
@@ -486,6 +518,8 @@ def main():
     c1 = clocks.count() if clocks is not None else 0
     ms = e0.elapsed_time(e1)
     launches = raw.LAUNCHES[0] - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss, last["pred"], arena)
     for _ in range(2):          # one more sampling period under load before the sampler stops
         run_step()
     torch.cuda.synchronize()
@@ -547,7 +581,7 @@ def main():
     fam_ms = {}
     method = None
     if graph_captured and args.config == 4:
-        graphed = None              # one captured step of config 4 holds > 60 GB of activations: release it before re-capturing
+        graphed = None              # a captured step of config 4 holds most of the card's memory: release it before re-capturing
         torch.cuda.empty_cache()
     if graph_captured:
         todo = [("tapgemm", ["linear", "conv"])]
@@ -585,18 +619,9 @@ def main():
             raw.tapgemm = orig
         gemm_ms = sum(s_.elapsed_time(e_) for s_, e_ in recs)
         method = "sum of CUDA-event pairs around every svdx_tapgemm launch of one eager step (host launch gaps included)"
-    traffic, traffic_src = None, None
-    pdir = os.path.join(ROOT, "profiles")
-    for tp in sorted([f for f in os.listdir(pdir) if f.endswith("_traffic.json")] if os.path.isdir(pdir) else [], reverse=True):
-        try:
-            tj = json.load(open(os.path.join(pdir, tp)))
-            traffic, traffic_src = tj["traffic_bytes_per_launch"], f"profiles/{tp} (ncu dram__bytes_read+write summed over the {tj['launches_per_step']} tapgemm launches of one step, per launch)"
-            break
-        except Exception:
-            pass
     achieved = gemm_flops / (gemm_ms / 1e3) / 1e12 if gemm_ms and gemm_ms > 0 else 0.0
-    roofline = {"bound": "tensor", "kernel": "svdx::tapgemm2_kernel / tapgemm_kernel (tcgen05)", "achieved": achieved, "peak": sustained, "unit": "TFLOP/s",
-                "frac": achieved / sustained, "traffic": traffic, "traffic_source": traffic_src,
+    roofline = {"bound": "tensor", "kernel": "svdx::tapgemm_kernel (wgmma)", "achieved": achieved, "peak": sustained, "unit": "TFLOP/s",
+                "frac": achieved / sustained,
                 "algorithmic_bytes_note": "tensor-bound kernel: algorithmic work is FLOPs (2*M*N*K*taps per launch, summed); see DESIGN.md §3",
                 "peak_source": src + ", bf16_tflops_sustained (kernel timed inside a long step)",
                 "launches_per_step": gemm_launches, "algorithmic_tflop_per_step": gemm_flops / 1e12, "kernel_ms_per_step": gemm_ms,
@@ -769,7 +794,12 @@ def main():
     gpu_base = None
     if world == 1 and not args.no_gpu_baseline:
         try:
-            graphed = None
+            # the eager baseline builds its own copy of the model: release ours (model, arena, optimizer, graphs) first, an
+            # 80 GB card does not hold both
+            graphed = unet = arena = opt = loss = None
+            last.clear()
+            import gc
+            gc.collect()
             torch.cuda.empty_cache()
             gpu_base = gpu_eager_baseline(dev, cfg)
         except Exception as e:
@@ -789,7 +819,7 @@ def main():
         "config": {"workload": cfg["name"], "baseline_config": args.config, "frames": frames, "latent_hw": [lat_h, lat_w], "per_gpu_batch": 1,
                    "global_batch": world, "trainable_params": n_train, "total_params": n_total, "parallelism": f"dp{world}" + ("" if world == 1 else "-zero1-p2p" if isinstance(opt, P2PShardedAdamW) else "-zero1" if sharded else "-allreduce"),
                    "cuda_graph": graph_captured, "gradient_checkpointing": bool(cfg["grad_ckpt"]), "lora_rank": cfg["lora_rank"],
-                   "l2": "no explicit flush: the per-step working set (3 GB bf16 operand weights + >10 GB activations) is >> 126 MB L2",
+                   "l2": "no explicit flush: the per-step working set (3 GB bf16 operand weights + >10 GB activations) is >> 50 MB L2",
                    "final_loss": final_loss, "cpu_arm": CPU_ARM_NOTE},
         "clocks": clk,
         "e2e": {"value": e2e_value, "unit": "frames/s", "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": 4},

@@ -1,5 +1,5 @@
 /*
- * svd_xtend_b200 — C ABI of the B200-native SVD spatio-temporal UNet hot path.
+ * svd_xtend_b200 — C ABI of the H100-native (sm_90a) SVD spatio-temporal UNet hot path.
  *
  * Every entry point takes raw device pointers, explicit shapes/strides and a CUDA stream
  * (passed as void* == cudaStream_t). Contract for ALL functions:
@@ -41,7 +41,7 @@ extern "C" {
 #define SVDX_OUT_F32_ATOMIC 2  /* out += result (fp32 red.add), used by split-K weight gradients */
 
 /*
- * svdx_tapgemm — the one tensor-core contraction of the path (tcgen05.mma, TMEM accumulators,
+ * svdx_tapgemm — the one tensor-core contraction of the path (wgmma, register accumulators,
  * TMA-fed 128B-swizzled shared memory, warp-specialised persistent CTAs):
  *
  *     acc[m, n] = sum_{t < num_taps} sum_{k < K}  A_t[m, k] * B[n, t*K + k]
@@ -85,7 +85,7 @@ typedef struct SvdxTapGemm {
                               group, zero outside (dW of a (3,1,1) temporal conv tap) */
   /* problem */
   int32_t M, N, K;      /* M output rows, N = B rows (before GEGLU halving), K = contraction per tap */
-  int32_t block_n;      /* multiple of 32, <= 256 (multiple of 64 when b_major_mn); 320 = the CTA-pair kernel's 256 x 320 tile
+  int32_t block_n;      /* multiple of 32, <= 256 (multiple of 64 when b_major_mn); 320 = 320-column tiles (run as two 160-wide tiles)
                            (two N = 160 MMAs per k-step on one A stage): M >= 512, N % 320 == 0, bf16 TMA-store epilogues only */
   int32_t split_k;      /* >= 1; > 1 requires SVDX_OUT_F32_ATOMIC */
   /* epilogue */
@@ -137,7 +137,7 @@ int svdx_tapgemm(const SvdxTapGemm* desc, void* stream);
 
 /* Second half of a split-K svdx_tapgemm (fp32 partial sums accumulated with SVDX_OUT_F32_ATOMIC into ws): applies the
  * same epilogue  out = scales[0]*(ws + bias + rowbias[m / rowbias_div]) + scales[1]*res1 + scales[2]*res2  -> bf16.
- * Used for the 5x8 / 10x16 latent levels where M gives too few output tiles to fill 148 SMs.
+ * Used for the 5x8 / 10x16 latent levels where M gives too few output tiles to fill the SMs.
  * The workspace is CONSUMED: every element read is reset to zero, so a caller can keep one zeroed workspace per shape
  * and never memset it again. */
 int svdx_splitk_epilogue(float* ws, int64_t ldw, void* out, int64_t ldo, int64_t rows, int32_t cols, const float* bias,

@@ -1,4 +1,4 @@
-"""svd_xtend_b200 — B200-native (sm_100a) implementation of the SVD spatio-temporal UNet hot path
+"""svd_xtend_b200 — H100-native (sm_90a) implementation of the SVD spatio-temporal UNet hot path
 of pixeli99/SVD_Xtend (the forward/backward step train_svd.py loops over)."""
 
 __version__ = "0.1.0"

@@ -2,7 +2,7 @@
 
 The product path has no CPU fallback: if the shared library is missing or fails to load,
 importing any op raises. (It is built in-tree by ``svd_xtend_b200.build`` /
-``__graft_entry__.build`` and travels to the GPU box with the repo snapshot.)
+``__graft_entry__.build`` and lives in the source tree.)
 """
 from __future__ import annotations
 
@@ -11,7 +11,7 @@ import os
 from pathlib import Path
 
 PKG = Path(__file__).resolve().parent
-# SVDX_LIB selects an alternative build of the same library (kernel tuning experiments: svd_xtend_b200.build.build_variant)
+# SVDX_LIB selects an alternative build of the same library
 LIB_PATH = Path(os.environ["SVDX_LIB"]) if os.environ.get("SVDX_LIB") else PKG / "lib" / "libsvdx_b200.so"
 
 SVDX_MAX_TAPS = 27

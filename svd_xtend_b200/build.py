@@ -1,7 +1,7 @@
-"""Build the sm_100a C-ABI library (nvcc, in-tree) — `python -m svd_xtend_b200.build`.
+"""Build the sm_90a (H100) C-ABI library (nvcc, in-tree) — `python -m svd_xtend_b200.build`.
 
-The shared object lands in ``svd_xtend_b200/lib/libsvdx_b200.so`` (git-ignored, shipped to the
-GPU box by gpurun). No torch headers are involved: the boundary is plain C (include/svd_xtend_b200.h).
+The shared object lands in ``svd_xtend_b200/lib/libsvdx_b200.so`` (git-ignored, rebuilt by
+``__graft_entry__.build``). No torch headers are involved: the boundary is plain C (include/svd_xtend_b200.h).
 """
 from __future__ import annotations
 
@@ -19,7 +19,7 @@ LIB = LIBDIR / "libsvdx_b200.so"
 OBJDIR = LIBDIR / "obj"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -45,26 +45,6 @@ def _digest() -> str:
         h.update(f.read_bytes())
     h.update(" ".join(NVCC_FLAGS).encode())
     return h.hexdigest()
-
-
-def build_variant(name: str, defines: list) -> Path:
-    """an alternative build of the library with extra -D flags (kernel tuning experiments, scripts/kbench.py): lands in
-    lib/alt_<name>/libsvdx_b200.so and is selected at run time with SVDX_LIB=<path>"""
-    out_dir = LIBDIR / f"alt_{name}"
-    (out_dir / "obj").mkdir(parents=True, exist_ok=True)
-    nvcc = _nvcc()
-    objs = []
-    for src in _sources():
-        obj = out_dir / "obj" / (src.stem + ".o")
-        r = subprocess.run([nvcc, *NVCC_FLAGS, *[f"-D{d}" for d in defines], "-c", str(src), "-o", str(obj)], capture_output=True, text=True)
-        if r.returncode != 0:
-            raise RuntimeError(f"nvcc failed for {src.name}:\n{r.stdout}\n{r.stderr}")
-        objs.append(obj)
-    lib = out_dir / "libsvdx_b200.so"
-    r = subprocess.run([nvcc, "-shared", "-o", str(lib), *map(str, objs), "-cudart", "static"], capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")
-    return lib
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:

@@ -1,18 +1,20 @@
-// Scaled-dot-product attention (head_dim 64, no mask), forward and backward, on tcgen05.
+// Scaled-dot-product attention (head_dim 64, no mask), forward and backward, on wgmma (sm_90a).
 //
 // Replaces AttnProcessor2_0 -> F.scaled_dot_product_attention [D: diffusers models/attention_processor.py]
 // for BasicTransformerBlock.attn1 (spatial, S = H*W per frame) and
 // TemporalBasicTransformerBlock.attn1 (temporal, S = T per pixel) of the SVD UNet
-// (reached from /root/reference/src/unet_spatio_temporal_condition.py:170-233).
+// (reference: src/unet_spatio_temporal_condition.py:170-233).
 //
 // Layout: q/k/v/o are column slices of token-major [tokens][ld] bf16 matrices (channels-last
-// activations), head h = columns [64h, 64h+64). One 128-row MMA tile holds G interleaved sequences
+// activations), head h = columns [64h, 64h+64). One 128-row tile holds G interleaved sequences
 // x RT = 128/G tokens (tile row r -> sequence r % G, token r / G); spatial attention uses G = 1,
 // temporal attention packs G = 8 neighbouring pixels (T <= 16) so the tensor-core tile is full and
 // the strided token rows are gathered by ONE 4-D TMA box. Cross-sequence score entries are masked.
 //
-//   forward  : S = Q K^T (TMEM) -> online softmax in registers (exp2) -> P (bf16, swizzled smem)
-//              -> O_j = P V (TMEM, V as MN-major B operand) -> fp32 register accumulation.
+// Every kernel: one TMA producer warp and two consumer warpgroups; warpgroup g owns rows [64g, 64g + 64) of the tile.
+// Scores are computed 64 columns at a time into wgmma register fragments, the element-wise work runs on those
+// registers, and the bf16 probabilities / score gradients feed the next wgmma directly as register A operands.
+//   forward  : S = Q K^T -> online softmax (exp2) -> O += P V (V as MN-major B operand)
 //   backward : bwd_dq  (CTA per query tile, loops key tiles):  dQ += dS K
 //              bwd_dkv (CTA per key tile, loops query tiles):  dV += P^T dO, dK += dS^T Q
 //              with P = exp(scale*S - lse) recomputed, dS = P o (dP - delta) * scale.
@@ -22,10 +24,10 @@
 
 namespace svdx {
 
-constexpr int AT_THREADS = 192;    // forward: producer, MMA issuer, 4 softmax warps
-constexpr int BWD_THREADS = 320;   // backward: producer, MMA issuer, 8 element-wise warps
+constexpr int AT_THREADS = 288;   // two consumer warpgroups (warps 0..7) + the TMA producer (warp 8)
+constexpr int AT_PRODUCER = 8;
+constexpr int AT_CONSUMER_WARPS = 8;
 constexpr int TILE_BYTES = 128 * 64 * 2;  // one [128 rows][64 cols] bf16 operand tile, 16 KB
-constexpr int PT_BYTES = 2 * TILE_BYTES;  // one [128][128] bf16 score tile (two 64-column halves)
 constexpr float LOG2E = 1.4426950408889634f;
 
 struct AttnKParams {
@@ -56,43 +58,47 @@ SVDX_DEVINL RowInfo row_info(const AttnKParams& p, int r, int tile, int outer, i
   return ri;
 }
 
-// store 32 consecutive bf16 score values of tile row r, columns [c0, c0+32), into a K-major
-// 128B-swizzled [128][128] tile (two [128][64] halves)
-SVDX_DEVINL void store_score_chunk(uint32_t tile_base, int r, int c0, const float (&f)[32]) {
-  const uint32_t half_base = tile_base + (c0 >> 6) * TILE_BYTES + r * 128;
-  const int chunk0 = (c0 & 63) >> 3;
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const uint32_t addr = half_base + (((chunk0 + k) ^ (r & 7)) << 4);
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(pack_bf16x2(f[8 * k], f[8 * k + 1])),
-                 "r"(pack_bf16x2(f[8 * k + 2], f[8 * k + 3])), "r"(pack_bf16x2(f[8 * k + 4], f[8 * k + 5])),
-                 "r"(pack_bf16x2(f[8 * k + 6], f[8 * k + 7]))
-                 : "memory");
-  }
-}
-
 SVDX_DEVINL float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
 
-SVDX_DEVINL void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
+// [64 rows x 64 cols] (=) A[64 rows x 64] * B[64 rows x 64]^T, both K-major 128B-swizzled tiles of 128-byte rows; committed,
+// not waited for
+SVDX_DEVINL void mma_abt64(float (&d)[32], uint32_t a_rows, uint32_t b_rows) {
+  const uint64_t a = make_smem_desc_sw128(a_rows, 16, 1024), b = make_smem_desc_sw128(b_rows, 16, 1024);
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) wgmma_ss_n64<0, 0>(d, a + 2 * ks, b + 2 * ks, ks > 0 ? 1u : 0u);
+  wgmma_commit();
+}
+// acc[64 x 64] += P[64 x 64] (a D fragment, rounded to bf16) * B[64 rows x 64 cols] (rows = the contraction, MN-major);
+// committed, not waited for
+SVDX_DEVINL void mma_pb64(float (&acc)[32], const float (&p)[32], uint32_t b_rows) {
+  const uint64_t b = make_smem_desc_sw128(b_rows, 8192, 1024);
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks)
+    wgmma_rs_n64_tb(acc, pack_bf16x2(p[8 * ks], p[8 * ks + 1]), pack_bf16x2(p[8 * ks + 2], p[8 * ks + 3]),
+                    pack_bf16x2(p[8 * ks + 4], p[8 * ks + 5]), pack_bf16x2(p[8 * ks + 6], p[8 * ks + 7]), b + (2048 >> 4) * ks, 1u);
+  wgmma_commit();
+}
+// column (inside a 64-column fragment) of D-fragment register i of this lane; its row is row_lo + 8 * frag_hi(i)
+SVDX_DEVINL int frag_col(int i, int lane) { return 8 * (i >> 2) + 2 * (lane & 3) + (i & 1); }
+SVDX_DEVINL int frag_hi(int i) { return (i >> 1) & 1; }
+SVDX_DEVINL float quad_max(float v) { return fmaxf(fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1)), __shfl_xor_sync(0xffffffffu, fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1)), 2)); }
+SVDX_DEVINL float quad_sum(float v) { v += __shfl_xor_sync(0xffffffffu, v, 1); return v + __shfl_xor_sync(0xffffffffu, v, 2); }
 
-// The MMA issuer is ONE thread: rebuilding two 64-bit shared-memory descriptors per tcgen05.mma (a dozen dependent
-// integer ops each) made it the critical path of the backward kernels (ncu: 8 element-wise warps waiting 25 % of the
-// time for S). Descriptors are therefore built once per tile; a k-step / half-tile advance is an add on the
-// 14-bit start-address field (units of 16 bytes, no carry: shared memory is < 256 KB).
-SVDX_DEVINL void mma_kk64_d(uint32_t d_tmem, uint64_t a, uint64_t b, uint32_t idesc, bool acc_first) {
+// the 32 bf16 values of a D fragment of rows row_lo / row_lo + 8, scaled by inv[hi], to 64 consecutive columns of two rows
+SVDX_DEVINL void store_frag_rows(bf16* row_lo, bf16* row_hi, const float (&d)[32], float inv_lo, float inv_hi, int lane) {
 #pragma unroll
-  for (int ks = 0; ks < 4; ++ks) umma_bf16(d_tmem, a + 2 * ks, b + 2 * ks, idesc, (acc_first || ks > 0) ? 1u : 0u);
+  for (int j = 0; j < 8; ++j) {
+    const int c = 8 * j + 2 * (lane & 3);
+    if (row_lo) *reinterpret_cast<uint32_t*>(row_lo + c) = pack_bf16x2(d[4 * j] * inv_lo, d[4 * j + 1] * inv_lo);
+    if (row_hi) *reinterpret_cast<uint32_t*>(row_hi + c) = pack_bf16x2(d[4 * j + 2] * inv_hi, d[4 * j + 3] * inv_hi);
+  }
 }
-// acc[128 x 64] (+)= P[128 x 64 keys] (K-major half score tile) * V[64 keys x 64] (MN-major rows, 2 KB per 16 keys)
-SVDX_DEVINL void mma_pv64_d(uint32_t d_tmem, uint64_t a, uint64_t b, uint32_t idesc, bool acc_first) {
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks) umma_bf16(d_tmem, a + 2 * ks, b + 128 * ks, idesc, (acc_first || ks > 0) ? 1u : 0u);
-}
-constexpr uint64_t HALF_ROWS_DESC = 8192 >> 4;   // 64 rows of 128 bytes further down an operand tile
 
 SVDX_DEVINL void decode_block(const AttnKParams& p, int& tile, int& head, int& outer, int& inner0) {
   tile = blockIdx.x;
@@ -101,442 +107,229 @@ SVDX_DEVINL void decode_block(const AttnKParams& p, int& tile, int& head, int& o
   inner0 = (blockIdx.z % p.inner_groups) * p.G;
 }
 
-// =====================================================================================
-// forward
-// Two CTAs per SM (<= 113 KB shared memory, 256 TMEM columns, <= 168 registers): the softmax of one CTA overlaps
-// the tensor-core work of the other, and every SM sub-partition has two softmax warps to hide MUFU/TMEM latency.
-//   smem : Q | KV ring 2 x (K,V) | P | barriers (in the 1 KB alignment slack)
-//   TMEM : S [128 x 128] | O [128 x 64]. O accumulates in TMEM across key blocks (tcgen05.mma accumulate); the
-//          running maximum is only raised -- and O / l rescaled by the owning warp -- when a row's new maximum
-//          exceeds the one in use by more than 2^8, so the per-block TMEM round trip of O is gone.
-constexpr int FWD_KV_STAGES = 2;   // the MMA issuer keeps one descriptor per stage
-constexpr int FWD_DATA = TILE_BYTES + FWD_KV_STAGES * 2 * TILE_BYTES + PT_BYTES;   // 112 KB
-constexpr int FWD_SMEM = 1024 + FWD_DATA;                                           // 113 KB: two CTAs per SM
-constexpr float FWD_RESCALE_LOG2 = 8.0f;
+// a consumer warp is done with a ring slot
+SVDX_DEVINL void release(uint32_t bar, int lane) {
+  __syncwarp();
+  if (lane == 0) mbar_arrive(bar);
+}
 
-__global__ void __launch_bounds__(AT_THREADS, 2) attn_fwd_kernel(const __grid_constant__ AttnKParams p) {
+// =====================================================================================
+// forward. smem: Q | KV ring 2 x (K,V). O accumulates in registers; the running maximum of a row is updated every key
+// block and O / l rescaled with it (flash-attention 2).
+constexpr int FWD_KV_STAGES = 2;
+constexpr int FWD_SMEM = 1024 + TILE_BYTES + FWD_KV_STAGES * 2 * TILE_BYTES + 256;
+
+__global__ void __launch_bounds__(AT_THREADS, 1) attn_fwd_kernel(const __grid_constant__ AttnKParams p) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sQ = base;
   const uint32_t sKV = sQ + TILE_BYTES;
-  const uint32_t sP = sKV + FWD_KV_STAGES * 2 * TILE_BYTES;
-  // 1024 bytes of the allocation are alignment slack: (base - raw) in front, the rest behind the data
-  const uint32_t sBar = (base - raw >= 256u) ? raw : sP + PT_BYTES;
+  const uint32_t sBar = sKV + FWD_KV_STAGES * 2 * TILE_BYTES;
   const uint32_t b_qfull = sBar;
   const uint32_t b_kvfull = sBar + 8;          // [2]
   const uint32_t b_kvempty = sBar + 8 * 3;     // [2]
-  const uint32_t b_sfull = sBar + 8 * 5;
-  const uint32_t b_sempty = sBar + 8 * 6;
-  const uint32_t b_pfull = sBar + 8 * 7;
-  const uint32_t b_odone = sBar + 8 * 8;
-  const uint32_t tmem_slot = sBar + 8 * 9;
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - raw));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int tile, head, outer, inner0;
   decode_block(p, tile, head, outer, inner0);
   const int nkv = p.tiles;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == AT_PRODUCER && lane == 0) {
     prefetch_tmap(&p.tq); prefetch_tmap(&p.tk); prefetch_tmap(&p.tv);
     mbar_init(b_qfull, 1);
-    for (int i = 0; i < FWD_KV_STAGES; ++i) { mbar_init(b_kvfull + 8 * i, 1); mbar_init(b_kvempty + 8 * i, 1); }
-    mbar_init(b_sfull, 1); mbar_init(b_sempty, 4);     // one arrive per softmax warp (not per thread:
-    mbar_init(b_pfull, 4); mbar_init(b_odone, 1);      // 128 same-address arrives serialise in the SYNCS unit)
+    for (int i = 0; i < FWD_KV_STAGES; ++i) { mbar_init(b_kvfull + 8 * i, 1); mbar_init(b_kvempty + 8 * i, AT_CONSUMER_WARPS); }
     fence_barrier_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, 256); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot_ptr;
-  const uint32_t tS = tmem, tO = tmem + 128;
 
-  if (warp == 0) {
+  if (warp == AT_PRODUCER) {
     if (lane == 0) {
       mbar_expect_tx(b_qfull, TILE_BYTES);
       tma_load_4d(&p.tq, b_qfull, sQ, head * 64, inner0, tile * p.RT, outer);
       for (int j = 0; j < nkv; ++j) {
         const int st = j % FWD_KV_STAGES;
-        mbar_wait(b_kvempty + 8 * st, ((j / FWD_KV_STAGES) & 1) ^ 1);
+        mbar_wait_mma(b_kvempty + 8 * st, ((j / FWD_KV_STAGES) & 1) ^ 1);
         mbar_expect_tx(b_kvfull + 8 * st, 2 * TILE_BYTES);
         tma_load_4d(&p.tk, b_kvfull + 8 * st, sKV + st * 2 * TILE_BYTES, head * 64, inner0, j * p.RT, outer);
         tma_load_4d(&p.tv, b_kvfull + 8 * st, sKV + st * 2 * TILE_BYTES + TILE_BYTES, head * 64, inner0, j * p.RT, outer);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc_bf16(128, 128, 0, 0);
-      const uint32_t idesc_o = make_idesc_bf16(128, 64, 0, 1);
-      const uint64_t dQ = make_smem_desc_sw128(sQ, 16, 1024);
-      const uint64_t dK0 = make_smem_desc_sw128(sKV, 16, 1024), dK1 = make_smem_desc_sw128(sKV + 2 * TILE_BYTES, 16, 1024);
-      const uint64_t dV0 = make_smem_desc_sw128(sKV + TILE_BYTES, 8192, 1024), dV1 = make_smem_desc_sw128(sKV + 3 * TILE_BYTES, 8192, 1024);
-      const uint64_t dP0 = make_smem_desc_sw128(sP, 16, 1024), dP1 = make_smem_desc_sw128(sP + TILE_BYTES, 16, 1024);
-      mbar_wait(b_qfull, 0);
-      for (int j = 0; j <= nkv; ++j) {
-        if (j < nkv) {
-          const int st = j % FWD_KV_STAGES;
-          mbar_wait(b_kvfull + 8 * st, (j / FWD_KV_STAGES) & 1);
-          mbar_wait(b_sempty, (j & 1) ^ 1);      // the softmax warps hold S_{j-1} in registers
-          tc_fence_after();
-          mma_kk64_d(tS, dQ, st ? dK1 : dK0, idesc_s, false);
-          umma_commit(b_sfull);
-        }
-        if (j >= 1) {
-          const int k = j - 1;
-          const int st = k % FWD_KV_STAGES;
-          mbar_wait(b_pfull, k & 1);
-          tc_fence_after();
-          const uint64_t dV = st ? dV1 : dV0;
-          mma_pv64_d(tO, dP0, dV, idesc_o, k > 0);
-          mma_pv64_d(tO, dP1, dV + HALF_ROWS_DESC, idesc_o, true);
-          umma_commit(b_odone);                  // P is free again, O holds blocks 0..k
-          umma_commit(b_kvempty + 8 * st);
-        }
-      }
-    }
-  } else {
-    // ---------------- softmax threads: one thread per tile row
-    const int q4 = warp & 3;
-    const int r = q4 * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(q4 * 32) << 16;
-    const RowInfo ri = row_info(p, r, tile, outer, inner0);
-    const float sc = p.scale * LOG2E;
-    float m_used = 0.f, l_run = 0.f;   // exponentials are taken relative to m_used
-
-    for (int j = 0; j < nkv; ++j) {
-      mbar_wait(b_sfull, j & 1);
-      tc_fence_after();
-      const uint32_t ts = tS + lane_off;
-      const int kvalid = p.S - j * p.RT;                 // valid key tokens in this block
-      const bool nomask = (p.G == 1) && (kvalid >= 128);  // warp-uniform fast path: nothing to mask
-      // single TMEM pass: the 128 scores of this row stay in registers
-      uint32_t sv[4][32];
-      tmem_ld32(ts, sv[0]);
-      tmem_ld32(ts + 32, sv[1]);
-      tmem_ld32(ts + 64, sv[2]);
-      tmem_ld32(ts + 96, sv[3]);
-      tc_wait_ld();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(b_sempty);   // S can be overwritten by the next QK^T
-      float bmax;
-      if (nomask) {
-        float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;   // 4 independent chains
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-#pragma unroll
-          for (int i = 0; i < 32; i += 4) {
-            m0 = fmaxf(m0, __uint_as_float(sv[q][i]));
-            m1 = fmaxf(m1, __uint_as_float(sv[q][i + 1]));
-            m2 = fmaxf(m2, __uint_as_float(sv[q][i + 2]));
-            m3 = fmaxf(m3, __uint_as_float(sv[q][i + 3]));
-          }
-        }
-        bmax = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-      } else {
-        bmax = -INFINITY;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const int c = q * 32 + i;
-            const bool ok = (((c & p.gmask) == ri.g)) && ((c >> p.gshift) < kvalid);
-            if (ok) bmax = fmaxf(bmax, __uint_as_float(sv[q][i]));
-          }
-        }
-      }
-      if (bmax == -INFINITY) bmax = 0.f;   // a row with no visible key in this block (padding rows of a packed tile)
-      if (j == 0) {
-        m_used = bmax;                     // PV_0 overwrites O: nothing to rescale
-      } else {
-        const bool grow = (bmax - m_used) * sc > FWD_RESCALE_LOG2;
-        mbar_wait(b_odone, (j - 1) & 1);   // PV_{j-1} retired: P is free and O is quiescent until we publish P_j
-        if (__any_sync(0xffffffffu, grow)) {
-          const float alpha = grow ? fast_exp2((m_used - bmax) * sc) : 1.f;
-          if (grow) m_used = bmax;
-          l_run *= alpha;
-          tc_fence_after();
-#pragma unroll 1
-          for (int h = 0; h < 64; h += 32) {   // 32 columns at a time: the 128 scores stay live in registers
-            uint32_t ov[32];
-            tmem_ld32(tO + h + lane_off, ov);
-            tc_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) ov[i] = __float_as_uint(__uint_as_float(ov[i]) * alpha);
-            tmem_st32(tO + h + lane_off, ov);
-          }
-          tc_wait_st();
-          tc_fence_before();
-        }
-      }
-      const float msc = m_used * sc;
-      // probabilities: the row sum uses the fp32 values (the bf16 rounding of P averages out, as in flash-attention)
-      float r0 = 0.f, r1 = 0.f, r2 = 0.f, r3 = 0.f;
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        float f[32];
-        if (nomask) {
-#pragma unroll
-          for (int i = 0; i < 32; i += 4) {
-            f[i] = fast_exp2(fmaf(__uint_as_float(sv[q][i]), sc, -msc));
-            f[i + 1] = fast_exp2(fmaf(__uint_as_float(sv[q][i + 1]), sc, -msc));
-            f[i + 2] = fast_exp2(fmaf(__uint_as_float(sv[q][i + 2]), sc, -msc));
-            f[i + 3] = fast_exp2(fmaf(__uint_as_float(sv[q][i + 3]), sc, -msc));
-            r0 += f[i]; r1 += f[i + 1]; r2 += f[i + 2]; r3 += f[i + 3];
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const int c = q * 32 + i;
-            const bool ok = (((c & p.gmask) == ri.g)) && ((c >> p.gshift) < kvalid);
-            f[i] = ok ? fast_exp2(fmaf(__uint_as_float(sv[q][i]), sc, -msc)) : 0.f;
-            r0 += f[i];
-          }
-        }
-        store_score_chunk(sP, r, q * 32, f);
-      }
-      l_run += (r0 + r1) + (r2 + r3);
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(b_pfull);
-    }
-    // epilogue: O / l
-    mbar_wait(b_odone, (nkv - 1) & 1);
-    tc_fence_after();
-    uint32_t o0[32], o1[32];
-    tmem_ld32(tO + lane_off, o0);
-    tmem_ld32(tO + 32 + lane_off, o1);
-    tc_wait_ld();
-    if (ri.valid) {
-      const float inv = 1.f / l_run;
-      bf16* orow = p.o + ri.token * p.ldo + head * 64;
-#pragma unroll
-      for (int i = 0; i < 32; i += 8) {
-        uint4 u;
-        u.x = pack_bf16x2(__uint_as_float(o0[i]) * inv, __uint_as_float(o0[i + 1]) * inv);
-        u.y = pack_bf16x2(__uint_as_float(o0[i + 2]) * inv, __uint_as_float(o0[i + 3]) * inv);
-        u.z = pack_bf16x2(__uint_as_float(o0[i + 4]) * inv, __uint_as_float(o0[i + 5]) * inv);
-        u.w = pack_bf16x2(__uint_as_float(o0[i + 6]) * inv, __uint_as_float(o0[i + 7]) * inv);
-        *reinterpret_cast<uint4*>(orow + i) = u;
-      }
-#pragma unroll
-      for (int i = 0; i < 32; i += 8) {
-        uint4 u;
-        u.x = pack_bf16x2(__uint_as_float(o1[i]) * inv, __uint_as_float(o1[i + 1]) * inv);
-        u.y = pack_bf16x2(__uint_as_float(o1[i + 2]) * inv, __uint_as_float(o1[i + 3]) * inv);
-        u.z = pack_bf16x2(__uint_as_float(o1[i + 4]) * inv, __uint_as_float(o1[i + 5]) * inv);
-        u.w = pack_bf16x2(__uint_as_float(o1[i + 6]) * inv, __uint_as_float(o1[i + 7]) * inv);
-        *reinterpret_cast<uint4*>(orow + 32 + i) = u;
-      }
-      if (p.lse) p.lse[ri.token * p.heads + head] = m_used * p.scale + __logf(l_run);
-    }
+    return;
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem, 256); }
+  const int wg = warp >> 2;
+  const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows: r_lo, r_lo + 8
+  const RowInfo ri[2] = {row_info(p, r_lo, tile, outer, inner0), row_info(p, r_lo + 8, tile, outer, inner0)};
+  const float sc = p.scale * LOG2E;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // l_run: this lane's partial row sums
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  mbar_wait_mma(b_qfull, 0);
+  for (int j = 0; j < nkv; ++j) {
+    const int st = j % FWD_KV_STAGES;
+    const uint32_t sK = sKV + st * 2 * TILE_BYTES, sV = sK + TILE_BYTES;
+    mbar_wait_mma(b_kvfull + 8 * st, (j / FWD_KV_STAGES) & 1);
+    float s0[32], s1[32];
+    mma_abt64(s0, sQ + wg * 8192, sK);
+    mma_abt64(s1, sQ + wg * 8192, sK + 8192);
+    wgmma_wait<0>();
+    reg_fence(s0); reg_fence(s1);
+    const int kvalid = p.S - j * p.RT;                 // valid key tokens in this block
+    if (!(p.G == 1 && kvalid >= 128)) {                // warp-uniform: something to mask
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int c0 = frag_col(i, lane), c1 = 64 + c0;
+        const RowInfo& r = ri[frag_hi(i)];
+        if (!(((c0 & p.gmask) == r.g) && ((c0 >> p.gshift) < kvalid))) s0[i] = -INFINITY;
+        if (!(((c1 & p.gmask) == r.g) && ((c1 >> p.gshift) < kvalid))) s1[i] = -INFINITY;
+      }
+    }
+    float bm[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < 32; ++i) bm[frag_hi(i)] = fmaxf(bm[frag_hi(i)], fmaxf(s0[i], s1[i]));
+    float msc[2], alpha[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float m_new = fmaxf(m_run[h], quad_max(bm[h]));
+      const float m_use = m_new == -INFINITY ? 0.f : m_new;   // a row with no visible key so far (padding rows)
+      alpha[h] = fast_exp2((m_run[h] - m_use) * sc);
+      m_run[h] = m_new;
+      msc[h] = m_use * sc;
+      l_run[h] *= alpha[h];
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const int h = frag_hi(i);
+      o[i] *= alpha[h];
+      // probabilities: the row sum uses the fp32 values (the bf16 rounding of P averages out, as in flash-attention)
+      s0[i] = fast_exp2(fmaf(s0[i], sc, -msc[h]));
+      s1[i] = fast_exp2(fmaf(s1[i], sc, -msc[h]));
+      l_run[h] += s0[i] + s1[i];
+    }
+    mma_pb64(o, s0, sV);
+    mma_pb64(o, s1, sV + 8192);
+    wgmma_wait<0>();
+    reg_fence(o);
+    release(b_kvempty + 8 * st, lane);
+  }
+  // epilogue: O / l
+  bf16* rows[2];
+  float inv[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const float l = quad_sum(l_run[h]);
+    const float m_use = m_run[h] == -INFINITY ? 0.f : m_run[h];
+    inv[h] = 1.f / l;
+    rows[h] = ri[h].valid ? p.o + ri[h].token * p.ldo + head * 64 : nullptr;
+    if (ri[h].valid && p.lse && (lane & 3) == 0) p.lse[ri[h].token * p.heads + head] = m_use * p.scale + __logf(l);
+  }
+  store_frag_rows(rows[0], rows[1], o, inv[0], inv[1], lane);
 }
 
 // =====================================================================================
-// backward, dQ:  CTA owns a query tile, loops key tiles.
-// smem: Q | dO | KV ring 2 x (K,V) | dS | barriers.  TMEM: S [0,128) dP [128,256) dQ [256,320)
-// Each 128-key block is processed as two 64-key halves with their own barriers: while the element-wise warps drain
-// S/dP of one half from TMEM (the scarce resource: 128 KB per block at ~64 B/clk), the tensor core already computes
-// the other half, and dQ += dS_h K_h trails by one half.
+// backward, dQ:  CTA owns a query tile, loops key tiles (two 64-key halves each).
+// smem: Q | dO | KV ring 2 x (K,V).
 constexpr int BWD_STAGES = 2;
-constexpr int BDQ_SMEM = 1024 + 2 * TILE_BYTES + BWD_STAGES * 2 * TILE_BYTES + PT_BYTES + 256;
+constexpr int BDQ_SMEM = 1024 + 2 * TILE_BYTES + BWD_STAGES * 2 * TILE_BYTES + 256;
 
-// 8 element-wise warps: warp (w & 3) owns a TMEM lane quarter, ((w - 2) >> 2) picks the 64-column half of the score
-// tile it processes -- two warps per SM sub-partition hide the MUFU / TMEM / shared-memory latencies of each other.
-__global__ void __launch_bounds__(BWD_THREADS, 1) attn_bwd_dq_kernel(const __grid_constant__ AttnKParams p) {
+__global__ void __launch_bounds__(AT_THREADS, 1) attn_bwd_dq_kernel(const __grid_constant__ AttnKParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sQ = base, sDO = sQ + TILE_BYTES;
   const uint32_t sKV = sDO + TILE_BYTES;
-  const uint32_t sDS = sKV + BWD_STAGES * 2 * TILE_BYTES;
-  const uint32_t sBar = sDS + PT_BYTES;
+  const uint32_t sBar = sKV + BWD_STAGES * 2 * TILE_BYTES;
   const uint32_t b_qfull = sBar;
   const uint32_t b_kvfull = sBar + 8;        // [2]
   const uint32_t b_kvempty = sBar + 8 * 3;   // [2]
-  const uint32_t b_sfull = sBar + 8 * 5;     // [2] one per 64-key half
-  const uint32_t b_sempty = sBar + 8 * 7;    // [2]
-  const uint32_t b_dsfull = sBar + 8 * 9;    // [2]
-  const uint32_t b_dsempty = sBar + 8 * 11;  // [2]
-  const uint32_t b_done = sBar + 8 * 13;
-  const uint32_t tmem_slot = sBar + 8 * 14;
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int tile, head, outer, inner0;
   decode_block(p, tile, head, outer, inner0);
   const int nkv = p.tiles;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == AT_PRODUCER && lane == 0) {
     prefetch_tmap(&p.tq); prefetch_tmap(&p.tk); prefetch_tmap(&p.tv); prefetch_tmap(&p.tdo);
     mbar_init(b_qfull, 1);
-    for (int i = 0; i < BWD_STAGES; ++i) { mbar_init(b_kvfull + 8 * i, 1); mbar_init(b_kvempty + 8 * i, 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(b_sfull + 8 * i, 1); mbar_init(b_sempty + 8 * i, 8);     // one arrive per element-wise warp
-      mbar_init(b_dsfull + 8 * i, 8); mbar_init(b_dsempty + 8 * i, 1);
-    }
-    mbar_init(b_done, 1);
+    for (int i = 0; i < BWD_STAGES; ++i) { mbar_init(b_kvfull + 8 * i, 1); mbar_init(b_kvempty + 8 * i, AT_CONSUMER_WARPS); }
     fence_barrier_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot_ptr;
-  const uint32_t tS = tmem, tDP = tmem + 128, tDQ = tmem + 256;
 
-  if (warp == 0) {
+  if (warp == AT_PRODUCER) {
     if (lane == 0) {
       mbar_expect_tx(b_qfull, 2 * TILE_BYTES);
       tma_load_4d(&p.tq, b_qfull, sQ, head * 64, inner0, tile * p.RT, outer);
       tma_load_4d(&p.tdo, b_qfull, sDO, head * 64, inner0, tile * p.RT, outer);
       for (int j = 0; j < nkv; ++j) {
         const int st = j % BWD_STAGES;
-        mbar_wait(b_kvempty + 8 * st, ((j / BWD_STAGES) & 1) ^ 1);
+        mbar_wait_mma(b_kvempty + 8 * st, ((j / BWD_STAGES) & 1) ^ 1);
         mbar_expect_tx(b_kvfull + 8 * st, 2 * TILE_BYTES);
         tma_load_4d(&p.tk, b_kvfull + 8 * st, sKV + st * 2 * TILE_BYTES, head * 64, inner0, j * p.RT, outer);
         tma_load_4d(&p.tv, b_kvfull + 8 * st, sKV + st * 2 * TILE_BYTES + TILE_BYTES, head * 64, inner0, j * p.RT, outer);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc_bf16(128, 64, 0, 0);   // one 64-key half of S / dP
-      const uint32_t idesc_o = make_idesc_bf16(128, 64, 0, 1);
-      // dQ += dS_h K_h for sub-block t = 2 * block + half (trails the score MMAs by one sub-block)
-      const uint64_t dQa = make_smem_desc_sw128(sQ, 16, 1024), dDOa = make_smem_desc_sw128(sDO, 16, 1024);
-      const uint64_t dKk0 = make_smem_desc_sw128(sKV, 16, 1024), dKk1 = make_smem_desc_sw128(sKV + 2 * TILE_BYTES, 16, 1024);
-      const uint64_t dVk0 = make_smem_desc_sw128(sKV + TILE_BYTES, 16, 1024), dVk1 = make_smem_desc_sw128(sKV + 3 * TILE_BYTES, 16, 1024);
-      const uint64_t dKm0 = make_smem_desc_sw128(sKV, 8192, 1024), dKm1 = make_smem_desc_sw128(sKV + 2 * TILE_BYTES, 8192, 1024);
-      const uint64_t dDS0 = make_smem_desc_sw128(sDS, 16, 1024), dDS1 = make_smem_desc_sw128(sDS + TILE_BYTES, 16, 1024);
-      auto dq_step = [&](int t) {
-        const int jj = t >> 1, hh = t & 1;
-        mbar_wait(b_dsfull + 8 * hh, jj & 1);
-        tc_fence_after();
-        mma_pv64_d(tDQ, hh ? dDS1 : dDS0, ((jj % BWD_STAGES) ? dKm1 : dKm0) + hh * HALF_ROWS_DESC, idesc_o, t > 0);
-        umma_commit(b_dsempty + 8 * hh);
-        if (hh == 1) umma_commit(b_kvempty + 8 * (jj % BWD_STAGES));
-      };
-      mbar_wait(b_qfull, 0);
-      int t = 0;
-      for (int j = 0; j < nkv; ++j) {
-        const int st = j % BWD_STAGES;
-        mbar_wait(b_kvfull + 8 * st, (j / BWD_STAGES) & 1);
-        for (int h = 0; h < 2; ++h, ++t) {
-          mbar_wait(b_sempty + 8 * h, (j & 1) ^ 1);
-          tc_fence_after();
-          mma_kk64_d(tS + h * 64, dQa, (st ? dKk1 : dKk0) + h * HALF_ROWS_DESC, idesc_s, false);     // S_h  = Q K_h^T
-          mma_kk64_d(tDP + h * 64, dDOa, (st ? dVk1 : dVk0) + h * HALF_ROWS_DESC, idesc_s, false);   // dP_h = dO V_h^T
-          umma_commit(b_sfull + 8 * h);
-          if (t >= 1) dq_step(t - 1);
-        }
-      }
-      dq_step(t - 1);
-      umma_commit(b_done);
-    }
-  } else {
-    const int q4 = warp & 3;
-    const int ch = (warp - 2) >> 2;        // column half of the score tile
-    const int r = q4 * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(q4 * 32) << 16;
-    const RowInfo ri = row_info(p, r, tile, outer, inner0);
-    const float sc = p.scale * LOG2E;
-    const float lse2 = ri.valid ? p.lse[ri.token * p.heads + head] * LOG2E : 0.f;
-    const float dlt = ri.valid ? p.delta[ri.token * p.heads + head] : 0.f;
-    for (int j = 0; j < nkv; ++j) {
-      const int kvalid = p.S - j * p.RT;
-      const bool nomask = (p.G == 1) && (kvalid >= 128);
-#pragma unroll 1
-      for (int h = 0; h < 2; ++h) {
-        mbar_wait(b_sfull + 8 * h, j & 1);
-        tc_fence_after();
-        mbar_wait(b_dsempty + 8 * h, (j & 1) ^ 1);
-        const int c0 = h * 64 + ch * 32;
-        uint32_t vs[32], vd[32];
-        tmem_ld32(tS + lane_off + c0, vs);
-        tmem_ld32(tDP + lane_off + c0, vd);
-        tc_wait_ld();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(b_sempty + 8 * h);     // this half of S / dP may be overwritten by the next block
-        float f[32];
-        if (nomask && ri.valid) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float pr = fast_exp2(fmaf(__uint_as_float(vs[i]), sc, -lse2)) * p.scale;
-            f[i] = pr * (__uint_as_float(vd[i]) - dlt);
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const int c = c0 + i;
-            const bool ok = ri.valid && (nomask || ((((c & p.gmask) == ri.g)) && ((c >> p.gshift) < kvalid)));
-            const float pr = ok ? fast_exp2(fmaf(__uint_as_float(vs[i]), sc, -lse2)) * p.scale : 0.f;
-            f[i] = pr * (__uint_as_float(vd[i]) - dlt);
-          }
-        }
-        store_score_chunk(sDS, r, c0, f);
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(b_dsfull + 8 * h);
-      }
-    }
-    mbar_wait(b_done, 0);
-    tc_fence_after();
-    uint32_t v0[32];
-    tmem_ld32(tDQ + lane_off + ch * 32, v0);   // each warp of the pair writes 32 of the 64 head columns
-    tc_wait_ld();
-    if (ri.valid) {
-      bf16* orow = p.dq + ri.token * p.lddq + head * 64 + ch * 32;
-#pragma unroll
-      for (int i = 0; i < 32; i += 8) {
-        uint4 u;
-        u.x = pack_bf16x2(__uint_as_float(v0[i]), __uint_as_float(v0[i + 1]));
-        u.y = pack_bf16x2(__uint_as_float(v0[i + 2]), __uint_as_float(v0[i + 3]));
-        u.z = pack_bf16x2(__uint_as_float(v0[i + 4]), __uint_as_float(v0[i + 5]));
-        u.w = pack_bf16x2(__uint_as_float(v0[i + 6]), __uint_as_float(v0[i + 7]));
-        *reinterpret_cast<uint4*>(orow + i) = u;
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem, 512); }
+  const int wg = warp >> 2;
+  const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const RowInfo ri[2] = {row_info(p, r_lo, tile, outer, inner0), row_info(p, r_lo + 8, tile, outer, inner0)};
+  const float sc = p.scale * LOG2E;
+  float lse2[2], dlt[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    lse2[h] = ri[h].valid ? p.lse[ri[h].token * p.heads + head] * LOG2E : 0.f;
+    dlt[h] = ri[h].valid ? p.delta[ri[h].token * p.heads + head] : 0.f;
+  }
+  float dq[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) dq[i] = 0.f;
+  mbar_wait_mma(b_qfull, 0);
+  for (int j = 0; j < nkv; ++j) {
+    const int st = j % BWD_STAGES;
+    const uint32_t sK = sKV + st * 2 * TILE_BYTES, sV = sK + TILE_BYTES;
+    mbar_wait_mma(b_kvfull + 8 * st, (j / BWD_STAGES) & 1);
+    const int kvalid = p.S - j * p.RT;
+    const bool nomask = (p.G == 1) && (kvalid >= 128);
+#pragma unroll 1
+    for (int kh = 0; kh < 2; ++kh) {
+      float s[32], dp[32];
+      mma_abt64(s, sQ + wg * 8192, sK + kh * 8192);     // S_h  = Q K_h^T
+      mma_abt64(dp, sDO + wg * 8192, sV + kh * 8192);   // dP_h = dO V_h^T
+      wgmma_wait<0>();
+      reg_fence(s); reg_fence(dp);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int c = kh * 64 + frag_col(i, lane), h = frag_hi(i);
+        const bool ok = ri[h].valid && (nomask || (((c & p.gmask) == ri[h].g) && ((c >> p.gshift) < kvalid)));
+        const float pr = ok ? fast_exp2(fmaf(s[i], sc, -lse2[h])) * p.scale : 0.f;
+        s[i] = pr * (dp[i] - dlt[h]);
+      }
+      mma_pb64(dq, s, sK + kh * 8192);                  // dQ += dS_h K_h
+      wgmma_wait<0>();
+      reg_fence(dq);
+    }
+    release(b_kvempty + 8 * st, lane);
+  }
+  store_frag_rows(ri[0].valid ? p.dq + ri[0].token * p.lddq + head * 64 : nullptr,
+                  ri[1].valid ? p.dq + ri[1].token * p.lddq + head * 64 : nullptr, dq, 1.f, 1.f, lane);
 }
 
 // =====================================================================================
-// backward, dK/dV: CTA owns a key tile, loops query tiles. Scores are computed transposed
-// (S^T = K Q^T, dP^T = V dO^T) so that P^T / dS^T land row-major-in-keys = K-major A operands.
-// smem: K | V | Q/dO ring 2 | P^T | dS^T | lse/delta | barriers
-// TMEM: S^T [0,128) dP^T [128,256) dV [256,320) dK [320,384)
-// Like the dQ kernel, every 128-query tile is processed as two 64-query halves with their own barriers, so that the
-// TMEM drain of one half overlaps the tensor-core work of the other; dV/dK accumulation trails by one half.
-constexpr int BKV_SMEM = 1024 + 2 * TILE_BYTES + BWD_STAGES * 2 * TILE_BYTES + 2 * PT_BYTES + 1024 + 256;
+// backward, dK/dV: CTA owns a key tile, loops query tiles (two 64-query halves each). Scores are computed transposed
+// (S^T = K Q^T, dP^T = V dO^T) so that P^T / dS^T are the A operands of dV += P^T dO and dK += dS^T Q.
+// smem: K | V | Q/dO ring 2 | lse/delta of the current query tile
+constexpr int BKV_SMEM = 1024 + 2 * TILE_BYTES + BWD_STAGES * 2 * TILE_BYTES + 1024 + 256;
 
-__global__ void __launch_bounds__(BWD_THREADS, 1) attn_bwd_dkv_kernel(const __grid_constant__ AttnKParams p) {
+__global__ void __launch_bounds__(AT_THREADS, 1) attn_bwd_dkv_kernel(const __grid_constant__ AttnKParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sK = base, sV = sK + TILE_BYTES;
   const uint32_t sQD = sV + TILE_BYTES;
-  const uint32_t sPT = sQD + BWD_STAGES * 2 * TILE_BYTES;
-  const uint32_t sDST = sPT + PT_BYTES;
-  const uint32_t sVec = sDST + PT_BYTES;  // float lse2[128], delta[128]
+  const uint32_t sVec = sQD + BWD_STAGES * 2 * TILE_BYTES;  // float lse2[128], delta[128]
   const uint32_t sBar = sVec + 1024;
   const uint32_t b_kvfull = sBar;
   const uint32_t b_qfull = sBar + 8;        // [2]
   const uint32_t b_qempty = sBar + 8 * 3;   // [2]
-  const uint32_t b_sfull = sBar + 8 * 5;     // [2] one per 64-query half
-  const uint32_t b_sempty = sBar + 8 * 7;    // [2]
-  const uint32_t b_pfull = sBar + 8 * 9;     // [2]
-  const uint32_t b_pempty = sBar + 8 * 11;   // [2]
-  const uint32_t b_done = sBar + 8 * 13;
-  const uint32_t tmem_slot = sBar + 8 * 14;
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
   float* vec = reinterpret_cast<float*>(smem_raw + (sVec - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -544,167 +337,83 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) attn_bwd_dkv_kernel(const __gr
   decode_block(p, tile, head, outer, inner0);
   const int nq = p.tiles;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == AT_PRODUCER && lane == 0) {
     prefetch_tmap(&p.tq); prefetch_tmap(&p.tk); prefetch_tmap(&p.tv); prefetch_tmap(&p.tdo);
     mbar_init(b_kvfull, 1);
-    for (int i = 0; i < BWD_STAGES; ++i) { mbar_init(b_qfull + 8 * i, 1); mbar_init(b_qempty + 8 * i, 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(b_sfull + 8 * i, 1); mbar_init(b_sempty + 8 * i, 8);     // one arrive per element-wise warp
-      mbar_init(b_pfull + 8 * i, 8); mbar_init(b_pempty + 8 * i, 1);
-    }
-    mbar_init(b_done, 1);
+    for (int i = 0; i < BWD_STAGES; ++i) { mbar_init(b_qfull + 8 * i, 1); mbar_init(b_qempty + 8 * i, AT_CONSUMER_WARPS); }
     fence_barrier_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot_ptr;
-  const uint32_t tST = tmem, tDPT = tmem + 128, tDV = tmem + 256, tDK = tmem + 320;
 
-  if (warp == 0) {
+  if (warp == AT_PRODUCER) {
     if (lane == 0) {
       mbar_expect_tx(b_kvfull, 2 * TILE_BYTES);
       tma_load_4d(&p.tk, b_kvfull, sK, head * 64, inner0, tile * p.RT, outer);
       tma_load_4d(&p.tv, b_kvfull, sV, head * 64, inner0, tile * p.RT, outer);
       for (int i = 0; i < nq; ++i) {
         const int st = i % BWD_STAGES;
-        mbar_wait(b_qempty + 8 * st, ((i / BWD_STAGES) & 1) ^ 1);
+        mbar_wait_mma(b_qempty + 8 * st, ((i / BWD_STAGES) & 1) ^ 1);
         mbar_expect_tx(b_qfull + 8 * st, 2 * TILE_BYTES);
         tma_load_4d(&p.tq, b_qfull + 8 * st, sQD + st * 2 * TILE_BYTES, head * 64, inner0, i * p.RT, outer);
         tma_load_4d(&p.tdo, b_qfull + 8 * st, sQD + st * 2 * TILE_BYTES + TILE_BYTES, head * 64, inner0, i * p.RT, outer);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc_bf16(128, 64, 0, 0);   // one 64-query half of S^T / dP^T
-      const uint32_t idesc_o = make_idesc_bf16(128, 64, 0, 1);
-      // dV += P^T_h dO_h, dK += dS^T_h Q_h for sub-block t = 2 * tile + half (trails the score MMAs by one sub-block)
-      const uint64_t dKa = make_smem_desc_sw128(sK, 16, 1024), dVa = make_smem_desc_sw128(sV, 16, 1024);
-      const uint64_t dQk0 = make_smem_desc_sw128(sQD, 16, 1024), dQk1 = make_smem_desc_sw128(sQD + 2 * TILE_BYTES, 16, 1024);
-      const uint64_t dOk0 = make_smem_desc_sw128(sQD + TILE_BYTES, 16, 1024), dOk1 = make_smem_desc_sw128(sQD + 3 * TILE_BYTES, 16, 1024);
-      const uint64_t dQm0 = make_smem_desc_sw128(sQD, 8192, 1024), dQm1 = make_smem_desc_sw128(sQD + 2 * TILE_BYTES, 8192, 1024);
-      const uint64_t dOm0 = make_smem_desc_sw128(sQD + TILE_BYTES, 8192, 1024), dOm1 = make_smem_desc_sw128(sQD + 3 * TILE_BYTES, 8192, 1024);
-      const uint64_t dPT0 = make_smem_desc_sw128(sPT, 16, 1024), dPT1 = make_smem_desc_sw128(sPT + TILE_BYTES, 16, 1024);
-      const uint64_t dST0 = make_smem_desc_sw128(sDST, 16, 1024), dST1 = make_smem_desc_sw128(sDST + TILE_BYTES, 16, 1024);
-      auto acc_step = [&](int t) {
-        const int ii = t >> 1, hh = t & 1;
-        const bool s1 = (ii % BWD_STAGES) != 0;
-        mbar_wait(b_pfull + 8 * hh, ii & 1);
-        tc_fence_after();
-        mma_pv64_d(tDV, hh ? dPT1 : dPT0, (s1 ? dOm1 : dOm0) + hh * HALF_ROWS_DESC, idesc_o, t > 0);   // dV += P^T_h dO_h
-        mma_pv64_d(tDK, hh ? dST1 : dST0, (s1 ? dQm1 : dQm0) + hh * HALF_ROWS_DESC, idesc_o, t > 0);   // dK += dS^T_h Q_h
-        umma_commit(b_pempty + 8 * hh);
-        if (hh == 1) umma_commit(b_qempty + 8 * (ii % BWD_STAGES));
-      };
-      mbar_wait(b_kvfull, 0);
-      int t = 0;
-      for (int i = 0; i < nq; ++i) {
-        const int st = i % BWD_STAGES;
-        mbar_wait(b_qfull + 8 * st, (i / BWD_STAGES) & 1);
-        for (int h = 0; h < 2; ++h, ++t) {
-          mbar_wait(b_sempty + 8 * h, (i & 1) ^ 1);
-          tc_fence_after();
-          mma_kk64_d(tST + h * 64, dKa, (st ? dQk1 : dQk0) + h * HALF_ROWS_DESC, idesc_s, false);     // S^T_h  = K Q_h^T
-          mma_kk64_d(tDPT + h * 64, dVa, (st ? dOk1 : dOk0) + h * HALF_ROWS_DESC, idesc_s, false);   // dP^T_h = V dO_h^T
-          umma_commit(b_sfull + 8 * h);
-          if (t >= 1) acc_step(t - 1);
-        }
-      }
-      acc_step(t - 1);
-      umma_commit(b_done);
-    }
-  } else {
-    const int q4 = warp & 3;
-    const int ch = (warp - 2) >> 2;        // query-column half of the transposed score tile
-    const int r = q4 * 32 + lane;          // key row of this thread
-    const uint32_t lane_off = (uint32_t)(q4 * 32) << 16;
-    const RowInfo ki = row_info(p, r, tile, outer, inner0);
-    const float sc = p.scale * LOG2E;
-    // lse (warps with ch == 0) / delta (ch == 1) of query row r of a tile; +inf lse -> p = 0 for padding queries
-    auto load_stat = [&](int i) -> float {
-      const RowInfo qi = row_info(p, r, i, outer, inner0);
-      if (ch == 0) return qi.valid ? p.lse[qi.token * p.heads + head] * LOG2E : INFINITY;
-      return qi.valid ? p.delta[qi.token * p.heads + head] : 0.f;
-    };
-    float stat = load_stat(0);
-    for (int i = 0; i < nq; ++i) {
-      // stage lse/delta of the 128 queries of tile i (column vectors of the transposed scores); the values of the
-      // next tile are requested right away so that their latency hides behind this tile's work
-      named_bar_sync(1, 256);  // previous iteration finished reading vec[]
-      vec[ch * 128 + r] = stat;
-      named_bar_sync(1, 256);
-      if (i + 1 < nq) stat = load_stat(i + 1);
-#pragma unroll 1
-      for (int h = 0; h < 2; ++h) {
-        mbar_wait(b_sfull + 8 * h, i & 1);
-        tc_fence_after();
-        mbar_wait(b_pempty + 8 * h, (i & 1) ^ 1);
-        const int c0 = h * 64 + ch * 32;
-        uint32_t vs[32], vd[32];
-        tmem_ld32(tST + lane_off + c0, vs);
-        tmem_ld32(tDPT + lane_off + c0, vd);
-        tc_wait_ld();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(b_sempty + 8 * h);
-        float fp[32], fd[32];
-        if (p.G == 1 && ki.valid) {
-          // unmasked fast path (spatial attention): invalid query columns carry lse = +inf -> p = 0
-#pragma unroll
-          for (int k = 0; k < 32; ++k) {
-            const float pr = fast_exp2(fmaf(__uint_as_float(vs[k]), sc, -vec[c0 + k]));
-            fp[k] = pr;
-            fd[k] = (pr * p.scale) * (__uint_as_float(vd[k]) - vec[128 + c0 + k]);
-          }
-        } else {
-#pragma unroll
-          for (int k = 0; k < 32; ++k) {
-            const int c = c0 + k;  // query column
-            const bool ok = ki.valid && ((c & p.gmask) == ki.g);
-            const float pr = ok ? fast_exp2(fmaf(__uint_as_float(vs[k]), sc, -vec[c])) : 0.f;
-            fp[k] = pr;
-            fd[k] = (pr * p.scale) * (__uint_as_float(vd[k]) - vec[128 + c]);
-          }
-        }
-        store_score_chunk(sPT, r, c0, fp);
-        store_score_chunk(sDST, r, c0, fd);
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(b_pfull + 8 * h);
-      }
-    }
-    mbar_wait(b_done, 0);
-    tc_fence_after();
-    {
-      // warp pair: ch 0 writes dV, ch 1 writes dK
-      uint32_t v0[32], v1[32];
-      const uint32_t t = ch == 0 ? tDV : tDK;
-      tmem_ld32(t + lane_off, v0);
-      tmem_ld32(t + lane_off + 32, v1);
-      tc_wait_ld();
-      if (ki.valid) {
-        bf16* orow = ch == 0 ? (p.dv + ki.token * p.lddv + head * 64) : (p.dk + ki.token * p.lddk + head * 64);
-#pragma unroll
-        for (int k = 0; k < 32; k += 8) {
-          uint4 u;
-          u.x = pack_bf16x2(__uint_as_float(v0[k]), __uint_as_float(v0[k + 1]));
-          u.y = pack_bf16x2(__uint_as_float(v0[k + 2]), __uint_as_float(v0[k + 3]));
-          u.z = pack_bf16x2(__uint_as_float(v0[k + 4]), __uint_as_float(v0[k + 5]));
-          u.w = pack_bf16x2(__uint_as_float(v0[k + 6]), __uint_as_float(v0[k + 7]));
-          *reinterpret_cast<uint4*>(orow + k) = u;
-          u.x = pack_bf16x2(__uint_as_float(v1[k]), __uint_as_float(v1[k + 1]));
-          u.y = pack_bf16x2(__uint_as_float(v1[k + 2]), __uint_as_float(v1[k + 3]));
-          u.z = pack_bf16x2(__uint_as_float(v1[k + 4]), __uint_as_float(v1[k + 5]));
-          u.w = pack_bf16x2(__uint_as_float(v1[k + 6]), __uint_as_float(v1[k + 7]));
-          *reinterpret_cast<uint4*>(orow + 32 + k) = u;
-        }
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem, 512); }
+  const int wg = warp >> 2;
+  const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's key rows: r_lo, r_lo + 8
+  const RowInfo ki[2] = {row_info(p, r_lo, tile, outer, inner0), row_info(p, r_lo + 8, tile, outer, inner0)};
+  const float sc = p.scale * LOG2E;
+  // lse (threads 0..127) / delta (128..255) of query row threadIdx.x % 128 of a tile; +inf lse -> p = 0 for padding queries
+  const int vr = threadIdx.x & 127;
+  auto load_stat = [&](int i) -> float {
+    const RowInfo qi = row_info(p, vr, i, outer, inner0);
+    if (threadIdx.x < 128) return qi.valid ? p.lse[qi.token * p.heads + head] * LOG2E : INFINITY;
+    return qi.valid ? p.delta[qi.token * p.heads + head] : 0.f;
+  };
+  float stat = load_stat(0);
+  float dv[32], dk[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+  mbar_wait_mma(b_kvfull, 0);
+  for (int i = 0; i < nq; ++i) {
+    // stage lse/delta of the 128 queries of tile i (column vectors of the transposed scores); the values of the
+    // next tile are requested right away so that their latency hides behind this tile's work
+    named_bar_sync(1, 32 * AT_CONSUMER_WARPS);  // previous iteration finished reading vec[]
+    vec[threadIdx.x] = stat;
+    named_bar_sync(1, 32 * AT_CONSUMER_WARPS);
+    if (i + 1 < nq) stat = load_stat(i + 1);
+    const int st = i % BWD_STAGES;
+    const uint32_t sQ = sQD + st * 2 * TILE_BYTES, sDO = sQ + TILE_BYTES;
+    mbar_wait_mma(b_qfull + 8 * st, (i / BWD_STAGES) & 1);
+#pragma unroll 1
+    for (int qh = 0; qh < 2; ++qh) {
+      float s[32], dp[32];
+      mma_abt64(s, sK + wg * 8192, sQ + qh * 8192);     // S^T_h  = K Q_h^T
+      mma_abt64(dp, sV + wg * 8192, sDO + qh * 8192);   // dP^T_h = V dO_h^T
+      wgmma_wait<0>();
+      reg_fence(s); reg_fence(dp);
+#pragma unroll
+      for (int k = 0; k < 32; ++k) {
+        const int c = qh * 64 + frag_col(k, lane);       // query column
+        const RowInfo& r = ki[frag_hi(k)];
+        // G == 1: invalid query columns carry lse = +inf -> p = 0
+        const bool ok = r.valid && (p.G == 1 || (c & p.gmask) == r.g);
+        const float pr = ok ? fast_exp2(fmaf(s[k], sc, -vec[c])) : 0.f;
+        s[k] = pr;
+        dp[k] = (pr * p.scale) * (dp[k] - vec[128 + c]);
+      }
+      mma_pb64(dv, s, sDO + qh * 8192);                  // dV += P^T_h dO_h
+      mma_pb64(dk, dp, sQ + qh * 8192);                  // dK += dS^T_h Q_h
+      wgmma_wait<0>();
+      reg_fence(dv); reg_fence(dk);
+    }
+    release(b_qempty + 8 * st, lane);
+  }
+  store_frag_rows(ki[0].valid ? p.dv + ki[0].token * p.lddv + head * 64 : nullptr,
+                  ki[1].valid ? p.dv + ki[1].token * p.lddv + head * 64 : nullptr, dv, 1.f, 1.f, lane);
+  store_frag_rows(ki[0].valid ? p.dk + ki[0].token * p.lddk + head * 64 : nullptr,
+                  ki[1].valid ? p.dk + ki[1].token * p.lddk + head * 64 : nullptr, dk, 1.f, 1.f, lane);
 }
 
 // delta[token][head] = sum_d dO * O   — one warp per (token, head)
@@ -821,8 +530,8 @@ extern "C" int svdx_attention_bwd(const SvdxAttn* d, void* stream_v) {
   const long long warps = tokens * d->heads;
   attn_delta_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>(reinterpret_cast<const bf16*>(d->o), d->ldo,
                                                                          reinterpret_cast<const bf16*>(d->dout), d->lddo, tokens, d->heads, d->delta);
-  attn_bwd_dq_kernel<<<grid, BWD_THREADS, BDQ_SMEM, st>>>(p);
-  attn_bwd_dkv_kernel<<<grid, BWD_THREADS, BKV_SMEM, st>>>(p);
+  attn_bwd_dq_kernel<<<grid, AT_THREADS, BDQ_SMEM, st>>>(p);
+  attn_bwd_dkv_kernel<<<grid, AT_THREADS, BKV_SMEM, st>>>(p);
   SVDX_CHECK_LAUNCH("attention_bwd");
   return SVDX_OK;
 }

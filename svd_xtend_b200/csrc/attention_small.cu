@@ -2,18 +2,17 @@
 // (TemporalBasicTransformerBlock.attn1 [D], one sequence of T = 14 / 25 frames per pixel and head), forward and backward.
 //
 // Why a second kernel family: this op is HBM-bound, not tensor-bound — per (pixel, head) it does 2 x 14 x 14 x 64 MACs on
-// 3 x 14 x 128 bytes of input (0.64 GFLOP over 92 MB at the 40x64 level: 7 FLOP/byte). The tcgen05 kernel of attention.cu
-// packs 8 pixel sequences into one 128-row tile and masks 7/8 of the 128 x 128 scores; every CTA pays barrier set-up, a TMEM
-// allocation and three TMA round trips for 6 KB of useful data: 56 us forward / 235 us backward at the 40x64 level against
-// 14 us / 28 us of pure HBM traffic (profiles/r2_kbench_before.txt). A first CUDA-core version of this file (one lane per
-// query, K / V rows broadcast from shared memory) was shared-memory-bound and slower still (90 / 372 us).
+// 3 x 14 x 128 bytes of input (0.64 GFLOP over 92 MB at the 40x64 level: 7 FLOP/byte). The wgmma kernel of attention.cu
+// packs 8 pixel sequences into one 128-row tile and masks 7/8 of the 128 x 128 scores; every CTA pays barrier set-up and
+// three TMA round trips for 6 KB of useful data. A CUDA-core version (one lane per query, K / V rows broadcast from shared
+// memory) is shared-memory-bound.
 // This version gives each WARP one (sequence, head) and uses warp-level tensor-core MMAs (mma.sync m16n8k16, bf16 x bf16 ->
 // fp32) on 16-row tiles: the scores of a 14-token sequence are ONE 16 x 16 tile, the whole forward is 16 MMAs, the backward 56.
 // The tiny MMA work leaves the kernel bound by its loads: Q / K / V (/ dO) head slices are staged with coalesced 16-byte loads
 // into padded bf16 shared-memory tiles, fragments come from conflict-free 32-bit loads (K-major operands) or ldmatrix.trans
 // (key-major V / K / dO / Q as the k x n operand), results go back through shared memory as full 128-byte rows.
 // Token addressing follows the SvdxAttn descriptor (outer / inner / token strides): the strided "frames of one pixel" gather
-// needs no permute. (tcgen05.mma has a 128-row minimum and needs TMEM + mbarrier plumbing per CTA; for 16-row problems the
+// needs no permute. (the wgmma kernels work on 64-row warpgroup tiles of 128-row CTAs and need mbarrier plumbing per CTA; for 16-row problems the
 // warp-level MMA is the tensor-core path that fits, and the op's roofline is HBM either way.)
 //
 // forward : S = Q K^T * scale -> softmax over the S keys -> O = P V,  lse = log sum exp (natural log, as attention.cu)
@@ -354,7 +353,7 @@ __global__ void __launch_bounds__(AS_WARPS * 32) attn_small_bwd_kernel(const Sma
 
 using namespace svdx;
 
-// eligible: strided short sequences (the temporal attention); env SVDX_ATTN_SMALL=0 routes them back to the tcgen05 kernels
+// eligible: strided short sequences (the temporal attention); env SVDX_ATTN_SMALL=0 routes them back to the wgmma kernels
 bool svdx_attention_small_eligible(const SvdxAttn* d) {
   static int on = -1;
   if (on < 0) { const char* e = getenv("SVDX_ATTN_SMALL"); on = (e && e[0] == '0') ? 0 : 1; }

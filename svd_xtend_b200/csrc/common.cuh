@@ -1,5 +1,5 @@
-// Common sm_100a device helpers: mbarrier, TMA, tcgen05/TMEM inline PTX wrappers.
-// Hand-written for B200 (compile with -gencode arch=compute_100a,code=sm_100a).
+// Common sm_90a device helpers: mbarrier, TMA and wgmma inline PTX wrappers.
+// Hand-written for H100 (compile with -gencode arch=compute_90a,code=sm_90a).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -7,14 +7,16 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include "wgmma.cuh"
+
 namespace svdx {
 
 typedef __nv_bfloat16 bf16;
 
 #define SVDX_DEVINL __device__ __forceinline__
 
-// Spin budget before a barrier wait is declared dead (debug guard: a hung kernel on a
-// leased GPU box is far more expensive than a trap).
+// Spin budget before a barrier wait is declared dead (a hung kernel on a shared GPU is far more
+// expensive than a trap).
 #ifndef SVDX_WAIT_TIMEOUT_CYCLES
 #define SVDX_WAIT_TIMEOUT_CYCLES (4000000000ll)
 #endif
@@ -71,6 +73,14 @@ SVDX_DEVINL void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
+// the same wait without the report: inside a wgmma main loop a call (printf) would make ptxas serialise the wgmma pipeline
+SVDX_DEVINL void mbar_wait_mma(uint32_t bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity))
+    if (clock64() - t0 > SVDX_WAIT_TIMEOUT_CYCLES) __trap();
+}
+
 // ---------------------------------------------------------------- TMA (cp.async.bulk.tensor)
 SVDX_DEVINL void prefetch_tmap(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
@@ -114,98 +124,32 @@ SVDX_DEVINL void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c,
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-SVDX_DEVINL void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-}
-SVDX_DEVINL void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-SVDX_DEVINL void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-SVDX_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-SVDX_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-SVDX_DEVINL void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread.
-SVDX_DEVINL void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread retire.
-SVDX_DEVINL void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+// ---------------------------------------------------------------- wgmma (warpgroup MMA)
+SVDX_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+SVDX_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+SVDX_DEVINL void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+SVDX_DEVINL void reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread = TMEM lane).
-SVDX_DEVINL void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// 32 registers per thread -> 32 lanes x 32 consecutive fp32 columns
-SVDX_DEVINL void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%32], "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31};"
-      ::"r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-        "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-        "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31]),
-        "r"(taddr)
-      : "memory");
-}
-SVDX_DEVINL void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-SVDX_DEVINL void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
+SVDX_DEVINL void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
-// Shared-memory matrix descriptor (tcgen05), 128-byte swizzle.
+// Shared-memory matrix descriptor (wgmma), 128-byte swizzle.
 //   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version = 1 (Blackwell)
-//   bits [61,64) layout type: 2 = SWIZZLE_128B
-// K-major operand, rows of 64 bf16 (128 B): 8-row atom = 1024 B -> SBO = 1024, LBO unused.
+//   bits [32,46) stride byte offset >> 4   bits [62,64) layout type: 1 = SWIZZLE_128B
+// K-major operand, rows of 64 bf16 (128 B): 8-row atom = 1024 B -> SBO = 1024, LBO unused; a 16-deep k-step adds 32 B.
 // MN-major operand, 64 contiguous MN elements per 128 B line, 8 k-lines per atom:
-//   SBO = 1024 (next 8 k), LBO = byte distance between 64-wide MN blocks.
+//   SBO = 1024 (next 8 k), LBO = byte distance between 64-wide MN blocks; a 16-deep k-step adds 2048 B.
 SVDX_DEVINL uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// Instruction descriptor, kind::f16, bf16 x bf16 -> fp32, M x N tile.
-SVDX_DEVINL uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major, uint32_t b_mn_major) {
-  uint32_t d = 0;
-  d |= 1u << 4;    // D format: F32
-  d |= 1u << 7;    // A format: BF16
-  d |= 1u << 10;   // B format: BF16
-  d |= (a_mn_major & 1u) << 15;
-  d |= (b_mn_major & 1u) << 16;
-  d |= ((N >> 3) & 0x3F) << 17;
-  d |= ((M >> 4) & 0x1F) << 24;
+  d |= (uint64_t)1 << 62;
   return d;
 }
 

@@ -609,7 +609,7 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const bf16* __restric
 
 // ---- skinny products of the [B, C] conditioning vectors (time-embedding MLPs, all 44 time_emb_proj at once, the 1-key image
 // cross-attention collapse to_out(to_v(e)), their gradients): M = B rows. A 128-row tensor-core tile would be > 99 % padding and the
-// launch is latency-bound (17 us for a 1 x 1280 x 1280 product on the tcgen05 kernel); these are weight-streaming GEMVs.
+// launch is latency-bound (17 us for a 1 x 1280 x 1280 product on the tensor-core GEMM kernel); these are weight-streaming GEMVs.
 // out[m][n] = sum_k a[m][k] * w[n][k] (+ bias[n]), m < MR <= 8: one warp per output column, lanes stride K in 16-byte vectors.
 template <int MR>
 __global__ void __launch_bounds__(256) gemv_kernel(const bf16* __restrict__ a, long long lda, const bf16* __restrict__ w, long long ldw, int M, int N,

@@ -111,7 +111,7 @@ __global__ void gn_stats_finalize(float* mean, float* rstd, int total, float inv
 // ------------------------------------------------------------------ GroupNorm, cp.async ring variants
 // GroupNorm apply (+SiLU) and backward. Round 1-2's first versions kept 4 x 16-byte loads per tensor in flight per thread in
 // REGISTERS and then stalled on them; with 84-128 registers a thread only 15-30 warps were resident, so an SM had a load burst
-// in flight a fraction of the time (1-2.6 TB/s, profiles/r2_kbench_before.txt). Here every thread streams its rows through a private GN_RING-deep ring of 16-byte shared-memory slots filled by
+// in flight a fraction of the time (1-2.6 TB/s). Here every thread streams its rows through a private GN_RING-deep ring of 16-byte shared-memory slots filled by
 // cp.async (LDGSTS): GN_RING rows per tensor stay in flight per thread continuously, no registers are tied up by loads in
 // flight, and the first GN_RING rows are requested BEFORE the statistics prologue so its L2 round trips overlap the first
 // HBM round trip. A thread only ever reads slots it filled itself: cp.async.wait_group is the only synchronisation.

@@ -1,13 +1,13 @@
-// svdx_tapgemm: the tensor-core contraction of the SVD UNet hot path on sm_100a.
+// svdx_tapgemm: the tensor-core contraction of the SVD UNet hot path on sm_90a.
 //
-//   acc[m,n] = sum_taps sum_k A_tap[m,k] * B[n, tap*K + k]      (tcgen05.mma, fp32 accum in TMEM)
+//   acc[m,n] = sum_taps sum_k A_tap[m,k] * B[n, tap*K + k]      (wgmma, fp32 accumulators in registers)
 //
 // One persistent, warp-specialised kernel:
-//   warp 0      : TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer
-//   warps 2..5  : epilogue (tcgen05.ld TMEM->regs, bias/rowbias/GEGLU/residual/blend, global store)
-// Accumulators are double-buffered in TMEM (2 x 256 columns) so the epilogue of tile i overlaps
-// the main loop of tile i+1.
+//   warp 8      : TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
+//   warps 0..7  : two consumer warpgroups; warpgroup g multiplies rows [64g, 64g + 64) of the 128-row tile with wgmma,
+//                 then both park the fp32 tile in shared memory and run the epilogue on it (bias / rowbias / GEGLU /
+//                 residual / blend, staged TMA stores). The producer keeps filling the ring meanwhile, so the next
+//                 tile's operands are resident when the epilogue ends.
 //
 // A-operand modes (see include/svd_xtend_b200.h): plain/grouped rows with row-shifted taps
 // (linear, (3,1,1) temporal conv [D: TemporalResnetBlock]) and channels-last images with 2-D
@@ -17,51 +17,105 @@
 
 namespace svdx {
 
+// Main loop of one tile for one consumer warpgroup: rows [64 wg, 64 wg + 64) x BN columns, k-blocks [kb0, kb1) of the
+// ring, then the accumulator is written to the shared tile sAcc (row-major, ACC_LD floats per row).
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void tile_mainloop(int kb0, int kb1, uint32_t sA, uint32_t sB, uint32_t bar_full, uint32_t bar_empty,
+                                           uint32_t sAcc, int wg, int& stage, uint32_t& phase) {
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  const int lane = threadIdx.x & 31;
+  // K-major: + 32 B per 16-deep k-step; MN-major: + 2048 B (two 8-line groups), 64-wide MN blocks 8 KB apart
+  const uint32_t astep = TA ? (2048 >> 4) : (32 >> 4), bstep = TB ? (2048 >> 4) : (32 >> 4);
+  int prev_stage = -1;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait_mma(bar_full + 8 * stage, phase);
+    const uint32_t aaddr = sA + stage * A_STAGE_BYTES + wg * 8192;   // 64 rows: 8 KB in either major
+    const uint32_t baddr = sB + stage * B_STAGE_BYTES;
+    const uint64_t ad0 = make_smem_desc_sw128(aaddr, 8192, 1024);
+    const uint64_t bd0 = make_smem_desc_sw128(baddr, 8192, 1024);
+    wgmma_fence();
+#pragma unroll
+    for (int j = 0; j < BLOCK_K / 16; ++j) {
+      const uint32_t accumulate = (kb > kb0 || j > 0) ? 1u : 0u;
+      if constexpr (BN == 32) wgmma_ss_n32<TA, TB>(acc, ad0 + j * astep, bd0 + j * bstep, accumulate);
+      else if constexpr (BN == 64) wgmma_ss_n64<TA, TB>(acc, ad0 + j * astep, bd0 + j * bstep, accumulate);
+      else if constexpr (BN == 96) wgmma_ss_n96<TA, TB>(acc, ad0 + j * astep, bd0 + j * bstep, accumulate);
+      else if constexpr (BN == 128) wgmma_ss_n128<TA, TB>(acc, ad0 + j * astep, bd0 + j * bstep, accumulate);
+      else wgmma_ss_n160<TA, TB>(acc, ad0 + j * astep, bd0 + j * bstep, accumulate);
+    }
+    wgmma_commit();
+    // one group stays in flight: the previous k-block's operands are read out, its ring slot goes back to the producer
+    wgmma_wait<1>();
+    reg_fence(acc);
+    if (prev_stage >= 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * prev_stage);
+    }
+    prev_stage = stage;
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  reg_fence(acc);
+  __syncwarp();
+  if (lane == 0 && prev_stage >= 0) mbar_arrive(bar_empty + 8 * prev_stage);
+
+  // D fragment -> shared tile: register 4j + 2h + e is row 16 * warp + lane / 4 + 8h, column 8j + 2 * (lane % 4) + e
+  const int r0 = wg * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+  const uint32_t base = sAcc + (uint32_t)(r0 * ACC_LD + 2 * (lane & 3)) * 4u;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(base + (uint32_t)(h * 8 * ACC_LD + 8 * j) * 4u), "f"(acc[4 * j + 2 * h]),
+                   "f"(acc[4 * j + 2 * h + 1]) : "memory");
+  }
+}
+
+template <int TA, int TB>
+SVDX_DEVINL void tile_mainloop_bn(int bn, int kb0, int kb1, uint32_t sA, uint32_t sB, uint32_t bar_full, uint32_t bar_empty, uint32_t sAcc,
+                                  int wg, int& stage, uint32_t& phase) {
+  switch (bn) {
+    case 32: tile_mainloop<32, TA, TB>(kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase); break;
+    case 64: tile_mainloop<64, TA, TB>(kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase); break;
+    case 96: tile_mainloop<96, TA, TB>(kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase); break;
+    case 128: tile_mainloop<128, TA, TB>(kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase); break;
+    default: tile_mainloop<160, TA, TB>(kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase); break;
+  }
+}
+
 template <int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_constant__ TapGemmKParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sA = smem_base;
   const uint32_t sB = smem_base + STAGES * A_STAGE_BYTES;
-  const uint32_t sEpi = sB + STAGES * B_STAGE_BYTES;   // epilogue staging (TMA stores), 4 KB per epilogue warp
+  const uint32_t sAcc = sB + STAGES * B_STAGE_BYTES;     // the finished fp32 tile, read by the epilogue
+  const uint32_t sEpi = sAcc + ACC_BYTES;                // epilogue staging (TMA stores), 4 KB per epilogue warp
   const uint32_t sBar = sEpi + NUM_EPI_WARPS * EPI_STAGE_BYTES;
-  // barrier layout (8 B each): full[STAGES], empty[STAGES], tmem_full[ACC], tmem_empty[ACC], then tmem ptr
+  // barrier layout (8 B each): full[STAGES], empty[STAGES]
   const uint32_t bar_full = sBar;
   const uint32_t bar_empty = sBar + 8 * STAGES;
-  const uint32_t bar_tfull = sBar + 16 * STAGES;
-  const uint32_t bar_tempty = bar_tfull + 8 * ACC_STAGES;
-  const uint32_t tmem_slot = bar_tempty + 8 * ACC_STAGES;
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == PRODUCER_WARP && lane == 0) {
     prefetch_tmap(&p.tma);
     prefetch_tmap(&p.tmb);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(bar_full + 8 * i, 1);
-      mbar_init(bar_empty + 8 * i, 1);
-    }
-    for (int i = 0; i < ACC_STAGES; ++i) {
-      mbar_init(bar_tfull + 8 * i, 1);
-      mbar_init(bar_tempty + 8 * i, NUM_EPI_WARPS);  // one arrive per epilogue warp
+      mbar_init(bar_empty + 8 * i, NUM_EPI_WARPS);  // one arrive per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
   const int total_tiles = p.m_tiles * p.n_tiles * p.split_k;
   const int b_bytes = p.block_n * BLOCK_K * 2;
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // =========================== TMA producer ===========================
     const bool conv_par = (p.a_mode == SVDX_A_CONV2D) && !p.a_mn && !p.b_mn && !p.geglu && !p.wtiles && (BLOCK_M / p.W) <= 32;
     if (conv_par) {
@@ -83,7 +137,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
         for (int kb = kb0; kb < kb1; ++kb) {
           const uint32_t full = bar_full + 8 * stage;
           if (lane == 0) {
-            mbar_wait(bar_empty + 8 * stage, phase ^ 1);
+            mbar_wait_mma(bar_empty + 8 * stage, phase ^ 1);
             mbar_expect_tx(full, A_STAGE_BYTES + b_bytes);
           }
           __syncwarp();
@@ -114,7 +168,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
         for (int kb = kb0; kb < kb1; ++kb) {
           const uint32_t full = bar_full + 8 * stage;
           if (lane == 0) {
-            mbar_wait(bar_empty + 8 * stage, phase ^ 1);
+            mbar_wait_mma(bar_empty + 8 * stage, phase ^ 1);
             mbar_expect_tx(full, A_STAGE_BYTES + b_bytes);
           }
           __syncwarp();
@@ -147,7 +201,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
         int kci = kb0 - tap * p.kb_per_tap - 1;
         for (int kb = kb0; kb < kb1; ++kb) {
           if (++kci == p.kb_per_tap) { kci = 0; ++tap; }   // no per-k-block division on the issue path
-          mbar_wait(bar_empty + 8 * stage, phase ^ 1);
+          mbar_wait_mma(bar_empty + 8 * stage, phase ^ 1);
           const uint32_t full = bar_full + 8 * stage;
           mbar_expect_tx(full, A_STAGE_BYTES + b_bytes);
           const uint32_t dA = sA + stage * A_STAGE_BYTES;
@@ -243,59 +297,27 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
         }
       }
     }
-  } else if (warp == 1) {
-    // =========================== MMA issuer ===========================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(BLOCK_M, p.block_n, p.a_mn, p.b_mn);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int ks = tile / (p.n_tiles * p.m_tiles);
-        const int kb0 = ks * p.kb_per_split;
-        const int kb1 = min(kb0 + p.kb_per_split, p.kb_total);
-        mbar_wait(bar_tempty + 8 * acc, acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * 256;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(bar_full + 8 * stage, phase);
-          tc_fence_after();
-          const uint32_t aaddr = sA + stage * A_STAGE_BYTES;
-          const uint32_t baddr = sB + stage * B_STAGE_BYTES;
-          // one descriptor per operand and stage; a 16-deep k-step advances the 16-byte start-address field
-          const uint64_t ad0 = p.a_mn ? make_smem_desc_sw128(aaddr, 8192, 1024) : make_smem_desc_sw128(aaddr, 16, 1024);
-          const uint64_t bd0 = p.b_mn ? make_smem_desc_sw128(baddr, 8192, 1024) : make_smem_desc_sw128(baddr, 16, 1024);
-          const uint64_t astep = p.a_mn ? (2048 >> 4) : (32 >> 4), bstep = p.b_mn ? (2048 >> 4) : (32 >> 4);
-#pragma unroll
-          for (int j = 0; j < BLOCK_K / 16; ++j) {
-            const uint64_t ad = ad0 + j * astep;
-            const uint64_t bd = bd0 + j * bstep;
-            umma_bf16(d_tmem, ad, bd, idesc, (kb > kb0 || j > 0) ? 1u : 0u);
-          }
-          umma_commit(bar_empty + 8 * stage);  // frees the smem slot when these MMAs retire
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(bar_tfull + 8 * acc);  // accumulator complete
-        if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
-      }
-    }
   } else {
-    // =========================== epilogue warps ===========================
-    const int q = warp & 3;          // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;  // which of the two warps of the quarter: takes chunks half, half+2, ...
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    // =========================== consumer warpgroups: main loop + epilogue ===========================
+    const int wg = warp >> 2;
+    const int q = warp & 3;            // 32-row quarter of the tile this warp's epilogue writes
+    const int half = warp >> 2;        // which of the two warps of the quarter: takes chunks half, half+2, ...
+    int stage = 0;
+    uint32_t phase = 0;
     float s_acc = 1.f, s_r1 = 1.f, s_r2 = 1.f;
     if (p.scales) { s_acc = p.scales[0]; s_r1 = p.scales[1]; s_r2 = p.scales[2]; }
     const int n_out_total = p.geglu ? p.N / 2 : p.N;
     const int bn_out = p.geglu ? p.block_n / 2 : p.block_n;
     EpiStage st;
-    st.base = sEpi + (warp - 2) * EPI_STAGE_BYTES;
+    st.base = sEpi + warp * EPI_STAGE_BYTES;
     st.off = 0;
+    const uint32_t t_base = sAcc + (uint32_t)((q * 32 + lane) * ACC_LD) * 4u;   // this thread's accumulator row
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int nt = tile % p.n_tiles;
       const int mt = (tile / p.n_tiles) % p.m_tiles;
+      const int ks = tile / (p.n_tiles * p.m_tiles);
+      const int kb0 = ks * p.kb_per_split;
+      const int kb1 = min(kb0 + p.kb_per_split, p.kb_total);
       const int n0 = nt * bn_out;
       long long m;
       bool row_ok;
@@ -319,28 +341,20 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
       }
       if constexpr (EPI == EPI_RES || EPI == EPI_RES_GN || EPI == EPI_FAST_GNB)
         prefetch_epilogue_operands(p, EPI, m0, valid_rows, n0, bn_out, n_out_total, lane, half);
-      mbar_wait(bar_tfull + 8 * acc, acc_phase);
-      tc_fence_after();
-      const uint32_t t_base = tmem_base + acc * 256 + ((uint32_t)(q * 32) << 16);
+      // every warp has finished reading the previous tile's accumulator before it is overwritten
+      named_bar_sync(1, 32 * NUM_EPI_WARPS);
+      if (p.a_mn && p.b_mn) tile_mainloop_bn<1, 1>(p.block_n, kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase);
+      else if (p.a_mn) tile_mainloop_bn<1, 0>(p.block_n, kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase);
+      else if (p.b_mn) tile_mainloop_bn<0, 1>(p.block_n, kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase);
+      else tile_mainloop_bn<0, 0>(p.block_n, kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase);
+      named_bar_sync(1, 32 * NUM_EPI_WARPS);
       if constexpr (EPI == EPI_FAST || EPI == EPI_FAST_GN) epilogue_fast<EPI == EPI_FAST_GN>(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, st.base, st.row0, st.grp, lane, m0, valid_rows);
       else if constexpr (EPI == EPI_RES || EPI == EPI_RES_GN) epilogue_res<EPI == EPI_RES_GN>(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, s_acc, s_r1, s_r2, st.base, st.off, st.row0, st.grp, lane, m0, valid_rows);
       else if constexpr (EPI == EPI_GEGLU) epilogue_geglu(p, t_base, n0, half, bn_out, st.base, st.row0, st.grp, lane);
       else if constexpr (EPI == EPI_FAST_GNB) epilogue_fast_gnb(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, st.base, st.row0, st.grp, lane, m0, valid_rows);
       else epilogue_tile(p, t_base, m, row_ok, n0, half, bn_out, n_out_total, s_acc, s_r1, s_r2, st, lane);
-      // release the accumulator stage back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_tempty + 8 * acc);
-      if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
     }
     if (lane == 0) bulk_wait<0>();   // staged stores must have left shared memory (and landed) before the CTA exits
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
   }
 }
 
@@ -348,12 +362,25 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
 
 using namespace svdx;
 
-int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p, int cg) {
+// Tile width the kernel runs for a requested block_n: requests up to MAX_BN run as asked; wider ones (256, 192, 320, ...)
+// run as the widest multiple of 32 (64 for MN-major B and GEGLU, whose halves are 32-column chunks) up to MAX_BN (128) that
+// divides the request, so the tiles still cover every output column the requested width covers.
+static int kernel_block_n(int block_n, bool step64) {
+  const int step = step64 ? 64 : 32, cap = step64 ? 128 : MAX_BN;
+  if (block_n <= cap) return block_n;
+  for (int w = cap; w > step; w -= step)
+    if (block_n % w == 0) return w;
+  return step;
+}
+
+int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p) {
   if (!d || !d->a || !d->b || !d->out) return svdx_fail(SVDX_E_BADARG, "tapgemm: null pointer");
-  // block_n == 320: the CTA-pair kernel's two-MMA tile (256 x 320, see tapgemm2.cu) — pair-eligible problems only
-  const bool wide320 = (cg == 2 && d->block_n == 320);
+  // block_n == 320: 320-column tiles of bf16-output, non-GEGLU problems with M >= 512 (run as two 160-wide tiles)
+  const bool wide320 = d->block_n == 320;
+  if (wide320 && (d->geglu || d->N % 320 || d->M < 512 || d->out_dtype != SVDX_OUT_BF16))
+    return svdx_fail(SVDX_E_BADARG, "tapgemm: block_n 320 needs N %% 320 == 0, M >= 512 and a bf16 output without GEGLU");
   if (!wide320 && (d->block_n < 32 || d->block_n > 256 || d->block_n % 32))
-    return svdx_fail(SVDX_E_BADARG, "tapgemm: block_n must be a multiple of 32 in [32,256] (or 320 for CTA-pair eligible problems)");
+    return svdx_fail(SVDX_E_BADARG, "tapgemm: block_n must be a multiple of 32 in [32,256] (or 320)");
   if (d->b_major_mn && d->block_n % 64) return svdx_fail(SVDX_E_BADARG, "tapgemm: block_n %% 64 for MN-major B");
   if (d->num_taps < 1 || d->num_taps > SVDX_MAX_TAPS) return svdx_fail(SVDX_E_BADARG, "tapgemm: num_taps");
   if (d->M <= 0 || d->N <= 0 || d->K <= 0) return svdx_fail(SVDX_E_BADARG, "tapgemm: empty problem");
@@ -368,9 +395,10 @@ int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p, int cg) {
   p.a_mode = d->a_mode; p.a_mn = d->a_major_mn; p.b_mn = d->b_major_mn;
   p.num_taps = d->num_taps;
   for (int i = 0; i < d->num_taps; ++i) { p.tap_d0[i] = d->tap_d0[i]; p.tap_d1[i] = d->tap_d1[i]; p.tap_d2[i] = d->tap_d2[i]; }
-  p.M = d->M; p.N = d->N; p.K = d->K; p.block_n = d->block_n; p.split_k = d->split_k;
+  const int block_n = kernel_block_n(d->block_n, d->b_major_mn || d->geglu);
+  p.M = d->M; p.N = d->N; p.K = d->K; p.block_n = block_n; p.split_k = d->split_k;
   p.geglu = d->geglu;
-  const int bn_out = d->geglu ? d->block_n / 2 : d->block_n;
+  const int bn_out = d->geglu ? block_n / 2 : block_n;
   const int n_out = d->geglu ? d->N / 2 : d->N;
   p.n_tiles = (n_out + bn_out - 1) / bn_out;
 
@@ -451,13 +479,11 @@ int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p, int cg) {
   } else {
     uint64_t dims[2] = {(uint64_t)d->K * d->num_taps, (uint64_t)d->N};
     uint64_t strides[1] = {(uint64_t)d->ldb * 2};
-    // a CTA of a pair fetches half of the B tile; a GEGLU tile is already fetched as two halves (value | gate)
-    uint32_t box[2] = {64, (uint32_t)(wide320 ? 80 : (d->geglu || cg == 2) ? d->block_n / 2 : d->block_n)};
+    // a GEGLU tile is fetched as two halves (value | gate)
+    uint32_t box[2] = {64, (uint32_t)(d->geglu ? block_n / 2 : block_n)};
     rc = svdx_make_tmap(&p.tmb, d->b, 2, dims, strides, box);
   }
   if (rc) return rc;
-  p.tiles_per_group_pairs = (p.tiles_per_group + 1) / 2;
-  p.pair_m_tiles = p.tiles_per_group_pairs * p.groups;
 
   p.kb_per_tap = (d->K + BLOCK_K - 1) / BLOCK_K;
   p.kb_total = p.kb_per_tap * d->num_taps;
@@ -545,16 +571,11 @@ int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p, int cg) {
   return SVDX_OK;
 }
 
-int svdx_tapgemm2_launch(const TapGemmKParams& p, cudaStream_t stream);   // tapgemm2.cu
-bool svdx_tapgemm2_eligible(const SvdxTapGemm* d);
-
 extern "C" int svdx_tapgemm(const SvdxTapGemm* d, void* stream_v) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
   TapGemmKParams p;
-  const bool pair = svdx_tapgemm2_eligible(d);
-  int rc = svdx_tapgemm_fill(d, p, pair ? 2 : 1);
+  int rc = svdx_tapgemm_fill(d, p);
   if (rc) return rc;
-  if (pair) return svdx_tapgemm2_launch(p, stream);
   static bool attr_done[SVDX_MAX_DEVICES] = {false};
   const int slot = svdx_device_slot();
   if (!attr_done[slot]) {

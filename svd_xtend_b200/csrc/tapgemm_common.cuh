@@ -1,28 +1,29 @@
-// Shared pieces of the tcgen05 tapgemm kernels (1-CTA in tapgemm.cu, 2-CTA pairs in tapgemm2.cu):
-// kernel parameter block, tile geometry and the fused epilogue of one accumulator tile.
+// Shared pieces of the wgmma tapgemm kernel (tapgemm.cu): kernel parameter block, tile geometry and the fused epilogue
+// of one accumulator tile.
 #pragma once
 #include "common.cuh"
 #include "../../include/svd_xtend_b200.h"
 #include "host_util.h"
 
-// default of the SVDX_2CTA switch (env SVDX_2CTA=0/1 overrides): use the CTA-pair kernel where eligible
-#ifndef SVDX_2CTA_DEFAULT
-#define SVDX_2CTA_DEFAULT 1
-#endif
-
 namespace svdx {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;
-constexpr int STAGES = 4;
+constexpr int STAGES = 3;
+constexpr int MAX_BN = 160;                           // widest tile: 80 accumulator registers per thread
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
-constexpr int B_STAGE_BYTES = 256 * BLOCK_K * 2;      // 32 KB
-constexpr int ACC_STAGES = 2;
-constexpr int TMEM_COLS = 512;
-constexpr int NUM_EPI_WARPS = 8;   // two warps per TMEM lane quarter, each takes every other 32-column chunk
-constexpr int NUM_THREADS = 64 + 32 * NUM_EPI_WARPS;
+constexpr int B_STAGE_BYTES = MAX_BN * BLOCK_K * 2;   // 20 KB
+constexpr int NUM_EPI_WARPS = 8;   // the two consumer warpgroups: wgmma main loop, then the epilogue of the tile
+constexpr int PRODUCER_WARP = NUM_EPI_WARPS;
+constexpr int NUM_THREADS = 32 * NUM_EPI_WARPS + 32;
+// the finished fp32 accumulator tile in shared memory, one 128-row x MAX_BN tile; rows padded by 16 bytes so that the
+// epilogue's row-per-lane 16-byte reads are conflict-free
+constexpr int ACC_LD = MAX_BN + 4;
+constexpr int ACC_BYTES = BLOCK_M * ACC_LD * 4;
 constexpr int EPI_STAGE_BYTES = 4096;  // per epilogue warp: 2 x (32 rows x 64 B) bf16 halves or 1 x (32 rows x 128 B) fp32
-constexpr int SMEM_BYTES = 1024 + STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + NUM_EPI_WARPS * EPI_STAGE_BYTES + 256;
+constexpr int SMEM_BYTES = 1024 + STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + ACC_BYTES + NUM_EPI_WARPS * EPI_STAGE_BYTES + 256;
+static_assert(SMEM_BYTES <= 227 * 1024, "tapgemm shared memory exceeds the 227 KB a block may use");
+static_assert((ACC_BYTES % 1024) == 0 && (B_STAGE_BYTES % 1024) == 0, "staging buffers must stay 1024-byte aligned");
 
 struct __align__(64) TapGemmKParams {
   CUtensorMap tma;
@@ -37,7 +38,6 @@ struct __align__(64) TapGemmKParams {
   int tap_d0[SVDX_MAX_TAPS], tap_d1[SVDX_MAX_TAPS], tap_d2[SVDX_MAX_TAPS];
   int M, N, K;
   int block_n, m_tiles, n_tiles, split_k, kb_total, kb_per_split, kb_per_tap;
-  int pair_m_tiles, tiles_per_group_pairs;   // CTA-pair kernel: 256-row tiles (never straddling a group)
   // epilogue
   void* out;
   long long ldo;
@@ -73,6 +73,15 @@ struct __align__(64) TapGemmKParams {
 };
 
 
+// 32 consecutive fp32 accumulator columns [col, col + 32) of one tile row (row = the row's shared-memory address)
+SVDX_DEVINL void acc_ld32(uint32_t row, int col, uint32_t (&r)[32]) {
+  const uint32_t a = row + col * 4;
+#pragma unroll
+  for (int k = 0; k < 8; ++k)
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(r[4 * k]), "=r"(r[4 * k + 1]), "=r"(r[4 * k + 2]), "=r"(r[4 * k + 3])
+                 : "r"(a + 16 * k));
+}
+
 // output row of epilogue thread r (0..127) of m-tile mt, and whether it exists
 SVDX_DEVINL void tile_row(const TapGemmKParams& p, int mt, int r, long long& m, bool& row_ok) {
   if (p.a_mode == SVDX_A_ROWS && !p.a_mn) {
@@ -90,8 +99,8 @@ SVDX_DEVINL void tile_row(const TapGemmKParams& p, int mt, int r, long long& m, 
 // ---- conv A tiles: the 128 pixels of a tile are R = 128 / W consecutive image rows, fetched as a few multi-row TMA
 // boxes (image borders and tile/image straddling decide the split). The split depends on the tile only, so it is
 // computed once per tile with lane l of the producer warp keeping box l; per k-block every lane that owns a box
-// issues its TMA. (The per-k-block scalar decomposition cost ~1.5-3 k cycles and made the producer thread the
-// bottleneck of every 3x3 convolution: profiles/r1_conv_probe.txt.)
+// issues its TMA. (A per-k-block scalar decomposition costs ~1.5-3 k cycles and makes the producer thread the
+// bottleneck of a 3x3 convolution.)
 struct ConvBox {
   int lg, hh, n;
   uint32_t dst_off;
@@ -120,7 +129,7 @@ SVDX_DEVINL void conv_tile_boxes(const TapGemmKParams& p, int t, int lane, ConvB
 // ---- staged stores: a warp writes its 32-row x 32-column chunk into shared memory (one row per lane, swizzled so
 // that the 16-byte writes are conflict-free) and one lane hands it to the TMA unit. The global writes become full
 // 64/128-byte row segments issued asynchronously, instead of 32 scattered 16-byte sectors per store instruction
-// (measured: the scattered stores made every K<=640 GEMM epilogue-bound, profiles/r1_epilogue_probe.txt).
+// (scattered stores make the short-K GEMMs epilogue-bound).
 // Rows past the end of the group / matrix and columns past n_out are clipped by the tensor map.
 struct EpiStage {
   uint32_t base;   // this warp's 4 KB staging region (1024-aligned)
@@ -198,7 +207,7 @@ SVDX_DEVINL void gn_chunk_sums(const TapGemmKParams& p, uint32_t buf, int lane, 
 }
 
 // ---- specialised epilogues (kernel template parameter EPI): the hot shapes have short K, so the per-chunk instruction
-// count of the epilogue decides their speed (profiles/r1_epilogue_probe.txt). EPI_FAST / EPI_GEGLU assume a bf16 output
+// count of the epilogue decides their speed. EPI_FAST / EPI_GEGLU assume a bf16 output
 // written through TMA, whole 32-column chunks (n_out % 32 == 0) and 16-byte aligned bias rows; everything else takes
 // the generic epilogue_tile below.
 constexpr int EPI_GENERIC = 0, EPI_FAST = 1, EPI_GEGLU = 2, EPI_RES = 3;
@@ -232,9 +241,8 @@ SVDX_DEVINL void stage_row_bf16(uint32_t row, int sw, const float (&f)[32]) {
 }
 
 // Epilogue operands that are read per chunk (the residual of EPI_RES, the GroupNorm input of EPI_FAST_GNB) are usually not in L2
-// any more; a warp has ONE chunk's loads in flight, so the fetch was latency-bound (+12 us on a 15 us K = 320 residual GEMM,
-// +20 us on a conv dgrad with the backward sums). Each epilogue warp therefore requests its 32 rows x bn columns of the tile
-// into L2 BEFORE it waits for the accumulator: the lines arrive during the main loop. Lane = row; the two warps of a lane
+// any more; a warp has ONE chunk's loads in flight, so the fetch is latency-bound. Each epilogue warp therefore requests its 32 rows x bn columns of the tile
+// into L2 BEFORE its main loop: the lines arrive while the tensor cores work. Lane = row; the two warps of a lane
 // quarter take alternate 128-byte lines.
 SVDX_DEVINL void prefetch_rows_l2(const bf16* base, long long ld, long long m0, int valid_rows, int col0, int ncols, int lane, int half) {
   if (!base || lane >= valid_rows) return;
@@ -274,9 +282,8 @@ SVDX_DEVINL void epilogue_fast(const TapGemmKParams& p, uint32_t t_base, long lo
     const int colB = colA + 64;
     const bool hasB = (c + 64 < c_hi) && (colB < n_out_total);     // warp-uniform
     uint32_t va[32], vb[32];
-    tmem_ld32(t_base + c, va);
-    if (hasB) tmem_ld32(t_base + c + 64, vb);
-    tc_wait_ld();
+    acc_ld32(t_base, c, va);
+    if (hasB) acc_ld32(t_base, c + 64, vb);
     float fa[32], fb[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) { fa[i] = __uint_as_float(va[i]); fb[i] = __uint_as_float(vb[i]); }
@@ -393,7 +400,7 @@ SVDX_DEVINL void epilogue_fast_gnb(const TapGemmKParams& p, uint32_t t_base, lon
   for (int c = c_lo + half * 32; c < c_hi; c += 64) {
     const int col0 = n0 + c;
     if (col0 >= n_out_total) break;
-    // the matching chunk of the GroupNorm input, fetched coalesced (8 rows x 64 B per instruction) before the TMEM wait
+    // the matching chunk of the GroupNorm input, fetched coalesced (8 rows x 64 B per instruction) before the accumulator read
     const bool src1 = col0 < p.gnb_c1;
     const long long xld = src1 ? p.gnb_ldx : p.gnb_ldx2;
     const bf16* xs = (src1 ? p.gnb_x + col0 : p.gnb_x2 + (col0 - p.gnb_c1)) + m0 * xld + ppc * 8;
@@ -404,8 +411,7 @@ SVDX_DEVINL void epilogue_fast_gnb(const TapGemmKParams& p, uint32_t t_base, lon
       xa[j] = (rr < valid_rows) ? *reinterpret_cast<const uint4*>(xs + (long long)rr * xld) : make_uint4(0u, 0u, 0u, 0u);
     }
     uint32_t v[32];
-    tmem_ld32(t_base + c, v);
-    tc_wait_ld();
+    acc_ld32(t_base, c, v);
     float f[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
@@ -428,7 +434,7 @@ SVDX_DEVINL void epilogue_fast_gnb(const TapGemmKParams& p, uint32_t t_base, lon
 }
 
 // residual / AlphaBlender epilogue: out = s_acc*(acc + bias + rowbias) + s_r1*res1 + s_r2*res2; one chunk per round,
-// alternating staging halves; the residual rows are requested before the TMEM wait.
+// alternating staging halves; the residual rows are requested before the accumulator read.
 template <bool GN>
 SVDX_DEVINL void epilogue_res(const TapGemmKParams& p, uint32_t t_base, long long m, bool row_ok, int n0, int half, int c_lo, int c_hi,
                               int n_out_total, float s_acc, float s_r1, float s_r2, uint32_t sbase, uint32_t& off, int row0, int grp, int lane,
@@ -465,8 +471,7 @@ SVDX_DEVINL void epilogue_res(const TapGemmKParams& p, uint32_t t_base, long lon
       for (int k = 0; k < 4; ++k) a2[k] = q[k];
     }
     uint32_t v[32];
-    tmem_ld32(t_base + c, v);
-    tc_wait_ld();
+    acc_ld32(t_base, c, v);
     float f[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
@@ -514,9 +519,8 @@ SVDX_DEVINL void epilogue_geglu(const TapGemmKParams& p, uint32_t t_base, int n0
   for (int c = half * 32; c < bn_out; c += 64) {
     const int col0 = n0 + c;
     uint32_t v[32], gte[32];
-    tmem_ld32(t_base + c, v);
-    tmem_ld32(t_base + bn_out + c, gte);
-    tc_wait_ld();
+    acc_ld32(t_base, c, v);
+    acc_ld32(t_base, bn_out + c, gte);
     float f[32], g[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) { f[i] = __uint_as_float(v[i]); g[i] = __uint_as_float(gte[i]); }
@@ -555,7 +559,7 @@ SVDX_DEVINL void epilogue_geglu(const TapGemmKParams& p, uint32_t t_base, int n0
   }
 }
 
-// Epilogue of one accumulator tile for one thread (= one TMEM lane = one output row): this warp takes the 32-column
+// Epilogue of one accumulator tile for one thread (= one output row): this warp takes the 32-column
 // chunks half, half+2, ...; bias / row-bias / GEGLU / residuals / scales, then staged TMA stores (or direct 16-byte
 // stores when the output cannot be described by a tensor map).
 SVDX_DEVINL void epilogue_tile(const TapGemmKParams& p, uint32_t t_base, long long m, bool row_ok, int n0, int half, int bn_out,
@@ -568,7 +572,7 @@ SVDX_DEVINL void epilogue_tile(const TapGemmKParams& p, uint32_t t_base, long lo
         const int col0 = n0 + c;
         if (col0 >= n_out_total) break;   // warp-uniform
         const bool full_chunk = (col0 + 32 <= n_out_total);
-        // issue the global reads of this chunk before waiting on TMEM so their latency overlaps
+        // issue the global reads of this chunk before reading the accumulator so their latency overlaps
         uint4 rr1[4], rr2[4];
         if (row_ok && full_chunk) {
           if (p.res1) {
@@ -583,9 +587,8 @@ SVDX_DEVINL void epilogue_tile(const TapGemmKParams& p, uint32_t t_base, long lo
           }
         }
         __syncwarp();
-        tmem_ld32(t_base + c, v);
-        if (p.geglu) tmem_ld32(t_base + bn_out + c, gte);
-        tc_wait_ld();
+        acc_ld32(t_base, c, v);
+        if (p.geglu) acc_ld32(t_base, bn_out + c, gte);
         float f[32];
 #pragma unroll
         for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
@@ -759,5 +762,5 @@ SVDX_DEVINL void epilogue_tile(const TapGemmKParams& p, uint32_t t_base, long lo
 
 }  // namespace svdx
 
-// host: validates the descriptor and fills the kernel parameter block. cg = CTAs per tile (1 or 2).
-int svdx_tapgemm_fill(const SvdxTapGemm* d, svdx::TapGemmKParams& p, int cg);
+// host: validates the descriptor and fills the kernel parameter block.
+int svdx_tapgemm_fill(const SvdxTapGemm* d, svdx::TapGemmKParams& p);

@@ -1,6 +1,6 @@
-"""Execution engine of the B200 SVD-UNet step: a hand-rolled tape over the C-ABI kernels.
+"""Execution engine of the H100 SVD-UNet step: a hand-rolled tape over the C-ABI kernels.
 
-Design (B200-first, not a translation of diffusers' module-by-module autograd graph):
+Design (GPU-first, not a translation of diffusers' module-by-module autograd graph):
   * activations live as token-major channels-last bf16 matrices ``[B*T*H*W, C]`` for the WHOLE
     network — the (BT,C,H,W)<->(BT,HW,C)<->(B*HW,T,C) permutes of the reference
     (SURVEY.md K13) never happen: linears are row-permutation invariant, the temporal conv and

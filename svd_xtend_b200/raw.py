@@ -40,7 +40,7 @@ def check(rc: int, what: str = "") -> None:
 # outputs stay uninitialised: only for timing a captured step with that family removed, never for results).
 ABLATE: set = set()
 ACCOUNT = None
-SHAPE_LOG = None     # list: one record per svdx_tapgemm launch, in launch order (joined with the ncu launch list by scripts/)
+SHAPE_LOG = None     # list: one record per svdx_tapgemm launch, in launch order (bench.py --profile-one with SVDX_SHAPE_LOG)
 
 
 def _fam(family: str, flops: float = 0.0, nbytes: float = 0.0) -> bool:
@@ -85,32 +85,19 @@ def num_sms() -> int:
     return _NUM_SMS[0]
 
 
-PAIR_MODE = os.environ.get("SVDX_2CTA", "1") != "0"     # mirrors SVDX_2CTA_DEFAULT of tapgemm_common.cuh
-_L2_BYTES_PER_CLK = 4500.0                                # ~8.5 TB/s L2->SM at 1.9 GHz (measured, profiles/)
-
-
-def pair_eligible(M: int, n_out: int, bn_out: int, geglu: bool) -> bool:
-    """same rule as svdx_tapgemm2_eligible (tapgemm2.cu) for K-major problems without split-K"""
-    bn = 2 * bn_out if geglu else bn_out
-    return PAIR_MODE and M >= 512 and bn >= 64 and bn % 32 == 0 and (bn // 2) % 8 == 0 and n_out % bn_out == 0
+# Relative cost model of a tile width: the tensor pipe's time per k-block against the L2 -> SM bytes of the CTAs that run
+# at once. The widths are the ones the kernel runs (tapgemm.cu: at most 160 columns, 128 for MN-major B and GEGLU).
+_L2_BYTES_PER_CLK = 4500.0
 
 
 def _tile_cost(M: int, n_out: int, bn_out: int, geglu: bool, sms: int) -> float:
-    """relative time of the whole problem with output tiles 128 x bn_out (256 x bn_out for a CTA pair):
-    waves over the SMs x per-k-block time = max(tensor pipe, L2->SM bytes at the measured chip bandwidth)."""
+    """relative time of the whole problem with output tiles 128 x bn_out:
+    waves over the SMs x per-k-block time = max(tensor pipe, L2->SM bytes)."""
     bn = 2 * bn_out if geglu else bn_out
-    m_tiles = (M + 127) // 128
-    n_tiles = (n_out + bn_out - 1) // bn_out
-    pair = pair_eligible(M, n_out, bn_out, geglu)
-    if pair:
-        ctas = 2 * ((m_tiles + 1) // 2) * n_tiles
-        bytes_kb = 16384 + 64 * bn
-    else:
-        ctas = m_tiles * n_tiles
-        bytes_kb = 16384 + 128 * bn
+    ctas = ((M + 127) // 128) * ((n_out + bn_out - 1) // bn_out)
     active = min(ctas, sms)
-    mma = 4 * max(bn / 2.0, 32.0 + bn / 4.0 if not pair else bn / 2.0)
-    l2 = bytes_kb * active / _L2_BYTES_PER_CLK
+    mma = 4 * max(bn / 2.0, 32.0 + bn / 4.0)
+    l2 = (16384 + 128 * bn) * active / _L2_BYTES_PER_CLK
     waves = (ctas + sms - 1) // sms
     return waves * max(mma, l2)
 
@@ -123,12 +110,12 @@ def choose_block_n(M: int, n_out: int, geglu: bool = False, mn_major: bool = Fal
     if mn_major:
         best, best_cost = None, None
         m_tiles = (M + 127) // 128
-        for bn in (256, 192, 128, 64):
+        for bn in (128, 64):
             cost = m_tiles * ((n_out + bn - 1) // bn) * max(bn / 2.0, 32.0 + bn / 4.0)
             if best_cost is None or cost < best_cost - 1e-9:
                 best, best_cost = bn, cost
         return best
-    cands = [128, 64, 32] if geglu else [256, 160, 128, 96, 64, 32]
+    cands = [64, 32] if geglu else [160, 128, 96, 64, 32]
     best, best_cost = None, None
     for bn in cands:
         if n_out % bn and n_out > bn:
@@ -146,13 +133,9 @@ WIDE_MIN_K = int(os.environ.get("SVDX_WIDE_MIN_K", "960"))
 
 
 def _wide_tile_ok(M, N, k_total, out, ldo, geglu, a_mn, b_mn, b_mode, split_k, out_dtype, bias, rowbias) -> bool:
-    """256 x 320 CTA-pair tiles (svdx_tapgemm block_n = 320: the A tile crosses L2 once per 320 output columns instead of
-    once per 160) for the C = 320 / 640 / 960 layers when the contraction is long enough to hide the partly exposed epilogue
-    of the overlapping accumulators. Mirrors the library's conditions for the wide form (CTA-pair kernel, bf16 TMA-store
-    epilogues); anything else keeps choose_block_n's width."""
-    # measured (scripts/kbench.py gemm, profiles/r2_kbench_gemm.txt): wins 8-25 % where the alternative is 160-wide tiles and
-    # K * taps >= 960 (convs at C = 320 / 640: 1.06 -> 1.30-1.43 PFLOP/s); loses against 256-wide tiles (N % 256 == 0) and
-    # at short K, where the partly exposed epilogue costs more than the A traffic saved
+    """whether a problem may be launched with block_n = 320 (svdx_tapgemm accepts it for bf16-output, non-GEGLU problems
+    with N % 320 == 0 and M >= 512, and runs it as 160-wide tiles): the C = 320 / 640 / 960 layers with a long contraction.
+    Mirrors the library's conditions; anything else keeps choose_block_n's width."""
     if not WIDE_TILE or geglu or a_mn or b_mn or b_mode != 0 or split_k != 1 or N % 320 or N % 256 == 0 or M < 512 or k_total < WIDE_MIN_K:
         return False
     if out.dtype != bf16 or (out_dtype is not None and out_dtype != OUT_BF16):
@@ -167,20 +150,18 @@ def _wide_tile_ok(M, N, k_total, out, ldo, geglu, a_mn, b_mn, b_mode, split_k, o
     return True
 
 
-_WGRAD_L2_BYTES_PER_CLK = 6500.0     # fitted to profiles/r2_kbench.txt (weight-gradient GEMMs are L2 -> SM bound)
+_WGRAD_L2_BYTES_PER_CLK = 6500.0     # weight-gradient GEMMs are L2 -> SM bound
 
 
 def wgrad_plan(O: int, K: int, M: int):
     """(block_n, split_k) of a weight-gradient GEMM dW[O, K] += dy[M, O]^T x[M, K] (MN-major operands, fp32 reduce-add
-    epilogue). Tile width and the split of the token contraction are chosen TOGETHER by a small model fitted to measured
-    launches (profiles/r2_kbench.txt): CTAs = tiles * split, time = waves * (k-blocks per CTA * max(tensor pipe, L2 -> SM bytes of the
-    CTAs running concurrently) + tile reduce-add). The round-1 rule picked the tile width alone from MMA efficiency and
-    chose 128-wide tiles at K = 640, twice the L2 traffic of 256-wide ones (100 us vs 62 us for O = 5120, K = 640)."""
+    epilogue). Tile width and the split of the token contraction are chosen TOGETHER by a small model: CTAs = tiles * split,
+    time = waves * (k-blocks per CTA * max(tensor pipe, L2 -> SM bytes of the CTAs running concurrently) + tile reduce-add)."""
     sms = num_sms()
     kb = (M + 63) // 64
     m_tiles = (O + 127) // 128
     best = None
-    for bn in ((192, 256, 128) if K > 64 else (64,)):     # ties go to the earlier width
+    for bn in ((128, 64) if K > 64 else (64,)):     # ties go to the earlier width; MN-major tiles are at most 128 wide
         n_tiles = (K + bn - 1) // bn
         tiles = m_tiles * n_tiles
         splits = {1, max(1, min(kb // 32, sms // max(tiles, 1))), max(1, min(kb // 8, -(-sms // max(tiles, 1))))}

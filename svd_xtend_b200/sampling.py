@@ -1,4 +1,4 @@
-"""Forward-only UNet sampling on B200: the UNet-facing part of the reference's validation / inference path
+"""Forward-only UNet sampling on H100: the UNet-facing part of the reference's validation / inference path
 (`StableVideoDiffusionPipeline(...)(image, num_frames=…, motion_bucket_id=127, fps=7, noise_aug_strength=0.02)`,
 /root/reference/train_svd.py:1106-1140, infer_svd.ipynb cell 3).
 

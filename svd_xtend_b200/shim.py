@@ -1,4 +1,4 @@
-"""Launcher shim: run the reference's training scripts UNCHANGED on the B200 path.
+"""Launcher shim: run the reference's training scripts UNCHANGED on the H100 path.
 
     python -m svd_xtend_b200.shim train_svd.py --pretrained_model_name_or_path=... [script args]
     accelerate launch -m svd_xtend_b200.shim train_svd.py ...

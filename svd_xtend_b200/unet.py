@@ -1,4 +1,4 @@
-"""Drop-in `UNetSpatioTemporalConditionModel` for pixeli99/SVD_Xtend on B200.
+"""Drop-in `UNetSpatioTemporalConditionModel` for pixeli99/SVD_Xtend on H100.
 
 Host-side mirror of /root/reference/src/unet_spatio_temporal_condition.py (class at :32, forward
 signature at :357-364, attention-processor plugin API at :248-321, gradient-checkpointing flag at
@@ -7,7 +7,7 @@ signature at :357-364, attention-processor plugin API at :248-321, gradient-chec
 names (so `from_pretrained` state dicts, the `'temporal_transformer_block' in name` filter of
 train_svd.py:761-766 and PEFT's target matching at train_svd_lora.py:659-664 all work unchanged);
 the arithmetic never goes through `nn.Module.forward` of those holders — `forward()` below drives
-the sm_100a kernels through `engine.Engine` (token-major channels-last bf16, hand-rolled tape).
+the sm_90a kernels through `engine.Engine` (token-major channels-last bf16, hand-rolled tape).
 There is no PyTorch/CPU fallback: without the native library or a CUDA device forward raises.
 """
 from __future__ import annotations
@@ -36,19 +36,19 @@ class TimestepEmbedding(nn.Module):
 
 
 class SvdxAttnProcessor:
-    """The attention 'processor' of this build: tcgen05 flash attention for self-attention and the exact
+    """The attention 'processor' of this build: wgmma flash attention for self-attention and the exact
     1-key collapse for the image cross-attention. Kept as an object so that the reference's
     `attn_processors` / `set_attn_processor` API (src/unet_spatio_temporal_condition.py:248-308) round-trips."""
 
     def __repr__(self):
-        return "SvdxAttnProcessor(sm_100a)"
+        return "SvdxAttnProcessor(sm_90a)"
 
 
 # Processors whose arithmetic IS plain scaled-dot-product attention (softmax(q k^T / sqrt(d)) v followed by to_out): the
 # diffusers classes the reference can install — `AttnProcessor()` by set_default_attn_processor
 # (src/unet_spatio_temporal_condition.py:310-321), `AttnProcessor2_0` (the constructor default [D]) and
 # `XFormersAttnProcessor` (enable_xformers_memory_efficient_attention, train_svd.py:681-693). Setting one of them keeps the
-# object (the dict API round-trips) and the sm_100a kernel computes the same function. Any OTHER processor would change
+# object (the dict API round-trips) and the sm_90a kernel computes the same function. Any OTHER processor would change
 # the arithmetic (the reference calls it, :276-308); it cannot run on this path, so it is rejected instead of being
 # silently ignored.
 _SDPA_EQUIVALENT_PROCESSORS = ("SvdxAttnProcessor", "AttnProcessor", "AttnProcessor2_0", "XFormersAttnProcessor")
@@ -58,7 +58,7 @@ def _check_processor(processor):
     name = type(processor).__name__
     if name not in _SDPA_EQUIVALENT_PROCESSORS:
         raise ValueError(
-            f"svd_xtend_b200: attention processor {name!r} is not supported — the B200 path computes plain scaled-dot-product "
+            f"svd_xtend_b200: attention processor {name!r} is not supported — the H100 path computes plain scaled-dot-product "
             f"attention in one fused kernel and cannot call a custom processor; accepted (arithmetically identical): "
             f"{', '.join(_SDPA_EQUIVALENT_PROCESSORS)}")
     return processor
@@ -368,7 +368,7 @@ class _Config(SimpleNamespace):
 
 
 class UNetSpatioTemporalConditionModel(nn.Module):
-    """B200-native replacement with the constructor, attributes and forward of
+    """H100-native replacement with the constructor, attributes and forward of
     src/unet_spatio_temporal_condition.py:32-490."""
 
     _supports_gradient_checkpointing = True  # :68
@@ -544,7 +544,7 @@ class UNetSpatioTemporalConditionModel(nn.Module):
             rec(name, module, processor)
 
     def set_default_attn_processor(self):
-        """:310-321 — the default processor of this build is the sm_100a one."""
+        """:310-321 — the default processor of this build is the sm_90a one."""
         self.set_attn_processor(SvdxAttnProcessor())
 
     def _set_gradient_checkpointing(self, module, value=False):
@@ -652,7 +652,7 @@ class UNetSpatioTemporalConditionModel(nn.Module):
                 added_time_ids: torch.Tensor, return_dict: bool = True):
         """Same contract as src/unet_spatio_temporal_condition.py:357-490."""
         if not sample.is_cuda:
-            raise RuntimeError("svd_xtend_b200: the UNet hot path only runs on a CUDA (sm_100a) device; there is no CPU fallback")
+            raise RuntimeError("svd_xtend_b200: the UNet hot path only runs on a CUDA (sm_90a) device; there is no CPU fallback")
         self._validate(sample)
         timesteps = timestep
         if not torch.is_tensor(timesteps):

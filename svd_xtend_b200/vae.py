@@ -1,11 +1,11 @@
-"""`AutoencoderKLTemporalDecoder.encode` on B200 — SURVEY.md §8f-1: the VAE encode that sits on the critical path of every
+"""`AutoencoderKLTemporalDecoder.encode` on H100 — SURVEY.md §8f-1: the VAE encode that sits on the critical path of every
 training step of the reference (`tensor_to_vae_latent`, /root/reference/train_svd.py:283-291, called at :948 for the clip and
 at :959 for the noise-augmented conditioning frame):
 
     latents = vae.encode(frames).latent_dist.sample() * vae.config.scaling_factor
 
 Same kernels as the UNet (one channels-last bf16 token matrix for the whole encoder): 3x3 convolutions as tap-shifted TMA
-boxes on tcgen05 (`svdx_tapgemm`, here also for images wider than one 128-pixel tile: 320x512 frames), GroupNorm statistics
+boxes on wgmma (`svdx_tapgemm`, here also for images wider than one 128-pixel tile: 320x512 frames), GroupNorm statistics
 fused into the producing conv epilogue, GroupNorm+SiLU apply, the stride-2 convs over parity planes (the VAE's
 pad-(0,1,0,1) form), and the mid block's single-head dim-512 attention as QK^T / row-softmax / PV GEMMs (its S x S score
 matrix is small). Forward only: the VAE is frozen (`vae.requires_grad_(False)`, train_svd.py:659) — gradients are refused.
@@ -151,7 +151,7 @@ class AutoencoderKLTemporalDecoder(nn.Module):
     def encode(self, x: torch.Tensor, return_dict: bool = True):
         """x [N, 3, H, W] (H, W multiples of 2^(levels-1); W | 128 or 128 | W at every level) -> object with `.latent_dist`"""
         if not x.is_cuda:
-            raise RuntimeError("svd_xtend_b200: the VAE encode path only runs on a CUDA (sm_100a) device; there is no CPU fallback")
+            raise RuntimeError("svd_xtend_b200: the VAE encode path only runs on a CUDA (sm_90a) device; there is no CPU fallback")
         if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
             raise RuntimeError("svd_xtend_b200: AutoencoderKLTemporalDecoder.encode is forward-only (the reference freezes the VAE, "
                                "train_svd.py:659); call vae.requires_grad_(False) / use torch.no_grad()")

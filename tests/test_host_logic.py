@@ -87,7 +87,7 @@ def test_tile_selection_and_geometry():
 def test_shim_installs_the_replacement_under_both_reference_import_paths(monkeypatch):
     """svd_xtend_b200.shim.install(): `from diffusers import UNetSpatioTemporalConditionModel` (train_svd.py:49) and
     `from src.unet_spatio_temporal_condition import UNetSpatioTemporalConditionModel` (train_svd_lora.py:60) must both
-    resolve to the B200 class. diffusers is absent here, so a stand-in package plays its role."""
+    resolve to the H100 class. diffusers is absent here, so a stand-in package plays its role."""
     import importlib
     import sys
     import types
@@ -122,8 +122,8 @@ def test_shim_fails_loudly_without_diffusers(monkeypatch):
 
 
 def test_wide_tile_rule():
-    """256x320 CTA-pair tiles: only where the alternative is 160-wide tiles, the contraction is long, and the launch has the
-    bf16 TMA-store epilogue (raw._wide_tile_ok mirrors the library's conditions; profiles/r2_kbench_gemm.txt)"""
+    """320-wide tile requests: only where the alternative is 160-wide tiles, the contraction is long, and the launch has the
+    bf16 TMA-store epilogue (raw._wide_tile_ok mirrors the library's conditions)"""
     from svd_xtend_b200 import raw
     bf16 = torch.bfloat16
     out = torch.empty(1024, 640, dtype=bf16)
@@ -132,7 +132,7 @@ def test_wide_tile_rule():
     assert raw._wide_tile_ok(35840, 320, 2880, torch.empty(8, 320, dtype=bf16), **common)
     assert not raw._wide_tile_ok(1024, 640, 640, out, **common)                       # short contraction
     assert not raw._wide_tile_ok(1024, 1280, 5120, torch.empty(8, 1280, dtype=bf16), **common)   # 256-wide tiles divide N
-    assert not raw._wide_tile_ok(256, 640, 2560, out, **common)                        # small M: 1-CTA kernel
+    assert not raw._wide_tile_ok(256, 640, 2560, out, **common)                        # small M
     assert not raw._wide_tile_ok(1024, 480, 2560, torch.empty(8, 480, dtype=bf16), **common)     # N % 320
     assert not raw._wide_tile_ok(1024, 640, 2560, torch.empty(8, 640), **common)       # fp32 output
     assert not raw._wide_tile_ok(1024, 640, 2560, out, **{**common, "geglu": True})

@@ -1,5 +1,5 @@
 """Inference path (SURVEY.md §8f-3, UNet-facing part): Euler / classifier-free-guidance sampling loop around the forward-only
-B200 UNet against the oracle restatement of diffusers' StableVideoDiffusionPipeline loop (oracle/svd_sampling_oracle.py)."""
+H100 UNet against the oracle restatement of diffusers' StableVideoDiffusionPipeline loop (oracle/svd_sampling_oracle.py)."""
 import pytest
 import torch
 

@@ -1,4 +1,4 @@
-"""SURVEY.md §8f-1 — VAE encode (train_svd.py:283-291, :948, :959) on the B200 path against the oracle restatement of
+"""SURVEY.md §8f-1 — VAE encode (train_svd.py:283-291, :948, :959) on the H100 path against the oracle restatement of
 diffusers' AutoencoderKLTemporalDecoder.encode (oracle/svd_vae_oracle.py). Tolerance as for the UNet: rel-L2 of the moments
 <= max(2 x err(oracle under torch bf16 autocast), 2e-2) against the fp32 oracle."""
 import pytest
