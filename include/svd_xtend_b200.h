@@ -131,6 +131,15 @@ typedef struct SvdxTapGemm {
   float* gnb_sum;
   int32_t gnb_rows;
   int32_t gnb_silu;
+  /* Interleaved store: the phase form of Upsample2D [D] (nearest 2x upsample, then a 3x3 conv with padding 1), which is four
+   * 2x2-tap convolutions on the LOW-RES input, one per output parity (phase_h, phase_w). When interleave != 0 (CONV2D mode),
+   * output row (n, h, w) of the low-res geometry {W, H, nimg} is written to row (n*2H + 2h + phase_h) * 2W + 2w + phase_w of
+   * the [nimg][2H][2W][ldo] high-res output, so the four launches fill it without the upsampled input ever existing.
+   * gn_sum slabs still count low-res rows (gn_rows = H*W: the four phases of a frame accumulate into one slab).
+   * Requires the plain bf16 TMA-store epilogue (bias only: no rowbias / residual / scales / GEGLU / split-K / gnb sums) and
+   * whole images per 32-row store chunk (W >= 32, or H*W % 32 == 0). */
+  int32_t interleave;
+  int32_t phase_h, phase_w;
 } SvdxTapGemm;
 
 int svdx_tapgemm(const SvdxTapGemm* desc, void* stream);
@@ -268,6 +277,13 @@ int svdx_nchw_to_nhwc(const void* src, int32_t src_bf16, void* dst, int32_t N, i
                       int32_t c_pad, void* stream);
 int svdx_nhwc_to_nchw(const void* src, int64_t lds, void* dst, int32_t dst_bf16, int32_t N, int32_t C, int32_t H,
                       int32_t W, void* stream);
+/* The temporal VAE decoder's tail [D: TemporalDecoder.time_conv_out]: a Conv3d(C, C, (3,1,1), padding (1,0,0)) over the frames
+ * of each clip (zero frames past the clip edges), fused with the token-major -> NCHW conversion and the output cast:
+ *   y[n][o][p] = bias[o] + sum_{i, k} w[(o*C + i)*3 + k] * x[(n + k - 1) * H*W + p][i]      (clip b = n / T, n + k - 1 in clip b)
+ * x: fp32 [N*H*W][ldx] (the conv_out output, ldx % 4 == 0, 16-byte aligned, ldx >= C rounded up to 4), C <= 8, N = B*T;
+ * w fp32 [C][C][3], bias fp32 [C] or NULL; y NCHW [N][C][H][W] of dtype code y_dtype (0 fp32, 1 bf16, 2 fp16). One pass. */
+int svdx_time_conv_out(const float* x, int64_t ldx, int32_t N, int32_t T, int32_t C, int32_t H, int32_t W, const float* w,
+                       const float* bias, void* y, int32_t y_dtype, void* stream);
 /* nearest 2x upsample, channels-last (F.interpolate of Upsample2D [D]) and its adjoint (2x2 sum) */
 int svdx_upsample2x(const void* src, void* dst, int32_t N, int32_t H, int32_t W, int32_t C, void* stream);
 int svdx_upsample2x_bwd(const void* dsrc, void* ddst, int32_t N, int32_t H, int32_t W, int32_t C, void* stream);

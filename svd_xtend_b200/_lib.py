@@ -38,6 +38,7 @@ class SvdxTapGemm(C.Structure):
         ("gn_sum", c_void_p), ("gn_ld", c_i64), ("gn_rows", c_int),
         ("gnb_x", c_void_p), ("gnb_ldx", c_i64), ("gnb_x2", c_void_p), ("gnb_ldx2", c_i64), ("gnb_c1", c_int),
         ("gnb_ab", c_void_p), ("gnb_sum", c_void_p), ("gnb_rows", c_int), ("gnb_silu", c_int),
+        ("interleave", c_int), ("phase_h", c_int), ("phase_w", c_int),
     ]
 
 
@@ -92,6 +93,7 @@ _PROTOS = {
     "svdx_cast_f16_f32": [c_void_p, c_void_p, c_i64, c_void_p],
     "svdx_nchw_to_nhwc": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "svdx_nhwc_to_nchw": [c_void_p, c_i64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
+    "svdx_time_conv_out": [c_void_p, c_i64, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p],
     "svdx_upsample2x": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     "svdx_upsample2x_bwd": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     "svdx_space_to_planes": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],

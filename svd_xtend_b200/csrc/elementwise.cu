@@ -115,6 +115,58 @@ __global__ void nhwc_to_nchw_kernel(const bf16* __restrict__ src, long long lds,
   else dst[idx] = __float2bfloat16(v);
 }
 
+// time_conv_out: one thread per (clip, pixel) walks the clip's frames with a three-frame register window, so every input
+// row is read once; the C <= 8 outputs of a frame go to the NCHW planes (coalesced along the pixels of a warp).
+SVDX_DEVINL void ld_row8(const float* __restrict__ x, int nv4, float (&v)[8]) {
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const float4 q = j < nv4 ? __ldg(reinterpret_cast<const float4*>(x) + j) : make_float4(0.f, 0.f, 0.f, 0.f);
+    v[4 * j] = q.x; v[4 * j + 1] = q.y; v[4 * j + 2] = q.z; v[4 * j + 3] = q.w;
+  }
+}
+template <typename T>
+__global__ void time_conv_out_kernel(const float* __restrict__ x, long long ldx, int B, int frames, int C, long long HW,
+                                     const float* __restrict__ w, const float* __restrict__ bias, T* __restrict__ y) {
+  __shared__ float sw[8 * 8 * 3], sb[8];
+  for (int i = threadIdx.x; i < C * C * 3; i += blockDim.x) sw[i] = w[i];
+  if (threadIdx.x < 8) sb[threadIdx.x] = (bias && (int)threadIdx.x < C) ? bias[threadIdx.x] : 0.f;
+  __syncthreads();
+  const long long idx = gtid();
+  if (idx >= (long long)B * HW) return;
+  const int b = (int)(idx / HW);
+  const long long p = idx - (long long)b * HW;
+  const int nv4 = (C + 3) / 4;
+  const long long n0 = (long long)b * frames;
+  float prev[8], cur[8], next[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) prev[i] = 0.f;
+  ld_row8(x + (n0 * HW + p) * ldx, nv4, cur);
+  for (int t = 0; t < frames; ++t) {
+    if (t + 1 < frames) ld_row8(x + ((n0 + t + 1) * HW + p) * ldx, nv4, next);
+    else {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) next[i] = 0.f;
+    }
+    T* yo = y + (n0 + t) * C * HW + p;
+#pragma unroll
+    for (int o = 0; o < 8; ++o) {
+      if (o >= C) break;
+      float acc = sb[o];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        if (i >= C) break;
+        const float* wo = sw + (o * C + i) * 3;
+        acc = fmaf(wo[0], prev[i], fmaf(wo[1], cur[i], fmaf(wo[2], next[i], acc)));
+      }
+      if constexpr (sizeof(T) == 4) yo[o * HW] = acc;
+      else if constexpr (std::is_same<T, __half>::value) yo[o * HW] = __float2half(acc);
+      else yo[o * HW] = __float2bfloat16(acc);
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { prev[i] = cur[i]; cur[i] = next[i]; }
+  }
+}
+
 // nearest 2x: dst[n][2h+a][2w+b][:] = src[n][h][w][:]   (16 B vectors)
 __global__ void upsample2x_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, int N, int H, int W, int CV) {
   const long long idx = gtid();
@@ -791,6 +843,20 @@ extern "C" int svdx_nchw_to_nhwc(const void* src, int32_t src_bf16, void* dst, i
   else if (src_bf16 == 2) nchw_to_nhwc_kernel<__half><<<nblocks(total), 256, 0, ST(stream)>>>(reinterpret_cast<const __half*>(src), reinterpret_cast<bf16*>(dst), N, C, H, W, c_pad);
   else nchw_to_nhwc_kernel<float><<<nblocks(total), 256, 0, ST(stream)>>>(reinterpret_cast<const float*>(src), reinterpret_cast<bf16*>(dst), N, C, H, W, c_pad);
   SVDX_CHECK_LAUNCH("nchw_to_nhwc");
+  return SVDX_OK;
+}
+extern "C" int svdx_time_conv_out(const float* x, int64_t ldx, int32_t N, int32_t T, int32_t C, int32_t H, int32_t W, const float* w,
+                                  const float* bias, void* y, int32_t y_dtype, void* stream) {
+  if (!x || !w || !y || N <= 0 || T <= 0 || N % T || C <= 0 || C > 8 || H <= 0 || W <= 0 || y_dtype < 0 || y_dtype > 2 ||
+      ldx % 4 || ldx < (C + 3) / 4 * 4 || (reinterpret_cast<uintptr_t>(x) & 15))
+    return svdx_fail(SVDX_E_BADARG, "time_conv_out: bad arguments (N = B*T, 1 <= C <= 8, fp32 rows 16-byte aligned with ldx %% 4 == 0)");
+  const int B = N / T;
+  const long long HW = (long long)H * W;
+  const long long total = (long long)B * HW;
+  if (y_dtype == 1) time_conv_out_kernel<bf16><<<nblocks(total), 256, 0, ST(stream)>>>(x, ldx, B, T, C, HW, w, bias, reinterpret_cast<bf16*>(y));
+  else if (y_dtype == 2) time_conv_out_kernel<__half><<<nblocks(total), 256, 0, ST(stream)>>>(x, ldx, B, T, C, HW, w, bias, reinterpret_cast<__half*>(y));
+  else time_conv_out_kernel<float><<<nblocks(total), 256, 0, ST(stream)>>>(x, ldx, B, T, C, HW, w, bias, reinterpret_cast<float*>(y));
+  SVDX_CHECK_LAUNCH("time_conv_out");
   return SVDX_OK;
 }
 extern "C" int svdx_nhwc_to_nchw(const void* src, int64_t lds, void* dst, int32_t dst_bf16, int32_t N, int32_t C, int32_t H, int32_t W,

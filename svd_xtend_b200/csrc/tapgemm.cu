@@ -349,6 +349,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
       else tile_mainloop_bn<0, 0>(p.block_n, kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase);
       named_bar_sync(1, 32 * NUM_EPI_WARPS);
       if constexpr (EPI == EPI_FAST || EPI == EPI_FAST_GN) epilogue_fast<EPI == EPI_FAST_GN>(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, st.base, st.row0, st.grp, lane, m0, valid_rows);
+      else if constexpr (EPI == EPI_FAST_IL || EPI == EPI_FAST_IL_GN) epilogue_fast<EPI == EPI_FAST_IL_GN, true>(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, st.base, st.row0, st.grp, lane, m0, valid_rows);
       else if constexpr (EPI == EPI_RES || EPI == EPI_RES_GN) epilogue_res<EPI == EPI_RES_GN>(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, s_acc, s_r1, s_r2, st.base, st.off, st.row0, st.grp, lane, m0, valid_rows);
       else if constexpr (EPI == EPI_GEGLU) epilogue_geglu(p, t_base, n0, half, bn_out, st.base, st.row0, st.grp, lane);
       else if constexpr (EPI == EPI_FAST_GNB) epilogue_fast_gnb(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, st.base, st.row0, st.grp, lane, m0, valid_rows);
@@ -553,10 +554,30 @@ int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p) {
       return svdx_fail(SVDX_E_BADARG, "tapgemm: gnb operands (x rows 16-byte aligned, gnb_rows > 0, scale/shift table for SiLU, concat split % 32)");
     p.epi_mode = EPI_FAST_GNB;
   }
-  if (wide320 && p.epi_mode != EPI_FAST && p.epi_mode != EPI_RES && p.epi_mode != EPI_FAST_GNB)
+  if (d->interleave) {
+    // phase (phase_h, phase_w) of a nearest-2x upsample + conv: the low-res output pixels land on every second row / column of
+    // the [nimg][2H][2W] output, through the 4-D view {n_out, W, H, nimg} with strides {2, 4W, 4HW} output rows
+    if (d->a_mode != SVDX_A_CONV2D || d->a_major_mn || d->b_major_mn || (d->phase_h & ~1) || (d->phase_w & ~1))
+      return svdx_fail(SVDX_E_BADARG, "tapgemm: interleave needs CONV2D mode and phases in {0, 1}");
+    if (p.epi_mode != EPI_FAST || p.rowbias || p.split_k > 1 || p.gnb_sum)
+      return svdx_fail(SVDX_E_BADARG, "tapgemm: interleave needs the plain bf16 TMA-store epilogue (bias only: no rowbias / residual / "
+                                      "scales / GEGLU / split-K / gnb sums; N %% 32 == 0, aligned rows)");
+    if (p.W < 32 && (32 % p.W || (p.H * p.W) % 32))
+      return svdx_fail(SVDX_E_BADARG, "tapgemm: interleave with W < 32 needs H*W %% 32 == 0 (a store chunk must not straddle images)");
+    const uint64_t rb = (uint64_t)d->ldo * 2;   // bytes per output row
+    uint64_t dims[4] = {(uint64_t)n_out, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.nimg};
+    uint64_t strides[3] = {2 * rb, 4 * (uint64_t)p.W * rb, 4 * (uint64_t)p.W * p.H * rb};
+    uint32_t box[4] = {32, (uint32_t)(p.W < 32 ? p.W : 32), (uint32_t)(p.W < 32 ? 32 / p.W : 1), 1};
+    const bf16* base = reinterpret_cast<const bf16*>(d->out) + (2LL * p.W * d->phase_h + d->phase_w) * d->ldo;
+    rc = svdx_make_tmap_ex(&p.tmo, base, 0, 64, 4, dims, strides, box);
+    if (rc) return rc;
+    p.interleave = 1;
+    p.epi_mode = EPI_FAST_IL;
+  }
+  if (wide320 && p.epi_mode != EPI_FAST && p.epi_mode != EPI_RES && p.epi_mode != EPI_FAST_GNB && p.epi_mode != EPI_FAST_IL)
     return svdx_fail(SVDX_E_BADARG, "tapgemm: block_n 320 needs a bf16 output through the TMA-store epilogues (N % 320 == 0, aligned rows)");
   if (p.gn_sum) {
-    if (p.epi_mode != EPI_FAST && p.epi_mode != EPI_RES)
+    if (p.epi_mode != EPI_FAST && p.epi_mode != EPI_RES && p.epi_mode != EPI_FAST_IL)
       return svdx_fail(SVDX_E_BADARG, "tapgemm: gn_sum needs a bf16 output through the TMA-store epilogues (N % 32 == 0, aligned rows), no split-K / GEGLU");
     if (p.gn_rows <= 0 || p.gn_ld < n_out || (p.gn_ld & 1) || (reinterpret_cast<uintptr_t>(p.gn_sum) & 7))
       return svdx_fail(SVDX_E_BADARG, "tapgemm: gn_sum needs gn_rows > 0, even gn_ld >= N, 8-byte aligned buffer");
@@ -586,13 +607,17 @@ extern "C" int svdx_tapgemm(const SvdxTapGemm* d, void* stream_v) {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_FAST_GN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_RES_GN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_FAST_GNB>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_FAST_IL>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_FAST_IL_GN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e != cudaSuccess) return svdx_fail_cuda(e, "tapgemm: set smem attribute");
     attr_done[slot] = true;
   }
   const int total_tiles = p.m_tiles * p.n_tiles * p.split_k;
   int grid = svdx_num_sms();
   if (grid > total_tiles) grid = total_tiles;
-  if (p.epi_mode == EPI_FAST_GNB) tapgemm_kernel<EPI_FAST_GNB><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
+  if (p.epi_mode == EPI_FAST_IL && p.gn_sum) tapgemm_kernel<EPI_FAST_IL_GN><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
+  else if (p.epi_mode == EPI_FAST_IL) tapgemm_kernel<EPI_FAST_IL><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
+  else if (p.epi_mode == EPI_FAST_GNB) tapgemm_kernel<EPI_FAST_GNB><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
   else if (p.epi_mode == EPI_FAST && p.gn_sum) tapgemm_kernel<EPI_FAST_GN><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
   else if (p.epi_mode == EPI_RES && p.gn_sum) tapgemm_kernel<EPI_RES_GN><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
   else if (p.epi_mode == EPI_FAST) tapgemm_kernel<EPI_FAST><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);

@@ -70,6 +70,7 @@ struct __align__(64) TapGemmKParams {
   int tma_store;       // epilogue stores through shared memory + TMA (tmo / tmpre valid)
   int epi_mode;        // EPI_GENERIC / EPI_FAST / EPI_GEGLU / EPI_RES: which kernel instantiation runs
   int probe;   // dev switch SVDX_EPI_PROBE: 1 = epilogue without global stores, 2 = no epilogue work at all
+  int interleave;      // tmo is the 4-D phase view {n_out, W, H, nimg} of a 2x-upsampled output (EPI_FAST_IL*)
 };
 
 
@@ -215,6 +216,20 @@ constexpr int EPI_GENERIC = 0, EPI_FAST = 1, EPI_GEGLU = 2, EPI_RES = 3;
 constexpr int EPI_FAST_GN = 4, EPI_RES_GN = 5;
 // + fused GroupNorm BACKWARD sums (the output is the gradient of a GroupNorm's output)
 constexpr int EPI_FAST_GNB = 6;
+// plain epilogue with the interleaved (upsample phase) store, without / with fused GroupNorm statistics
+constexpr int EPI_FAST_IL = 7, EPI_FAST_IL_GN = 8;
+
+// TMA store of one staged 32-row chunk whose first row is row0 of group grp. Interleaved: the chunk is 32 consecutive pixels
+// of the low-res geometry, addressed through the 4-D phase view {column, w, h, image} (whole images per chunk: checked on the host).
+template <bool IL>
+SVDX_DEVINL void store_chunk(const TapGemmKParams& p, uint32_t src, int col, int row0, int grp) {
+  if constexpr (IL) {
+    const int w0 = row0 % p.W, r = row0 / p.W;
+    tma_store_4d(&p.tmo, src, col, w0, r % p.H, r / p.H);
+  } else {
+    tma_store_3d(&p.tmo, src, col, row0, grp);
+  }
+}
 
 SVDX_DEVINL void add_vec32(float (&f)[32], const float* __restrict__ src) {
   const float4* bp = reinterpret_cast<const float4*>(src);
@@ -267,8 +282,8 @@ SVDX_DEVINL void prefetch_epilogue_operands(const TapGemmKParams& p, int epi, lo
 }
 
 // plain epilogue (bias / row-bias only): two 32-column chunks per round (both staging halves), one proxy fence and one
-// bulk group per round.
-template <bool GN>
+// bulk group per round. IL: interleaved (upsample phase) store.
+template <bool GN, bool IL = false>
 SVDX_DEVINL void epilogue_fast(const TapGemmKParams& p, uint32_t t_base, long long m, bool row_ok, int n0, int half, int c_lo, int c_hi,
                                int n_out_total, uint32_t sbase, int row0, int grp, int lane, long long m0, int valid_rows) {
   const float* bias = p.bias;
@@ -296,8 +311,8 @@ SVDX_DEVINL void epilogue_fast(const TapGemmKParams& p, uint32_t t_base, long lo
     fence_proxy_async_smem();
     __syncwarp();
     if (lane == 0) {
-      tma_store_3d(&p.tmo, sbase, colA, row0, grp);
-      if (hasB) tma_store_3d(&p.tmo, sbase + 2048, colB, row0, grp);
+      store_chunk<IL>(p, sbase, colA, row0, grp);
+      if (hasB) store_chunk<IL>(p, sbase + 2048, colB, row0, grp);
       bulk_commit();
     }
     if constexpr (GN) {

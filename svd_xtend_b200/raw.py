@@ -210,10 +210,13 @@ def tapgemm(
     gn_sum: Optional[torch.Tensor] = None,
     gn_rows: int = 0,
     gnb: Optional[dict] = None,
+    phase: Optional[Sequence[int]] = None,
 ) -> torch.Tensor:
     """Launch svdx_tapgemm on the current stream. All tensors are CUDA; a/b/res/pre are bf16.
     gn_sum: zeroed fp32 [slabs, 2, C] buffer that receives the per-channel sum / sum of squares of the output (fused
-    GroupNorm statistics), one slab per gn_rows output rows."""
+    GroupNorm statistics), one slab per gn_rows output rows.
+    phase: (ph, pw) — interleaved store of one output parity of a 2x-upsampled conv (CONV2D mode): low-res row (n, h, w) of
+    conv_whn goes to row (n*2H + 2h + ph)*2W + 2w + pw of `out` ([nimg*2H*2W, ldo])."""
     family = "conv" if (mode == A_CONV2D or len(taps) > 1 or b_mode != 0) else "linear"
     if _fam(family, 2.0 * M * N * K * len(taps)):
         return out
@@ -296,6 +299,9 @@ def tapgemm(
         d.gnb_sum = gnb["sum"].data_ptr()
         d.gnb_rows = gnb["rows"]
         d.gnb_silu = int(gnb["silu"])
+    if phase is not None:
+        d.interleave = 1
+        d.phase_h, d.phase_w = int(phase[0]), int(phase[1])
     check(load().svdx_tapgemm(C.byref(d), _stream()), "svdx_tapgemm")
     return out
 
@@ -538,6 +544,24 @@ def nhwc_to_nchw(src, dst, N, Cc, H, W):
     check(load().svdx_nhwc_to_nchw(src.data_ptr(), _rowmajor(src, "src"), dst.data_ptr(), dtype_code(dst, "NCHW output"), N, Cc, H, W, _stream()),
           "nhwc_to_nchw")
     return dst
+
+
+def time_conv_out(x, weight, bias, out, T):
+    """the temporal VAE decoder's tail: Conv3d(C, C, (3,1,1), padding (1,0,0)) over clips of T frames of the fp32 token-major
+    x [N*H*W, ldx] (C <= 8 valid columns), written to the NCHW `out` [N, C, H, W] (fp32 / bf16 / fp16) in one pass.
+    weight: fp32 with C*C*3 elements in [C][C][3] order (a contiguous Conv3d weight), bias fp32 [C] or None"""
+    N, Cc, H, W = out.shape
+    if weight.dtype != torch.float32 or not weight.is_contiguous() or weight.numel() != Cc * Cc * 3:
+        raise ValueError("time_conv_out: weight must be a contiguous fp32 [C, C, 3(, 1, 1)] tensor")
+    if bias is not None and (bias.dtype != torch.float32 or bias.numel() != Cc):
+        raise ValueError("time_conv_out: bias must be fp32 [C]")
+    if x.dtype != torch.float32 or x.shape[0] != N * H * W:
+        raise ValueError("time_conv_out: x must be fp32 [N*H*W, ldx]")
+    if _fam("elementwise", 2.0 * 3 * Cc * Cc * out.numel(), 4.0 * x.shape[0] * Cc + out.element_size() * out.numel()):
+        return out
+    check(load().svdx_time_conv_out(x.data_ptr(), _rowmajor(x, "x"), N, T, Cc, H, W, weight.data_ptr(), _ptr(bias), out.data_ptr(),
+                                    dtype_code(out, "time_conv_out output"), _stream()), "svdx_time_conv_out")
+    return out
 
 
 def upsample2x(src, dst, N, H, W, Cc):

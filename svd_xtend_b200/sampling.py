@@ -9,8 +9,9 @@ CUDA graph replays all `num_inference_steps` steps; between replays the host onl
 
 Scheduler constants follow diffusers' EulerDiscreteScheduler in the SVD configuration [D] (Karras sigmas, rho 7, sigma in
 [0.002, 700], timesteps 0.25 ln sigma, init_noise_sigma sqrt(sigma_max^2 + 1)); tests/test_sampling_gpu.py checks the loop
-against oracle/svd_sampling_oracle.py. Out of scope here: VAE encode / decode and the CLIP image encoder (SURVEY.md §8f-1/-4) —
-`image_latents` and `image_embeddings` are inputs, denoised latents are the output.
+against oracle/svd_sampling_oracle.py. `image_latents` and `image_embeddings` are inputs (the VAE encode lives in vae.py, the CLIP
+image encoder is out of scope), denoised latents are the output; `decode_latents` turns them into frames with the temporal VAE
+decoder (`vae.AutoencoderKLTemporalDecoder(with_decoder=True)`), chunk by chunk like the pipeline.
 """
 from __future__ import annotations
 
@@ -117,3 +118,21 @@ class VideoLatentSampler:
         out = st["latents"].clone()
         torch.cuda.current_stream().synchronize()      # `host` must outlive the queued copies
         return out
+
+
+@torch.no_grad()
+def decode_latents(vae, latents: torch.Tensor, decode_chunk_size: Optional[int] = None) -> torch.Tensor:
+    """[D] StableVideoDiffusionPipeline.decode_latents: latents [B, F, 4, h, w] (as the sampler returns them) -> frames
+    [B, 3, F, H, W] fp32 in [-1, 1] scale. The B*F frames are unscaled (1 / scaling_factor) and decoded decode_chunk_size at a
+    time (default F); every chunk is its own clip for the temporal layers (14 frames in chunks of 8 decode as 8 + 6)."""
+    b, f = latents.shape[:2]
+    chunk = f if decode_chunk_size is None else int(decode_chunk_size)
+    if chunk < 1:
+        raise ValueError("decode_chunk_size must be >= 1")
+    lat = latents.flatten(0, 1) * (1.0 / vae.config.scaling_factor)
+    frames = []
+    for i in range(0, lat.shape[0], chunk):
+        part = lat[i:i + chunk]
+        frames.append(vae.decode(part, num_frames=part.shape[0]).sample)
+    frames = torch.cat(frames, dim=0)
+    return frames.reshape(-1, f, *frames.shape[1:]).permute(0, 2, 1, 3, 4).float()
