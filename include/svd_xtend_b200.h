@@ -140,7 +140,16 @@ typedef struct SvdxTapGemm {
    * whole images per 32-row store chunk (W >= 32, or H*W % 32 == 0). */
   int32_t interleave;
   int32_t phase_h, phase_w;
+  /* Activation epilogue (the MLP fc1 of the CLIP image encoder [transformers CLIPMLP]): out = act(acc + bias), bf16, with
+   * act = SVDX_ACT_GELU (erf form, gelu_erf_f) or SVDX_ACT_QUICK_GELU (x * sigmoid(1.702 x)); SVDX_ACT_NONE (0) = no activation.
+   * Requires the plain bf16 TMA-store epilogue (bias only: no rowbias / residual / scales / GEGLU / split-K / gn_sum / gnb sums /
+   * interleave; N % 32 == 0, 16-byte aligned rows). */
+  int32_t act;
 } SvdxTapGemm;
+
+#define SVDX_ACT_NONE 0
+#define SVDX_ACT_GELU 1
+#define SVDX_ACT_QUICK_GELU 2
 
 int svdx_tapgemm(const SvdxTapGemm* desc, void* stream);
 
@@ -252,6 +261,33 @@ typedef struct SvdxAttn {
 } SvdxAttn;
 int svdx_attention_fwd(const SvdxAttn* d, void* stream);
 int svdx_attention_bwd(const SvdxAttn* d, void* stream);
+
+/* Head dim 80, forward only: the self-attention of the CLIP ViT-H/14 image encoder [transformers CLIPAttention -> SDPA,
+ * 16 heads x 80, no mask]. Sequence s (0 <= s < nseq) is rows [s*S, s*S + S) of the token-major q / k / v / o matrices;
+ * head h uses columns [80h, 80h + 80) of each (column slices of the fused q|k|v GEMM output allowed):
+ *   o = softmax(scale * q k^T) v     over all S keys (any S >= 1), fp32 softmax, bf16 in / out.
+ * q/k/v: ld % 8 == 0, 16-byte aligned; o: even ld, 4-byte aligned. Rows of o outside [0, nseq*S) are never written. */
+int svdx_attention_hd80_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o,
+                            int64_t ldo, int32_t nseq, int32_t heads, int32_t S, float scale, void* stream);
+
+/* ------------------------------------------------------------------ CLIP image preprocessing
+ * The conditioning frame -> the A operand of the patch-embedding GEMM in one pass (train_svd.py:857-876 encode_image:
+ * _resize_with_antialiasing(x, (224, 224)) -> (x + 1) / 2 -> CLIPImageProcessor normalisation -> Conv2d(3, C, 14, stride 14)).
+ * x: contiguous NCHW [B][3][H][W] (x_strides = its 4 element strides, checked as torch defines contiguity: the stride of a
+ * size-1 dimension is ignored, so a batch-1 frame slice of a video is accepted), dtype code x_dtype (0 fp32, 1 bf16, 2 fp16).
+ * Per output pixel (oy, ox) of the out_size^2 image and channel c:
+ *   blurred(y, x) = sum_a gy[a] sum_b gx[b] x[c][refl(y + a - (ky-1)/2)][refl(x + b - (kx-1)/2)]    (reflect padding)
+ *   v = bicubic(blurred; A = -0.75, align_corners, border-clamped taps) at (oy * (H-1)/(out_size-1), ox * (W-1)/(out_size-1))
+ *   out = v * affine[c] + affine[3 + c]
+ * gy / gx: HOST arrays of ky / kx fp32 weights (odd sizes <= SVDX_CLIP_MAX_TAPS, (k-1)/2 < the dimension, as torch's reflect pad);
+ * affine: HOST float[6] {a_0, a_1, a_2, b_0, b_1, b_2}. All three are copied into the launch (graph-capturable).
+ * out: bf16 [B * (1 + P^2)][ldo], P = out_size / patch: row 0 of each image is all zero (the class-token slot), row 1 + py*P + px
+ * holds patch (py, px) with column c*patch^2 + ky*patch + kx (the conv weight's (c, kh, kw) order); columns [3*patch^2, Kp) are
+ * zero, Kp = 3*patch^2 rounded up to 64 (ldo >= Kp). ky = kx = 1 with H = W = out_size reproduces x exactly (rounded to bf16). */
+#define SVDX_CLIP_MAX_TAPS 63
+int svdx_clip_preprocess(const void* x, int32_t x_dtype, const int64_t* x_strides, int32_t B, int32_t H, int32_t W,
+                         const float* gy, int32_t ky, const float* gx, int32_t kx, const float* affine,
+                         int32_t out_size, int32_t patch, void* out, int64_t ldo, void* stream);
 
 /* ------------------------------------------------------------------ elementwise / layout */
 /* weights -> bf16, optionally re-laid-out. src_bf16 is the SOURCE DTYPE CODE used by every entry of this section:

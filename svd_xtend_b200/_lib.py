@@ -15,8 +15,10 @@ PKG = Path(__file__).resolve().parent
 LIB_PATH = Path(os.environ["SVDX_LIB"]) if os.environ.get("SVDX_LIB") else PKG / "lib" / "libsvdx_b200.so"
 
 SVDX_MAX_TAPS = 27
+SVDX_CLIP_MAX_TAPS = 63
 A_ROWS, A_CONV2D = 0, 1
 OUT_BF16, OUT_F32, OUT_F32_ATOMIC = 0, 1, 2
+ACT_NONE, ACT_GELU, ACT_QUICK_GELU = 0, 1, 2
 
 c_void_p, c_int, c_i64, c_float = C.c_void_p, C.c_int32, C.c_int64, C.c_float
 
@@ -39,6 +41,7 @@ class SvdxTapGemm(C.Structure):
         ("gnb_x", c_void_p), ("gnb_ldx", c_i64), ("gnb_x2", c_void_p), ("gnb_ldx2", c_i64), ("gnb_c1", c_int),
         ("gnb_ab", c_void_p), ("gnb_sum", c_void_p), ("gnb_rows", c_int), ("gnb_silu", c_int),
         ("interleave", c_int), ("phase_h", c_int), ("phase_w", c_int),
+        ("act", c_int),
     ]
 
 
@@ -84,6 +87,9 @@ _PROTOS = {
                            c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_void_p, c_void_p],
     "svdx_attention_fwd": [C.POINTER(SvdxAttn), c_void_p],
     "svdx_attention_bwd": [C.POINTER(SvdxAttn), c_void_p],
+    "svdx_attention_hd80_fwd": [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_int, c_int, c_int, c_float, c_void_p],
+    "svdx_clip_preprocess": [c_void_p, c_int, C.POINTER(c_i64), c_int, c_int, c_int, C.POINTER(c_float), c_int, C.POINTER(c_float), c_int,
+                             C.POINTER(c_float), c_int, c_int, c_void_p, c_i64, c_void_p],
     "svdx_prep_weight": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "svdx_unprep_conv_grad": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     "svdx_dot_diff": [c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_void_p],

@@ -350,6 +350,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
       named_bar_sync(1, 32 * NUM_EPI_WARPS);
       if constexpr (EPI == EPI_FAST || EPI == EPI_FAST_GN) epilogue_fast<EPI == EPI_FAST_GN>(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, st.base, st.row0, st.grp, lane, m0, valid_rows);
       else if constexpr (EPI == EPI_FAST_IL || EPI == EPI_FAST_IL_GN) epilogue_fast<EPI == EPI_FAST_IL_GN, true>(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, st.base, st.row0, st.grp, lane, m0, valid_rows);
+      else if constexpr (EPI == EPI_FAST_ACT) epilogue_fast<false, false, true>(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, st.base, st.row0, st.grp, lane, m0, valid_rows);
       else if constexpr (EPI == EPI_RES || EPI == EPI_RES_GN) epilogue_res<EPI == EPI_RES_GN>(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, s_acc, s_r1, s_r2, st.base, st.off, st.row0, st.grp, lane, m0, valid_rows);
       else if constexpr (EPI == EPI_GEGLU) epilogue_geglu(p, t_base, n0, half, bn_out, st.base, st.row0, st.grp, lane);
       else if constexpr (EPI == EPI_FAST_GNB) epilogue_fast_gnb(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, st.base, st.row0, st.grp, lane, m0, valid_rows);
@@ -574,7 +575,15 @@ int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p) {
     p.interleave = 1;
     p.epi_mode = EPI_FAST_IL;
   }
-  if (wide320 && p.epi_mode != EPI_FAST && p.epi_mode != EPI_RES && p.epi_mode != EPI_FAST_GNB && p.epi_mode != EPI_FAST_IL)
+  if (d->act != SVDX_ACT_NONE) {
+    if (d->act != SVDX_ACT_GELU && d->act != SVDX_ACT_QUICK_GELU) return svdx_fail(SVDX_E_BADARG, "tapgemm: act must be SVDX_ACT_GELU or SVDX_ACT_QUICK_GELU");
+    if (p.epi_mode != EPI_FAST || p.rowbias || p.split_k > 1 || p.gn_sum)
+      return svdx_fail(SVDX_E_BADARG, "tapgemm: act needs the plain bf16 TMA-store epilogue (bias only: no rowbias / residual / scales / "
+                                      "GEGLU / split-K / gn_sum / gnb sums / interleave; N %% 32 == 0, aligned rows)");
+    p.act = d->act;
+    p.epi_mode = EPI_FAST_ACT;
+  }
+  if (wide320 && p.epi_mode != EPI_FAST && p.epi_mode != EPI_RES && p.epi_mode != EPI_FAST_GNB && p.epi_mode != EPI_FAST_IL && p.epi_mode != EPI_FAST_ACT)
     return svdx_fail(SVDX_E_BADARG, "tapgemm: block_n 320 needs a bf16 output through the TMA-store epilogues (N % 320 == 0, aligned rows)");
   if (p.gn_sum) {
     if (p.epi_mode != EPI_FAST && p.epi_mode != EPI_RES && p.epi_mode != EPI_FAST_IL)
@@ -609,13 +618,15 @@ extern "C" int svdx_tapgemm(const SvdxTapGemm* d, void* stream_v) {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_FAST_GNB>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_FAST_IL>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_FAST_IL_GN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_FAST_ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e != cudaSuccess) return svdx_fail_cuda(e, "tapgemm: set smem attribute");
     attr_done[slot] = true;
   }
   const int total_tiles = p.m_tiles * p.n_tiles * p.split_k;
   int grid = svdx_num_sms();
   if (grid > total_tiles) grid = total_tiles;
-  if (p.epi_mode == EPI_FAST_IL && p.gn_sum) tapgemm_kernel<EPI_FAST_IL_GN><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
+  if (p.epi_mode == EPI_FAST_ACT) tapgemm_kernel<EPI_FAST_ACT><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
+  else if (p.epi_mode == EPI_FAST_IL && p.gn_sum) tapgemm_kernel<EPI_FAST_IL_GN><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
   else if (p.epi_mode == EPI_FAST_IL) tapgemm_kernel<EPI_FAST_IL><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
   else if (p.epi_mode == EPI_FAST_GNB) tapgemm_kernel<EPI_FAST_GNB><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
   else if (p.epi_mode == EPI_FAST && p.gn_sum) tapgemm_kernel<EPI_FAST_GN><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);

@@ -71,6 +71,7 @@ struct __align__(64) TapGemmKParams {
   int epi_mode;        // EPI_GENERIC / EPI_FAST / EPI_GEGLU / EPI_RES: which kernel instantiation runs
   int probe;   // dev switch SVDX_EPI_PROBE: 1 = epilogue without global stores, 2 = no epilogue work at all
   int interleave;      // tmo is the 4-D phase view {n_out, W, H, nimg} of a 2x-upsampled output (EPI_FAST_IL*)
+  int act;             // SVDX_ACT_GELU / SVDX_ACT_QUICK_GELU applied after the bias (EPI_FAST_ACT)
 };
 
 
@@ -218,6 +219,19 @@ constexpr int EPI_FAST_GN = 4, EPI_RES_GN = 5;
 constexpr int EPI_FAST_GNB = 6;
 // plain epilogue with the interleaved (upsample phase) store, without / with fused GroupNorm statistics
 constexpr int EPI_FAST_IL = 7, EPI_FAST_IL_GN = 8;
+// plain epilogue + activation (act(acc + bias)): its own instantiation, so the others keep their register budget
+constexpr int EPI_FAST_ACT = 9;
+
+// the activations of EPI_FAST_ACT: GELU (erf) and quick_gelu x * sigmoid(1.702 x)
+SVDX_DEVINL void act32(float (&f)[32], int act) {
+  if (act == SVDX_ACT_GELU) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) f[i] = gelu_erf_f(f[i]);
+  } else {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) f[i] = __fdividef(f[i], 1.0f + __expf(-1.702f * f[i]));
+  }
+}
 
 // TMA store of one staged 32-row chunk whose first row is row0 of group grp. Interleaved: the chunk is 32 consecutive pixels
 // of the low-res geometry, addressed through the 4-D phase view {column, w, h, image} (whole images per chunk: checked on the host).
@@ -282,8 +296,8 @@ SVDX_DEVINL void prefetch_epilogue_operands(const TapGemmKParams& p, int epi, lo
 }
 
 // plain epilogue (bias / row-bias only): two 32-column chunks per round (both staging halves), one proxy fence and one
-// bulk group per round. IL: interleaved (upsample phase) store.
-template <bool GN, bool IL = false>
+// bulk group per round. IL: interleaved (upsample phase) store. ACT: activation after the bias (p.act).
+template <bool GN, bool IL = false, bool ACT = false>
 SVDX_DEVINL void epilogue_fast(const TapGemmKParams& p, uint32_t t_base, long long m, bool row_ok, int n0, int half, int c_lo, int c_hi,
                                int n_out_total, uint32_t sbase, int row0, int grp, int lane, long long m0, int valid_rows) {
   const float* bias = p.bias;
@@ -304,6 +318,7 @@ SVDX_DEVINL void epilogue_fast(const TapGemmKParams& p, uint32_t t_base, long lo
     for (int i = 0; i < 32; ++i) { fa[i] = __uint_as_float(va[i]); fb[i] = __uint_as_float(vb[i]); }
     if (bias) { add_vec32(fa, bias + colA); if (hasB) add_vec32(fb, bias + colB); }
     if (rb) { add_vec32(fa, rb + colA); if (hasB) add_vec32(fb, rb + colB); }
+    if constexpr (ACT) { act32(fa, p.act); if (hasB) act32(fb, p.act); }
     if (lane == 0) bulk_wait_read<0>();   // the previous round's stores have drained both halves
     __syncwarp();
     stage_row_bf16(rowX, sw, fa);

@@ -8,7 +8,7 @@ from typing import Optional, Sequence
 import torch
 
 from . import _lib
-from ._lib import A_CONV2D, A_ROWS, OUT_BF16, OUT_F32, OUT_F32_ATOMIC, SvdxAttn, SvdxTapGemm, load
+from ._lib import ACT_GELU, ACT_NONE, ACT_QUICK_GELU, A_CONV2D, A_ROWS, OUT_BF16, OUT_F32, OUT_F32_ATOMIC, SvdxAttn, SvdxTapGemm, load
 
 bf16 = torch.bfloat16
 
@@ -211,12 +211,14 @@ def tapgemm(
     gn_rows: int = 0,
     gnb: Optional[dict] = None,
     phase: Optional[Sequence[int]] = None,
+    act: int = ACT_NONE,
 ) -> torch.Tensor:
     """Launch svdx_tapgemm on the current stream. All tensors are CUDA; a/b/res/pre are bf16.
     gn_sum: zeroed fp32 [slabs, 2, C] buffer that receives the per-channel sum / sum of squares of the output (fused
     GroupNorm statistics), one slab per gn_rows output rows.
     phase: (ph, pw) — interleaved store of one output parity of a 2x-upsampled conv (CONV2D mode): low-res row (n, h, w) of
-    conv_whn goes to row (n*2H + 2h + ph)*2W + 2w + pw of `out` ([nimg*2H*2W, ldo])."""
+    conv_whn goes to row (n*2H + 2h + ph)*2W + 2w + pw of `out` ([nimg*2H*2W, ldo]).
+    act: ACT_GELU / ACT_QUICK_GELU — out = act(acc + bias) (the plain bf16 epilogue only)."""
     family = "conv" if (mode == A_CONV2D or len(taps) > 1 or b_mode != 0) else "linear"
     if _fam(family, 2.0 * M * N * K * len(taps)):
         return out
@@ -302,6 +304,7 @@ def tapgemm(
     if phase is not None:
         d.interleave = 1
         d.phase_h, d.phase_w = int(phase[0]), int(phase[1])
+    d.act = int(act)
     check(load().svdx_tapgemm(C.byref(d), _stream()), "svdx_tapgemm")
     return out
 
@@ -346,12 +349,14 @@ def tapgemm_auto(a, b, out, *, M, N, K, taps=((0, 0, 0),), bias=None, rowbias=No
     kw = dict(kw)
     if kw.get("block_n") is None:
         kw.pop("block_n", None)
-    if (M <= 8 and len(taps) == 1 and kw.get("mode", A_ROWS) == A_ROWS and not kw.get("geglu") and not kw.get("a_mn") and not kw.get("b_mn")
+    if (M <= 8 and not kw.get("act") and len(taps) == 1 and kw.get("mode", A_ROWS) == A_ROWS and not kw.get("geglu") and not kw.get("a_mn") and not kw.get("b_mn")
             and rowbias is None and res1 is None and res2 is None and scales is None and gn_sum is None and kw.get("groups", 1) == 1
             and K % 8 == 0 and a.stride(-1) == 1 and b.stride(-1) == 1 and out.dtype in (bf16, torch.float32)):
         # conditioning vectors ([B, C] rows): a GEMV, not a 128-row tensor-core tile
         return gemv(a, b, out, M=M, N=N, K=K, bias=bias, lda=kw.get("lda"), ldw=kw.get("ldb"))
-    plan = split_plan(out.dtype == bf16, M, N, K, len(taps), kw.get("geglu"), kw.get("a_mn"), kw.get("b_mn"), kw.get("block_n"))
+    # the activation epilogue exists on the whole-problem path only
+    plan = None if kw.get("act") else split_plan(out.dtype == bf16, M, N, K, len(taps), kw.get("geglu"), kw.get("a_mn"), kw.get("b_mn"),
+                                                 kw.get("block_n"))
     if plan is not None:
         assert gn_sum is None, "fused GroupNorm statistics are not available on the split-K path"
         bn, split = plan
@@ -408,6 +413,19 @@ def attention_bwd(q, k, v, o, dout, dq, dk, dv, lse, delta, *, heads, S, nseq, i
     d.lddq, d.lddk, d.lddv = _rowmajor(dq, "dq"), _rowmajor(dk, "dk"), _rowmajor(dv, "dv")
     d.delta = delta.data_ptr()
     check(load().svdx_attention_bwd(C.byref(d), _stream()), "svdx_attention_bwd")
+
+
+def attention_hd80_fwd(q, k, v, o, *, heads, S, nseq, scale):
+    """head-dim-80 SDPA (the CLIP image encoder): q/k/v/o [nseq*S, >= heads*80] bf16 column slices, sequence s = rows
+    [s*S, (s+1)*S), head h = columns [80h, 80h + 80)"""
+    for t, n in ((q, "q"), (k, "k"), (v, "v"), (o, "o")):
+        if t.dtype != bf16 or not t.is_cuda or t.shape[0] < nseq * S:
+            raise ValueError(f"attention_hd80_fwd: {n} must be a CUDA bf16 [nseq*S, ld] matrix")
+    if _fam("attention", 4.0 * nseq * heads * S * S * 80):
+        return o
+    check(load().svdx_attention_hd80_fwd(q.data_ptr(), _rowmajor(q, "q"), k.data_ptr(), _rowmajor(k, "k"), v.data_ptr(), _rowmajor(v, "v"),
+                                         o.data_ptr(), _rowmajor(o, "o"), nseq, heads, S, float(scale), _stream()), "svdx_attention_hd80_fwd")
+    return o
 
 
 # ----------------------------------------------------------------------------- norms
@@ -561,6 +579,28 @@ def time_conv_out(x, weight, bias, out, T):
         return out
     check(load().svdx_time_conv_out(x.data_ptr(), _rowmajor(x, "x"), N, T, Cc, H, W, weight.data_ptr(), _ptr(bias), out.data_ptr(),
                                     dtype_code(out, "time_conv_out output"), _stream()), "svdx_time_conv_out")
+    return out
+
+
+def clip_preprocess(x, gy, gx, affine, out, *, out_size, patch):
+    """svdx_clip_preprocess: NCHW image x [B, 3, H, W] (fp32 / bf16 / fp16, contiguous) -> the bf16 patch-embedding operand
+    out [B * (1 + (out_size/patch)^2), ld]. gy / gx: the 1-D Gaussian weights (sequences of floats, odd lengths), affine: the six
+    floats {a_c} + {b_c} of out = v * a_c + b_c. Non-contiguous images, kernels longer than SVDX_CLIP_MAX_TAPS and reflect
+    padding >= the input dimension are rejected by the library."""
+    B, Cc, H, W = x.shape
+    if Cc != 3 or out.dtype != bf16 or not x.is_cuda or not out.is_cuda:
+        raise ValueError("clip_preprocess: x must be a CUDA [B, 3, H, W] image and out a CUDA bf16 matrix")
+    if out.shape[0] != B * (1 + (out_size // patch) ** 2):
+        raise ValueError("clip_preprocess: out must have B * (1 + P^2) rows")
+    gy, gx, affine = [float(v) for v in gy], [float(v) for v in gx], [float(v) for v in affine]
+    if len(affine) != 6:
+        raise ValueError("clip_preprocess: affine holds 3 scales then 3 shifts")
+    strides = (C.c_int64 * 4)(*x.stride())
+    fy, fx, fa = (C.c_float * max(1, len(gy)))(*gy), (C.c_float * max(1, len(gx)))(*gx), (C.c_float * 6)(*affine)
+    if _fam("elementwise", 0.0, x.element_size() * x.numel() + 2.0 * out.numel()):
+        return out
+    check(load().svdx_clip_preprocess(x.data_ptr(), dtype_code(x, "image"), strides, B, H, W, fy, len(gy), fx, len(gx), fa, out_size, patch,
+                                      out.data_ptr(), _rowmajor(out, "out"), _stream()), "svdx_clip_preprocess")
     return out
 
 

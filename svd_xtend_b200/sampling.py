@@ -10,8 +10,9 @@ CUDA graph replays all `num_inference_steps` steps; between replays the host onl
 Scheduler constants follow diffusers' EulerDiscreteScheduler in the SVD configuration [D] (Karras sigmas, rho 7, sigma in
 [0.002, 700], timesteps 0.25 ln sigma, init_noise_sigma sqrt(sigma_max^2 + 1)); tests/test_sampling_gpu.py checks the loop
 against oracle/svd_sampling_oracle.py. `image_latents` and `image_embeddings` are inputs (the VAE encode lives in vae.py, the CLIP
-image encoder is out of scope), denoised latents are the output; `decode_latents` turns them into frames with the temporal VAE
-decoder (`vae.AutoencoderKLTemporalDecoder(with_decoder=True)`), chunk by chunk like the pipeline.
+image encoder in clip.py), denoised latents are the output; `decode_latents` turns them into frames with the temporal VAE
+decoder (`vae.AutoencoderKLTemporalDecoder(with_decoder=True)`), chunk by chunk like the pipeline. pipeline.ImageToVideoPipeline
+chains all of them: image -> CLIP embedding + conditioning latents -> sampling -> decode -> frames.
 """
 from __future__ import annotations
 

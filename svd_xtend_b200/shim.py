@@ -5,7 +5,8 @@
 
 Before the script body runs, the replacement class is installed under the two names the reference
 imports the UNet from: `diffusers.UNetSpatioTemporalConditionModel` (train_svd.py:49) and
-`src.unet_spatio_temporal_condition.UNetSpatioTemporalConditionModel` (train_svd_lora.py:60).
+`src.unet_spatio_temporal_condition.UNetSpatioTemporalConditionModel` (train_svd_lora.py:60). Where transformers is
+importable, the image encoder is also installed as `transformers.CLIPVisionModelWithProjection` (train_svd.py:646-647).
 diffusers / accelerate are NOT part of this image (no network), so this shim is exercised only where a
 user's environment provides them; it fails loudly when they are missing.
 """
@@ -38,6 +39,24 @@ def install() -> None:
     sys.modules["src"] = pkg
     sys.modules["src.unet_spatio_temporal_condition"] = sub
     pkg.unet_spatio_temporal_condition = sub
+    install_clip()
+
+
+def install_clip() -> bool:
+    """when transformers is importable, install the H100 image encoder as `transformers.CLIPVisionModelWithProjection`
+    (train_svd.py:646-647 loads it from there); without transformers nothing changes. Returns whether it was installed."""
+    from .clip import CLIPVisionModelWithProjection
+    try:
+        transformers = importlib.import_module("transformers")
+    except ModuleNotFoundError:
+        return False
+    transformers.CLIPVisionModelWithProjection = CLIPVisionModelWithProjection
+    try:
+        m = importlib.import_module("transformers.models.clip")
+        setattr(m, "CLIPVisionModelWithProjection", CLIPVisionModelWithProjection)
+    except Exception:
+        pass
+    return True
 
 
 def main(argv=None) -> None:
