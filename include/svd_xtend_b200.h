@@ -380,6 +380,29 @@ int svdx_adamw_graph(float* p, const float* g, float* m, float* v, int64_t n, fl
 int svdx_adamw_p2p(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world,
                    int64_t lo, int64_t n, float* state, float grad_scale, int32_t tick, void* stream);
 
+/* Exponential moving average of the weights (train_svd.py:676-679 EMAModel, :1053-1054 ema_unet.step(unet.parameters())
+ * -> [D] diffusers.training_utils.EMAModel.step: get_decay on the host, then per parameter tensor
+ * s.sub_((1 - d) * (s - p)) if p.requires_grad else s.copy_(p)).
+ * ema_state = double[9] in DEVICE memory: {optimization_step, decay, min_decay, update_after_step, use_ema_warmup (0/1),
+ * inv_gamma, power, cur_decay_value, 1 - cur_decay_value}. Every entry point below first advances the step and evaluates
+ * EMAModel.get_decay in fp64 on the device (a 1-thread kernel, capturable in a CUDA graph), then applies
+ * e = e - (float)(1 - d) * (e - p) with three separately rounded fp32 operations: bit-identical to the torch ops.
+ *
+ * svdx_adamw_graph_ema: svdx_adamw_graph whose update also advances the fp32 EMA buffer ema[0 .. n) at the same flat
+ * offsets from the freshly updated masters (16-byte aligned). Two launches. */
+int svdx_adamw_graph_ema(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
+                         void* shadow_bf16, float* ema, double* ema_state, void* stream);
+/* svdx_adamw_p2p plus the EMA of this rank's slice: ema points at the local slice (length n, 16-byte aligned), no peer
+ * traffic. tick != 0 advances both the AdamW state and ema_state. */
+int svdx_adamw_p2p_ema(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world,
+                       int64_t lo, int64_t n, float* state, float grad_scale, int32_t tick, float* ema, double* ema_state,
+                       void* stream);
+/* the EMA update over many tensors in one launch (EMAModel.step over parameters outside a fused optimizer).
+ * jobs: device array of {float* shadow; const float* param; int64 n}; block_prefix[j] = first 4096-element block of job j,
+ * total_blocks = sum of ceil(n_j / 4096). Two launches (tick + update). */
+int svdx_ema_multi(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, double* ema_state,
+                   void* stream);
+
 /* many bf16 transposes dst[i][o] = src_base[src_off + o*I + i] in one launch (dgrad operands of all trainable linears).
  * jobs: device array of {int64 src_off; void* dst; int32 O; int32 I}; tile_prefix[j] = first 32x32 tile of job j. */
 int svdx_multi_transpose(const void* src_base, const void* jobs, const int32_t* tile_prefix, int32_t njobs, int32_t total_tiles,

@@ -119,6 +119,10 @@ _PROTOS = {
                    c_int, c_float, c_void_p, c_void_p],
     "svdx_adamw_graph": [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_float, c_void_p, c_void_p],
     "svdx_adamw_p2p": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_i64, c_i64, c_void_p, c_float, c_int, c_void_p],
+    "svdx_adamw_graph_ema": [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p],
+    "svdx_adamw_p2p_ema": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_i64, c_i64, c_void_p, c_float, c_int, c_void_p,
+                           c_void_p, c_void_p],
+    "svdx_ema_multi": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p],
     "svdx_multi_transpose": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p],
 }
 

@@ -512,14 +512,44 @@ __global__ void adamw_kernel(float* __restrict__ p, const float* __restrict__ g,
 //   state[0] lr  [1] beta1  [2] beta2  [3] eps  [4] weight_decay  [5] step (float, exact up to 2^24)  [6] 1-beta1^step  [7] 1-beta2^step
 // adamw_tick advances the step count and the bias corrections on the device, so a captured graph that contains
 // tick + update replays torch.optim.AdamW's step sequence; the learning rate is whatever the host last wrote to state[0].
-__global__ void adamw_tick_kernel(float* state) {
+SVDX_DEVINL void adamw_advance(float* state) {
   const float step = state[5] + 1.f;
   state[5] = step;
   state[6] = 1.f - powf(state[1], step);
   state[7] = 1.f - powf(state[2], step);
 }
+__global__ void adamw_tick_kernel(float* state) { adamw_advance(state); }
+
+// EMA of the fp32 masters (diffusers.training_utils.EMAModel, the --use_ema path of train_svd.py:676-679, :1053-1054).
+// ema_state = double[9]: [0] optimization_step [1] decay [2] min_decay [3] update_after_step [4] use_ema_warmup (0/1)
+// [5] inv_gamma [6] power [7] cur_decay_value [8] 1 - cur_decay_value. The tick evaluates EMAModel.get_decay in fp64 (the
+// host's Python doubles), so a captured graph replays the right decay sequence; the step count is an exact fp64 integer.
+// The update e -= (1 - d) * (e - p) uses 1 - d rounded to fp32, as torch's fp32 tensor ops do with a Python scalar.
+SVDX_DEVINL void ema_advance(double* s) {
+  const double t = s[0] + 1.0;
+  s[0] = t;
+  const double st = fmax(0.0, t - s[3] - 1.0);
+  double d = 0.0;
+  if (st > 0.0) {
+    d = s[4] != 0.0 ? 1.0 - pow(1.0 + st / s[5], -s[6]) : (1.0 + st) / (10.0 + st);
+    d = fmax(fmin(d, s[1]), s[2]);
+  }
+  s[7] = d;
+  s[8] = 1.0 - d;
+}
+__global__ void ema_tick_kernel(double* ema_state) { ema_advance(ema_state); }
+__global__ void adamw_ema_tick_kernel(float* state, double* ema_state) {
+  adamw_advance(state);
+  ema_advance(ema_state);
+}
+// e - omd * (e - p) as three separately rounded fp32 operations (no FMA contraction): bit-identical to
+// torch's `s.sub_(omd * (s - p))`
+SVDX_DEVINL float ema_update(float e, float p, float omd) { return __fsub_rn(e, __fmul_rn(omd, __fsub_rn(e, p))); }
+
+template <bool EMA>
 __global__ void adamw_state_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, long long n4,
-                                   long long n, const float* __restrict__ state, float gscale, bf16* __restrict__ shadow) {
+                                   long long n, const float* __restrict__ state, float gscale, bf16* __restrict__ shadow,
+                                   float* __restrict__ ema, const double* __restrict__ ema_state) {
   const long long i4 = gtid();
   if (i4 >= n4) return;
   const float lr = state[0], b1 = state[1], b2 = state[2], eps = state[3], wd = state[4], bc1 = state[6], bc2 = state[7];
@@ -545,6 +575,13 @@ __global__ void adamw_state_kernel(float* __restrict__ p, const float* __restric
       o.y = pack_bf16x2(pp[2], pp[3]);
       *reinterpret_cast<uint2*>(shadow + i) = o;
     }
+    if constexpr (EMA) {
+      const float omd = (float)ema_state[8];
+      float4 e4 = *reinterpret_cast<float4*>(ema + i);
+      e4.x = ema_update(e4.x, pp[0], omd); e4.y = ema_update(e4.y, pp[1], omd);
+      e4.z = ema_update(e4.z, pp[2], omd); e4.w = ema_update(e4.w, pp[3], omd);
+      *reinterpret_cast<float4*>(ema + i) = e4;
+    }
   } else {
     for (long long k = i; k < n; ++k) {
       const float gi = g[k] * gscale;
@@ -552,6 +589,7 @@ __global__ void adamw_state_kernel(float* __restrict__ p, const float* __restric
       const float pi = p[k] * decay - step_size * mi / (sqrtf(vi) * inv_sqrt_bc2 + eps);
       m[k] = mi; v[k] = vi; p[k] = pi;
       if (shadow) shadow[k] = __float2bfloat16(pi);
+      if constexpr (EMA) ema[k] = ema_update(ema[k], pi, (float)ema_state[8]);
     }
   }
 }
@@ -568,8 +606,10 @@ struct AdamP2P {
   const float* grad[16];
   bf16* shadow[16];
 };
+template <bool EMA>
 __global__ void __launch_bounds__(256) adamw_p2p_kernel(float* __restrict__ p, float* __restrict__ m, float* __restrict__ v, const __grid_constant__ AdamP2P ptr,
-                                                        int world, long long lo, long long n4, const float* __restrict__ state, float gscale) {
+                                                        int world, long long lo, long long n4, const float* __restrict__ state, float gscale,
+                                                        float* __restrict__ ema, const double* __restrict__ ema_state) {
   const float lr = state[0], b1 = state[1], b2 = state[2], eps = state[3], wd = state[4], bc1 = state[6], bc2 = state[7];
   const float decay = 1.f - lr * wd, step_size = lr / bc1, inv_sqrt_bc2 = rsqrtf(bc2);
   const long long stride = (long long)gridDim.x * blockDim.x;
@@ -603,8 +643,51 @@ __global__ void __launch_bounds__(256) adamw_p2p_kernel(float* __restrict__ p, f
     o.x = pack_bf16x2(pp[0], pp[1]);
     o.y = pack_bf16x2(pp[2], pp[3]);
     for (int r = 0; r < world; ++r) *reinterpret_cast<uint2*>(ptr.shadow[r] + lo + i) = o;
+    if constexpr (EMA) {     // this rank's slice of the EMA only: no peer traffic
+      const float omd = (float)ema_state[8];
+      float4 e4 = *reinterpret_cast<float4*>(ema + i);
+      e4.x = ema_update(e4.x, pp[0], omd); e4.y = ema_update(e4.y, pp[1], omd);
+      e4.z = ema_update(e4.z, pp[2], omd); e4.w = ema_update(e4.w, pp[3], omd);
+      *reinterpret_cast<float4*>(ema + i) = e4;
+    }
   }
   __threadfence_system();     // the peer stores are performed system-wide before this kernel counts as complete
+}
+
+// EMAModel.step over many (shadow, parameter) pairs in ONE launch: block -> (job, chunk) through a block prefix table (the
+// pattern of multi_transpose_kernel). The same three fp32 roundings as the fused optimizer forms.
+struct EmaJob {
+  float* shadow;
+  const float* param;
+  long long n;
+};
+constexpr int EMA_CHUNK = 4096;     // elements per block: 256 threads x 4 float4
+__global__ void __launch_bounds__(256) multi_ema_kernel(const EmaJob* __restrict__ jobs, const int* __restrict__ block_prefix, int njobs,
+                                                        const double* __restrict__ ema_state) {
+  int lo = 0, hi = njobs - 1;
+  const int b = blockIdx.x;
+  while (lo < hi) {            // last job whose first block <= b
+    const int mid = (lo + hi + 1) >> 1;
+    if (block_prefix[mid] <= b) lo = mid; else hi = mid - 1;
+  }
+  const EmaJob j = jobs[lo];
+  const long long c0 = (long long)(b - block_prefix[lo]) * EMA_CHUNK;
+  const long long c1 = c0 + EMA_CHUNK < j.n ? c0 + EMA_CHUNK : j.n;
+  const float omd = (float)ema_state[8];
+  const bool vec = ((reinterpret_cast<uintptr_t>(j.shadow) | reinterpret_cast<uintptr_t>(j.param)) & 15) == 0;
+  if (vec && c1 - c0 == EMA_CHUNK) {
+#pragma unroll
+    for (int k = 0; k < EMA_CHUNK / 1024; ++k) {
+      const long long i = c0 + (k * 256 + threadIdx.x) * 4;
+      float4 e4 = *reinterpret_cast<float4*>(j.shadow + i);
+      const float4 p4 = __ldg(reinterpret_cast<const float4*>(j.param + i));
+      e4.x = ema_update(e4.x, p4.x, omd); e4.y = ema_update(e4.y, p4.y, omd);
+      e4.z = ema_update(e4.z, p4.z, omd); e4.w = ema_update(e4.w, p4.w, omd);
+      *reinterpret_cast<float4*>(j.shadow + i) = e4;
+    }
+  } else {
+    for (long long i = c0 + threadIdx.x; i < c1; i += 256) j.shadow[i] = ema_update(j.shadow[i], j.param[i], omd);
+  }
 }
 
 // row softmax of a bf16 score matrix, y[r][:] = softmax(scale * x[r][:]) (fp32 arithmetic, in place allowed): the single-head,
@@ -1038,13 +1121,38 @@ extern "C" int svdx_adamw_graph(float* p, const float* g, float* m, float* v, in
     return svdx_fail(SVDX_E_BADARG, "adamw_graph: bad arguments (16-byte aligned flat buffers, device state[8])");
   adamw_tick_kernel<<<1, 1, 0, ST(stream)>>>(state);
   const long long n4 = (n + 3) / 4;
-  adamw_state_kernel<<<nblocks(n4), 256, 0, ST(stream)>>>(p, g, m, v, n4, n, state, grad_scale, reinterpret_cast<bf16*>(shadow_bf16));
+  adamw_state_kernel<false><<<nblocks(n4), 256, 0, ST(stream)>>>(p, g, m, v, n4, n, state, grad_scale, reinterpret_cast<bf16*>(shadow_bf16),
+                                                                 nullptr, nullptr);
   SVDX_CHECK_LAUNCH("adamw_graph");
   return SVDX_OK;
 }
 
-extern "C" int svdx_adamw_p2p(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo, int64_t n,
-                              float* state, float grad_scale, int32_t tick, void* stream) {
+extern "C" int svdx_adamw_graph_ema(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
+                                    void* shadow_bf16, float* ema, double* ema_state, void* stream) {
+  if (!p || !g || !m || !v || !state || !ema || !ema_state || n <= 0 || (reinterpret_cast<uintptr_t>(p) & 15) ||
+      (reinterpret_cast<uintptr_t>(g) & 15) || (reinterpret_cast<uintptr_t>(m) & 15) || (reinterpret_cast<uintptr_t>(v) & 15) ||
+      (reinterpret_cast<uintptr_t>(ema) & 15) || (reinterpret_cast<uintptr_t>(ema_state) & 7) || (reinterpret_cast<uintptr_t>(shadow_bf16) & 7))
+    return svdx_fail(SVDX_E_BADARG, "adamw_graph_ema: bad arguments (16-byte aligned flat buffers and EMA, device state[8], ema_state[9])");
+  adamw_ema_tick_kernel<<<1, 1, 0, ST(stream)>>>(state, ema_state);
+  const long long n4 = (n + 3) / 4;
+  adamw_state_kernel<true><<<nblocks(n4), 256, 0, ST(stream)>>>(p, g, m, v, n4, n, state, grad_scale, reinterpret_cast<bf16*>(shadow_bf16),
+                                                                ema, ema_state);
+  SVDX_CHECK_LAUNCH("adamw_graph_ema");
+  return SVDX_OK;
+}
+
+extern "C" int svdx_ema_multi(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, double* ema_state,
+                              void* stream) {
+  if (!jobs || !block_prefix || !ema_state || njobs <= 0 || total_blocks <= 0 || (reinterpret_cast<uintptr_t>(ema_state) & 7))
+    return svdx_fail(SVDX_E_BADARG, "ema_multi: bad arguments");
+  ema_tick_kernel<<<1, 1, 0, ST(stream)>>>(ema_state);
+  multi_ema_kernel<<<total_blocks, 256, 0, ST(stream)>>>(reinterpret_cast<const EmaJob*>(jobs), block_prefix, njobs, ema_state);
+  SVDX_CHECK_LAUNCH("ema_multi");
+  return SVDX_OK;
+}
+
+static int adamw_p2p_launch(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo, int64_t n,
+                            float* state, float grad_scale, int32_t tick, float* ema, double* ema_state, void* stream) {
   if (!p || !m || !v || !grads || !shadows || !state || world < 1 || world > 16 || n <= 0 || n % 4 || lo % 4 ||
       (reinterpret_cast<uintptr_t>(p) & 15) || (reinterpret_cast<uintptr_t>(m) & 15) || (reinterpret_cast<uintptr_t>(v) & 15))
     return svdx_fail(SVDX_E_BADARG, "adamw_p2p: bad arguments (world <= 16, slice offset / length multiples of 4, 16-byte aligned buffers)");
@@ -1056,15 +1164,31 @@ extern "C" int svdx_adamw_p2p(float* p, float* m, float* v, const void* const* g
     ptr.grad[r] = reinterpret_cast<const float*>(grads[r]);
     ptr.shadow[r] = reinterpret_cast<bf16*>(shadows[r]);
   }
-  if (tick) adamw_tick_kernel<<<1, 1, 0, ST(stream)>>>(state);
+  if (tick) {
+    if (ema) adamw_ema_tick_kernel<<<1, 1, 0, ST(stream)>>>(state, ema_state);
+    else adamw_tick_kernel<<<1, 1, 0, ST(stream)>>>(state);
+  }
   const long long n4 = n / 4;
   // a few resident CTAs per SM, grid-stride: enough 16-byte loads in flight to cover the NVLink round trip
   long long blocks = (n4 + 255) / 256;
   const long long cap = (long long)svdx_num_sms() * 8;
   if (blocks > cap) blocks = cap;
-  adamw_p2p_kernel<<<(unsigned)blocks, 256, 0, ST(stream)>>>(p, m, v, ptr, world, lo, n4, state, grad_scale);
+  if (ema) adamw_p2p_kernel<true><<<(unsigned)blocks, 256, 0, ST(stream)>>>(p, m, v, ptr, world, lo, n4, state, grad_scale, ema, ema_state);
+  else adamw_p2p_kernel<false><<<(unsigned)blocks, 256, 0, ST(stream)>>>(p, m, v, ptr, world, lo, n4, state, grad_scale, nullptr, nullptr);
   SVDX_CHECK_LAUNCH("adamw_p2p");
   return SVDX_OK;
+}
+
+extern "C" int svdx_adamw_p2p(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo, int64_t n,
+                              float* state, float grad_scale, int32_t tick, void* stream) {
+  return adamw_p2p_launch(p, m, v, grads, shadows, world, lo, n, state, grad_scale, tick, nullptr, nullptr, stream);
+}
+
+extern "C" int svdx_adamw_p2p_ema(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo,
+                                  int64_t n, float* state, float grad_scale, int32_t tick, float* ema, double* ema_state, void* stream) {
+  if (!ema || !ema_state || (reinterpret_cast<uintptr_t>(ema) & 15) || (reinterpret_cast<uintptr_t>(ema_state) & 7))
+    return svdx_fail(SVDX_E_BADARG, "adamw_p2p_ema: null / misaligned EMA slice or ema_state[9]");
+  return adamw_p2p_launch(p, m, v, grads, shadows, world, lo, n, state, grad_scale, tick, ema, ema_state, stream);
 }
 
 extern "C" int svdx_multi_transpose(const void* src_base, const void* jobs, const int32_t* tile_prefix, int32_t njobs, int32_t total_tiles,

@@ -26,7 +26,8 @@ def dtype_code(t: torch.Tensor, what: str) -> int:
 
 # number of kernels launched through the C ABI since import (each wrapper adds what its entry point launches)
 LAUNCHES = [0]
-_KERNELS_PER_CALL = {"svdx_groupnorm_stats": 2, "svdx_groupnorm_bwd": 2, "svdx_groupnorm_apply_fused": 1, "svdx_attention_bwd": 3, "svdx_adamw_graph": 2, "svdx_adamw_p2p": 2}
+_KERNELS_PER_CALL = {"svdx_groupnorm_stats": 2, "svdx_groupnorm_bwd": 2, "svdx_groupnorm_apply_fused": 1, "svdx_attention_bwd": 3, "svdx_adamw_graph": 2, "svdx_adamw_p2p": 2,
+                     "svdx_adamw_graph_ema": 2, "svdx_adamw_p2p_ema": 2, "svdx_ema_multi": 2}
 
 
 def check(rc: int, what: str = "") -> None:
@@ -713,26 +714,58 @@ def adamw(p, g, m, v, lr, beta1, beta2, eps, weight_decay, step, grad_scale=1.0,
                             step, grad_scale, _ptr(shadow), _stream()), "adamw")
 
 
-def adamw_p2p(p, m, v, peer_grads, peer_shadows, lo, state, grad_scale, tick=True):
+def _ema_args(ema, ema_state, n):
+    if (ema is None) != (ema_state is None):
+        raise ValueError("ema and ema_state go together")
+    if ema is not None and (ema.dtype != torch.float32 or ema.numel() != n or ema_state.dtype != torch.float64 or ema_state.numel() < 9):
+        raise ValueError("ema: fp32 buffer of the updated slice's length; ema_state: float64[9] (svd_xtend_b200.h)")
+
+
+def adamw_p2p(p, m, v, peer_grads, peer_shadows, lo, state, grad_scale, tick=True, ema=None, ema_state=None):
     """reduce-scatter + AdamW + all-gather in one kernel over NVLink peer memory (svdx_adamw_p2p): p / m / v are this rank's
     slices, peer_grads / peer_shadows the FULL arenas of every rank (this rank's own included) as tensors mapped into this
-    process (train.map_peer_buffers)"""
+    process (train.map_peer_buffers). With `ema` (this rank's fp32 EMA slice) and `ema_state` the same launch also advances
+    the EMA of the updated masters (svdx_adamw_p2p_ema)."""
     world = len(peer_grads)
     n = p.numel()
-    if _fam("adamw", 0.0, (4.0 * world + 28.0 + 2.0 * world) * n):
+    _ema_args(ema, ema_state, n)
+    if _fam("adamw", 0.0, (4.0 * world + 28.0 + 2.0 * world + (8.0 if ema is not None else 0.0)) * n):
         return
     ga = (C.c_void_p * world)(*[t if isinstance(t, int) else t.data_ptr() for t in peer_grads])       # tensors or mapped addresses
     sa = (C.c_void_p * world)(*[t if isinstance(t, int) else t.data_ptr() for t in peer_shadows])
+    if ema is not None:
+        check(load().svdx_adamw_p2p_ema(p.data_ptr(), m.data_ptr(), v.data_ptr(), ga, sa, world, lo, n, state.data_ptr(), float(grad_scale),
+                                        int(tick), ema.data_ptr(), ema_state.data_ptr(), _stream()), "svdx_adamw_p2p_ema")
+        return
     check(load().svdx_adamw_p2p(p.data_ptr(), m.data_ptr(), v.data_ptr(), ga, sa, world, lo, n, state.data_ptr(), float(grad_scale),
                                 int(tick), _stream()), "svdx_adamw_p2p")
 
 
-def adamw_graph(p, g, m, v, state, grad_scale=1.0, shadow=None):
-    """CUDA-graph-safe AdamW: lr / betas / eps / weight decay / step / bias corrections live in the device float[8] `state`"""
-    if _fam("adamw", 0.0, (30.0 if shadow is not None else 28.0) * p.numel()):
+def adamw_graph(p, g, m, v, state, grad_scale=1.0, shadow=None, ema=None, ema_state=None):
+    """CUDA-graph-safe AdamW: lr / betas / eps / weight decay / step / bias corrections live in the device float[8] `state`.
+    With `ema` (fp32, same length as p) and `ema_state` (device float64[9]) the update also advances the EMA of the new
+    masters at the same offsets (svdx_adamw_graph_ema)."""
+    _ema_args(ema, ema_state, p.numel())
+    if _fam("adamw", 0.0, ((30.0 if shadow is not None else 28.0) + (8.0 if ema is not None else 0.0)) * p.numel()):
+        return
+    if ema is not None:
+        check(load().svdx_adamw_graph_ema(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(), state.data_ptr(), grad_scale,
+                                          _ptr(shadow), ema.data_ptr(), ema_state.data_ptr(), _stream()), "svdx_adamw_graph_ema")
         return
     check(load().svdx_adamw_graph(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(), state.data_ptr(), grad_scale,
                                   _ptr(shadow), _stream()), "svdx_adamw_graph")
+
+
+EMA_CHUNK = 4096     # elements per block of multi_ema_kernel
+
+
+def ema_multi(jobs, block_prefix, njobs, total_blocks, ema_state, nelem):
+    """EMA tick + update of many (shadow, parameter) fp32 pairs in one launch (svdx_ema_multi). jobs: device bytes of
+    {float* shadow; const float* param; int64 n} per job; nelem (the summed n) is for the byte accounting only."""
+    if _fam("adamw", 0.0, 12.0 * nelem):
+        return
+    check(load().svdx_ema_multi(jobs.data_ptr(), block_prefix.data_ptr(), njobs, total_blocks, ema_state.data_ptr(), _stream()),
+          "svdx_ema_multi")
 
 
 def multi_transpose(src_base, jobs, tile_prefix, njobs, total_tiles):

@@ -5,7 +5,8 @@
 
 Before the script body runs, the replacement class is installed under the two names the reference
 imports the UNet from: `diffusers.UNetSpatioTemporalConditionModel` (train_svd.py:49) and
-`src.unet_spatio_temporal_condition.UNetSpatioTemporalConditionModel` (train_svd_lora.py:60). Where transformers is
+`src.unet_spatio_temporal_condition.UNetSpatioTemporalConditionModel` (train_svd_lora.py:60), and the EMA as
+`diffusers.training_utils.EMAModel` (train_svd.py:52, used with --use_ema). Where transformers is
 importable, the image encoder is also installed as `transformers.CLIPVisionModelWithProjection` (train_svd.py:646-647).
 diffusers / accelerate are NOT part of this image (no network), so this shim is exercised only where a
 user's environment provides them; it fails loudly when they are missing.
@@ -39,6 +40,14 @@ def install() -> None:
     sys.modules["src"] = pkg
     sys.modules["src.unet_spatio_temporal_condition"] = sub
     pkg.unet_spatio_temporal_condition = sub
+    # train_svd.py:52 `from diffusers.training_utils import EMAModel` (--use_ema): the EMA on this package's kernels, whose
+    # copy_to / restore move the parameters' version counters (svd_xtend_b200.ema)
+    from .ema import EMAModel
+    try:
+        tu = importlib.import_module("diffusers.training_utils")
+        tu.EMAModel = EMAModel
+    except ModuleNotFoundError:
+        pass
     install_clip()
 
 

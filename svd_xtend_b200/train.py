@@ -68,10 +68,11 @@ class ParamArena:
         self.mark_synced()
 
     # ---- staleness of the derived bf16 operands -------------------------------------------------------------
-    # FusedAdamW updates masters, shadow and transposes together. Anything ELSE that writes the parameters
-    # (torch.optim.AdamW.step, load_state_dict, an EMA copy_to, p.data.copy_) goes through torch and bumps the
+    # FusedAdamW updates masters, shadow and transposes together. Other writers that go through torch ops on the
+    # parameter (torch.optim.AdamW.step, load_state_dict, svd_xtend_b200.ema.EMAModel.copy_to / restore) bump the
     # parameters' version counters: the model compares the stamp below at the start of every forward and re-derives
-    # the operands when it moved (UNetSpatioTemporalConditionModel._validate).
+    # the operands when it moved. A write through `p.data` (`p.data.copy_(...)`, which diffusers' own EMAModel.copy_to /
+    # restore use) does NOT bump the counter and stays invisible here: call unet.refresh_trainable_operands() after it.
     def _stamp(self) -> int:
         return sum(p._version for p in self.params)
 
@@ -174,6 +175,25 @@ class FusedAdamW:
         self.on_updated = None
         # torch.optim-style view for lr schedulers: `for g in opt.param_groups: g["lr"] = ...` then `opt.sync_lr()`
         self.param_groups = [{"lr": float(lr), "params": arena.params}]
+        self.ema = None
+
+    def attach_ema(self, ema):
+        """Advance `ema` (an svd_xtend_b200.ema.EMAModel built over the model's parameters, frozen ones included or not) inside
+        every step(): its shadows of the arena's parameters are re-homed into one flat fp32 buffer at the arena offsets and
+        updated by the AdamW kernel from the new masters (8 more bytes per parameter, no extra launch), so a captured
+        GraphedStep replays the EMA with the right decay sequence. The EMA's copies of frozen parameters are dropped: their
+        EMA is the parameter. From then on `ema.step()` raises."""
+        ema._attach(self, sharded=False)
+        self.ema = ema
+
+    def _ema_args(self, lo=None, hi=None):
+        if self.ema is None:
+            return {}
+        flat = self.ema._flat if lo is None else self.ema._flat[lo:hi]
+        return {"ema": flat, "ema_state": self.ema._state}
+
+    def _ema_tensors(self) -> List[torch.Tensor]:
+        return [] if self.ema is None else [self.ema._flat, self.ema._state]
 
     @property
     def lr(self) -> float:
@@ -198,7 +218,7 @@ class FusedAdamW:
 
     def step(self, grad_scale: float = 1.0):
         a = self.arena
-        raw.adamw_graph(a.data, a.grad, self.m, self.v, self.state, grad_scale, shadow=a.shadow)
+        raw.adamw_graph(a.data, a.grad, self.m, self.v, self.state, grad_scale, shadow=a.shadow, **self._ema_args())
         if self.on_updated is not None:
             self.on_updated()
 
@@ -206,11 +226,11 @@ class FusedAdamW:
         self.arena.zero_grad()
 
     def snapshot_tensors(self) -> List[torch.Tensor]:
-        """everything a warm-up step mutates (for GraphedStep(restore=...))"""
+        """everything a warm-up step mutates (for GraphedStep(restore=...)), the attached EMA included"""
         ts = [self.arena.data, self.m, self.v, self.state]
         if self.arena.shadow is not None:
             ts.append(self.arena.shadow)
-        return ts
+        return ts + self._ema_tensors()
 
 
 class ShardedAdamW:
@@ -243,10 +263,27 @@ class ShardedAdamW:
         self._lr_host = torch.empty(1, dtype=F32).pin_memory() if arena.data.is_cuda else torch.empty(1, dtype=F32)
         self.on_updated = None
         self.param_groups = [{"lr": float(lr), "params": arena.params}]
+        self.ema = None
 
     lr = FusedAdamW.lr
     sync_lr = FusedAdamW.sync_lr
     t = FusedAdamW.t
+    _ema_args = FusedAdamW._ema_args
+    _ema_tensors = FusedAdamW._ema_tensors
+
+    def attach_ema(self, ema):
+        """FusedAdamW.attach_ema for the sharded update: the EMA buffer has the arena's full length and each rank advances its
+        [lo, hi) slice. Call `gather_ema()` before copy_to / state_dict / save_pretrained (they raise on an EMA advanced
+        since the last gather)."""
+        ema._attach(self, sharded=True)
+        self.ema = ema
+
+    def gather_ema(self):
+        """make every slice of the attached EMA current on this rank (in-place all-gather, like gather_masters)"""
+        if self.ema is None:
+            raise RuntimeError("gather_ema: no EMA attached")
+        self.all_gather_(self.ema._flat)
+        self.ema._gathered_at = self.ema.optimization_step
 
     def reduce_scatter_grads(self):
         a = self.arena
@@ -274,7 +311,7 @@ class ShardedAdamW:
         a = self.arena
         g = self.reduce_scatter_grads()
         raw.adamw_graph(a.data[self.lo:self.hi], g, self.m, self.v, self.state, 1.0 / self.world,
-                        shadow=None if a.shadow is None else a.shadow[self.lo:self.hi])
+                        shadow=None if a.shadow is None else a.shadow[self.lo:self.hi], **self._ema_args(self.lo, self.hi))
         if a.shadow is not None:
             self.all_gather_(a.shadow)
         else:
@@ -293,7 +330,7 @@ class ShardedAdamW:
         ts = [self.arena.data, self.m, self.v, self.state]
         if self.arena.shadow is not None:
             ts.append(self.arena.shadow)
-        return ts
+        return ts + self._ema_tensors()
 
 
 def map_peer_buffers(t: torch.Tensor, group=None) -> List[int]:
@@ -361,7 +398,8 @@ class P2PShardedAdamW(ShardedAdamW):
         a = self.arena
         if self.world > 1:
             self._fence()                                   # every rank's gradients are final
-        raw.adamw_p2p(a.data[self.lo:self.hi], self.m, self.v, self.peer_grad, self.peer_shadow, self.lo, self.state, 1.0 / self.world)
+        raw.adamw_p2p(a.data[self.lo:self.hi], self.m, self.v, self.peer_grad, self.peer_shadow, self.lo, self.state, 1.0 / self.world,
+                      **self._ema_args(self.lo, self.hi))
         if self.world > 1:
             self._fence()                                   # every shadow is complete, nobody still reads this rank's gradients
         if self.on_updated is not None:
