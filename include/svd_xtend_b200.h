@@ -118,7 +118,7 @@ typedef struct SvdxTapGemm {
    * WRITES dy = dL/d(GroupNorm output) — the data gradient of the conv that consumed the normalised tensor. gnb_x (channels
    * [0, gnb_c1)) and gnb_x2 (the rest; NULL = single source) are the GroupNorm's bf16 INPUT, gnb_ab[(2*s + 0) * N + n] /
    * [(2*s + 1) * N + n] the forward scale / shift of channel n in statistics slab s = m / gnb_rows (written by
-   * svdx_groupnorm_apply*, y = act(x * scale + shift); only read when gnb_silu). The epilogue accumulates
+   * svdx_groupnorm_apply_fused, y = act(x * scale + shift); only read when gnb_silu). The epilogue accumulates
    *   gnb_sum[(2*s + 0) * N + n] += e,  gnb_sum[(2*s + 1) * N + n] += e * x[m][n],   e = dy[m][n] * act'(x * scale + shift)
    * on the bf16 values it stores (buffer zero on entry); svdx_groupnorm_bwd_fused turns them into dx / dgamma / dbeta with ONE
    * pass over x and dy. Requires the plain bf16 TMA-store epilogue (no residual / scales / GEGLU / split-K / gn_sum), N even. */
@@ -185,40 +185,32 @@ const char* svdx_last_error(void);
  * x is [ngroups_outer][rows][C] bf16 where one statistics group spans `rows` rows x (C/32) channels.
  * A second source x2 (C2 channels) is concatenated along channels (the up-block torch.cat).
  */
-int svdx_groupnorm_stats(const void* x, int64_t ldx, int32_t C1, const void* x2, int64_t ldx2, int32_t C2,
-                         int32_t outer, int32_t rows, int32_t num_groups, float eps,
-                         float* mean, float* rstd, void* stream);
-int svdx_groupnorm_apply(const void* x, int64_t ldx, int32_t C1, const void* x2, int64_t ldx2, int32_t C2,
-                         int32_t outer, int32_t rows, int32_t num_groups,
-                         const float* mean, const float* rstd, const float* gamma, const float* beta,
-                         int32_t fuse_silu, void* y, int64_t ldy, float* ab_out, void* stream);
-/* ab_out (optional, both apply forms): fp32 [outer][2][C], receives the per-channel scale / shift of every slab
- * (y = act(x * scale + shift)) — the gnb_ab table of the GroupNorm-backward sums fused into svdx_tapgemm's epilogue.
- * gamma / beta must be 16-byte aligned.
- *
- * GroupNorm(+SiLU) apply from per-CHANNEL sums produced by the svdx_tapgemm epilogues (gn_sum above): csum1 / csum2 are the
- * [outer][2][ld] fp32 sum / sum-of-squares arrays of the two channel-concatenated sources (csum2 NULL when C2 == 0). Every
- * CTA first folds the channels of its slab into the 32 group statistics (shared memory), the CTA with blockIdx.x == 0 of
- * each slab also writes mean / rstd [outer][groups] for the backward. Replaces stats + finalize + apply by ONE launch. */
+/* Per-(slab, channel) sums of a tensor no producing epilogue covered: sums[(2*s + 0) * ld + c] += x, sums[(2*s + 1) * ld + c]
+ * += x^2 over the rows of slab s, exactly the gn_sum contract of svdx_tapgemm (sums zero on entry, 16-byte aligned,
+ * ld >= C1 + C2, ld % 4 == 0). */
+int svdx_groupnorm_sums(const void* x, int64_t ldx, int32_t C1, const void* x2, int64_t ldx2, int32_t C2,
+                        int32_t outer, int32_t rows, float* sums, int64_t ld, void* stream);
+/* GroupNorm(+SiLU) apply from per-CHANNEL sums (gn_sum of the producing svdx_tapgemm epilogues, or svdx_groupnorm_sums):
+ * csum1 / csum2 are the [outer][2][ld] fp32 sum / sum-of-squares arrays of the two channel-concatenated sources (csum2 NULL
+ * when C2 == 0). Every CTA first folds the channels of its slab into the group statistics (shared memory), the CTA with
+ * blockIdx.x == 0 of each slab also writes mean / rstd [outer][groups] for the backward. gamma / beta must be 16-byte
+ * aligned. ab_out (optional): fp32 [outer][2][C], receives the per-channel scale / shift of every slab
+ * (y = act(x * scale + shift)): the gnb_ab table of the GroupNorm-backward sums (svdx_tapgemm, svdx_groupnorm_bwd_sums). */
 int svdx_groupnorm_apply_fused(const void* x, int64_t ldx, int32_t C1, const void* x2, int64_t ldx2, int32_t C2,
                                int32_t outer, int32_t rows, int32_t num_groups, float eps,
                                const float* csum1, int64_t ldc1, const float* csum2, int64_t ldc2,
                                float* mean, float* rstd, const float* gamma, const float* beta,
                                int32_t fuse_silu, void* y, int64_t ldy, float* ab_out, void* stream);
-/* backward: dx (and optional dgamma/dbeta accumulation, fp32 atomic). workspace: float[2 * outer * groups]; it must be
- * ZERO on entry when workspace_is_zero != 0 (a slice of a pre-zeroed arena: no memset node), else it is cleared here.
- * dres (optional, bf16 [outer*rows][lddres], single-source form only): a gradient already accumulated on x through its
- * residual use; dx = GroupNorm backward + dres in the same pass (replaces a separate bf16 add over the activation). */
-int svdx_groupnorm_bwd(const void* x, int64_t ldx, int32_t C1, const void* x2, int64_t ldx2, int32_t C2,
-                       const void* dy, int64_t lddy,
-                       int32_t outer, int32_t rows, int32_t num_groups,
-                       const float* mean, const float* rstd, const float* gamma, const float* beta,
-                       int32_t fuse_silu, void* dx, int64_t lddx, void* dx2, int64_t lddx2,
-                       float* dgamma, float* dbeta, float* workspace, int32_t workspace_is_zero,
-                       const void* dres, int64_t lddres, void* stream);
-/* backward when pass 1 already ran inside the epilogue that produced dy (svdx_tapgemm gnb_sum): csum = that [outer][2][C]
- * buffer (sum e, sum e*x per slab and channel). One launch, one pass over x and dy: every CTA folds the channel sums into the
- * group sums, dgamma / dbeta (optional, accumulated) come straight from the channel sums. Other arguments as svdx_groupnorm_bwd. */
+/* Backward pass 1 for a dy no dgrad epilogue covered: the gnb_sum contract of svdx_tapgemm, sums[(2*s + 0) * C + c] += e,
+ * sums[(2*s + 1) * C + c] += e * x, e = dy * silu'(x * scale + shift) with scale / shift from the ab table of
+ * svdx_groupnorm_apply_fused (read only when fuse_silu). sums: fp32 [outer][2][C], zero on entry, 16-byte aligned. */
+int svdx_groupnorm_bwd_sums(const void* x, int64_t ldx, int32_t C1, const void* x2, int64_t ldx2, int32_t C2,
+                            const void* dy, int64_t lddy, int32_t outer, int32_t rows, const float* ab, int32_t fuse_silu,
+                            float* sums, void* stream);
+/* backward pass 2: csum = the [outer][2][C] sums of pass 1 (svdx_tapgemm gnb_sum or svdx_groupnorm_bwd_sums). One launch,
+ * one pass over x and dy: every CTA folds the channel sums into the group sums, dgamma / dbeta (optional, fp32, accumulated)
+ * come straight from the channel sums. dres (optional, bf16 [outer*rows][lddres], single-source form only): a gradient
+ * already accumulated on x through its residual use; dx = GroupNorm backward + dres in the same pass. */
 int svdx_groupnorm_bwd_fused(const void* x, int64_t ldx, int32_t C1, const void* x2, int64_t ldx2, int32_t C2,
                              const void* dy, int64_t lddy, int32_t outer, int32_t rows, int32_t num_groups,
                              const float* mean, const float* rstd, const float* gamma, const float* beta,

@@ -68,19 +68,15 @@ _PROTOS = {
     "svdx_ipc_export": [c_void_p, c_void_p, c_void_p],
     "svdx_ipc_import": [c_void_p, c_i64, c_void_p],
     "svdx_struct_size": [c_int],
-    "svdx_groupnorm_stats": [c_void_p, c_i64, c_int, c_void_p, c_i64, c_int, c_int, c_int, c_int, c_float,
-                             c_void_p, c_void_p, c_void_p],
-    "svdx_groupnorm_apply": [c_void_p, c_i64, c_int, c_void_p, c_i64, c_int, c_int, c_int, c_int,
-                             c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_i64, c_void_p, c_void_p],
+    "svdx_groupnorm_sums": [c_void_p, c_i64, c_int, c_void_p, c_i64, c_int, c_int, c_int, c_void_p, c_i64, c_void_p],
     "svdx_groupnorm_apply_fused": [c_void_p, c_i64, c_int, c_void_p, c_i64, c_int, c_int, c_int, c_int, c_float,
                                    c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_i64, c_void_p,
                                    c_void_p],
     "svdx_groupnorm_bwd_fused": [c_void_p, c_i64, c_int, c_void_p, c_i64, c_int, c_void_p, c_i64, c_int, c_int, c_int,
                                  c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_i64, c_void_p, c_i64,
                                  c_void_p, c_void_p, c_void_p, c_i64, c_void_p],
-    "svdx_groupnorm_bwd": [c_void_p, c_i64, c_int, c_void_p, c_i64, c_int, c_void_p, c_i64, c_int, c_int, c_int,
-                           c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_i64, c_void_p, c_i64,
-                           c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_i64, c_void_p],
+    "svdx_groupnorm_bwd_sums": [c_void_p, c_i64, c_int, c_void_p, c_i64, c_int, c_void_p, c_i64, c_int, c_int, c_void_p, c_int,
+                                c_void_p, c_void_p],
     "svdx_layernorm_fwd": [c_void_p, c_i64, c_int, c_int, c_void_p, c_void_p, c_float, c_void_p, c_i64,
                            c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_i64, c_void_p],
     "svdx_layernorm_bwd": [c_void_p, c_i64, c_void_p, c_i64, c_int, c_int, c_void_p, c_void_p, c_void_p,

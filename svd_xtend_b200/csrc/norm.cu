@@ -23,33 +23,58 @@ struct GnSrc {
   int C2;
 };
 
-// ------------------------------------------------------------------ GroupNorm statistics
-// Vectorised: a thread owns ONE 8-channel vector (16 B) and walks rows, keeping 4 loads in flight; the block is
-// (C/8 channel vectors) x (row lanes). grid (row_chunks, outer). Accumulates sum / sumsq into mean[] / rstd[]
-// (pre-zeroed) through shared-memory then global fp32 atomics; finalised below.
 constexpr int GNV_MAX_THREADS = 512;
-constexpr int GN_RIF = 4;            // independent row loads per thread of the statistics kernel
+constexpr int GN_RIF = 4;            // independent row loads per thread of the channel-sum kernel
 #ifndef SVDX_LN_MINB
 #define SVDX_LN_MINB 1               // register-array LayerNorm kernels (C > 1280 only): minimum resident CTAs per SM
 #endif
+extern __shared__ uint4 gn_ring_smem[];
+
+// ------------------------------------------------------------------ GroupNorm channel sums
+// Every GroupNorm consumer reads its statistics as per-(slab, channel) sums, [outer][2][ld] fp32 and zero on entry: the
+// gn_sum / gnb_sum that svdx_tapgemm's epilogues accumulate (include/svd_xtend_b200.h). The two kernels below write the SAME
+// sums for a tensor no epilogue covered. Both end the same way: each active thread leaves its 8 channels' partials in
+// shared memory at part[(rl * 2 + moment) * C + c], and the block sums its RL row lanes there before one
+// red.global.add.v4.f32 per 4 channels and moment.
+SVDX_DEVINL void gn_csum_put(float* part, int C, int rl, int c0, const float (&a)[8], const float (&b)[8]) {
+  float* p = part + (2LL * rl) * C + c0;
+  *reinterpret_cast<float4*>(p) = make_float4(a[0], a[1], a[2], a[3]);
+  *reinterpret_cast<float4*>(p + 4) = make_float4(a[4], a[5], a[6], a[7]);
+  *reinterpret_cast<float4*>(p + C) = make_float4(b[0], b[1], b[2], b[3]);
+  *reinterpret_cast<float4*>(p + C + 4) = make_float4(b[4], b[5], b[6], b[7]);
+}
+
+SVDX_DEVINL void gn_csum_flush(const float* part, int C, int RL, float* out, long long ld) {
+  const int C4 = C / 4;
+  for (int i = threadIdx.x; i < 2 * C4; i += blockDim.x) {
+    const int m = i / C4, c = (i - m * C4) * 4;
+    float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 1                                     // unrolled, this tail would set the kernels' register count
+    for (int r = 0; r < RL; ++r) {
+      const float4 v = *reinterpret_cast<const float4*>(part + (2LL * r + m) * C + c);
+      t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w;
+    }
+    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(out + m * ld + c), "f"(t.x), "f"(t.y), "f"(t.z), "f"(t.w) : "memory");
+  }
+}
 
 SVDX_DEVINL uint4 load_vec8(const GnSrc& s, long long row, int c0) {
   const bf16* p = (c0 < s.C1) ? (s.x + row * s.ldx + c0) : (s.x2 + row * s.ldx2 + (c0 - s.C1));
   return *reinterpret_cast<const uint4*>(p);
 }
 
-__global__ void __launch_bounds__(GNV_MAX_THREADS, 1) gn_stats_partial(GnSrc s, int rows, int rows_per_cta, int G, float* sum, float* sumsq) {
-  __shared__ float sh_s[32 * 2];
+// forward: sum x, sum x^2 per (slab, channel) into sum[outer][2][ld] (the gn_sum layout). A thread owns ONE 8-channel vector
+// (16 B) and walks rows, keeping 4 loads in flight; the block is (C/8 channel vectors) x (row lanes), grid (row_chunks, outer),
+// dynamic shared memory 2 * C * RL floats for the row-lane reduction.
+__global__ void __launch_bounds__(GNV_MAX_THREADS, 1) gn_sums(GnSrc s, int rows, int rows_per_cta, float* sum, long long ld) {
   const int C = s.C1 + s.C2;
   const int CV = C / 8;
-  const int cpg = C / G;
   const int n = blockIdx.y;
   const int r0 = blockIdx.x * rows_per_cta;
   const int r1 = min(r0 + rows_per_cta, rows);
   const int RL = blockDim.x / CV;          // row lanes
   const int cv = threadIdx.x % CV, rl = threadIdx.x / CV;
-  for (int i = threadIdx.x; i < 2 * G; i += blockDim.x) sh_s[i] = 0.f;
-  __syncthreads();
+  float* part = reinterpret_cast<float*>(gn_ring_smem);
   if (rl < RL) {
     const int c0 = cv * 8;
     float a[8], b[8];
@@ -82,30 +107,10 @@ __global__ void __launch_bounds__(GNV_MAX_THREADS, 1) gn_stats_partial(GnSrc s, 
         b[2 * k] += v.x * v.x; b[2 * k + 1] += v.y * v.y;
       }
     }
-    // fold the 8 channels into their groups (consecutive channels -> non-decreasing group index)
-    int g = c0 / cpg, left = cpg - (c0 - g * cpg);
-    float sa = 0.f, sb = 0.f;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      if (left == 0) { atomicAdd(&sh_s[g], sa); atomicAdd(&sh_s[G + g], sb); sa = sb = 0.f; ++g; left = cpg; }
-      sa += a[k]; sb += b[k]; --left;
-    }
-    atomicAdd(&sh_s[g], sa); atomicAdd(&sh_s[G + g], sb);
+    gn_csum_put(part, C, rl, c0, a, b);
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < G; i += blockDim.x) {
-    atomicAdd(&sum[n * G + i], sh_s[i]);
-    atomicAdd(&sumsq[n * G + i], sh_s[G + i]);
-  }
-}
-
-__global__ void gn_stats_finalize(float* mean, float* rstd, int total, float inv_count, float eps) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const float m = mean[i] * inv_count;
-  const float var = fmaxf(rstd[i] * inv_count - m * m, 0.f);
-  mean[i] = m;
-  rstd[i] = rsqrtf(var + eps);
+  gn_csum_flush(part, C, RL, sum + (2LL * n) * ld, ld);
 }
 
 // ------------------------------------------------------------------ GroupNorm, cp.async ring variants
@@ -116,7 +121,6 @@ __global__ void gn_stats_finalize(float* mean, float* rstd, int total, float inv
 // flight, and the first GN_RING rows are requested BEFORE the statistics prologue so its L2 round trips overlap the first
 // HBM round trip. A thread only ever reads slots it filled itself: cp.async.wait_group is the only synchronisation.
 constexpr int GN_RING = 8;
-extern __shared__ uint4 gn_ring_smem[];
 
 SVDX_DEVINL void cp_async16(const void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
@@ -173,9 +177,8 @@ SVDX_DEVINL void gn_fold_csum(const GnSrc& s, int n, int C, int cpg, int G, floa
   __syncthreads();
 }
 
-// y = [silu](x * scale + shift). FUSED: statistics from the producer's per-channel sums (mean / rstd are OUTPUTS, published
-// by CTA x == 0 of the slab); otherwise mean / rstd are inputs. block = RL row lanes x CV channel vectors, padded to warps.
-template <bool FUSED>
+// y = [silu](x * scale + shift), statistics folded from the per-channel sums (mean / rstd are OUTPUTS, published by CTA
+// x == 0 of the slab). block = RL row lanes x CV channel vectors, padded to warps.
 __global__ void __launch_bounds__(GNV_MAX_THREADS, 2) gn_apply_ring(GnSrc s, int rows, int rows_per_cta, int RL, int G, float eps, float inv_count,
                                                                      const float* __restrict__ csum1, long long ldc1,
                                                                      const float* __restrict__ csum2, long long ldc2, float* mean, float* rstd,
@@ -212,13 +215,8 @@ __global__ void __launch_bounds__(GNV_MAX_THREADS, 2) gn_apply_ring(GnSrc s, int
     gm[0] = g0.x; gm[1] = g0.y; gm[2] = g0.z; gm[3] = g0.w; gm[4] = g1.x; gm[5] = g1.y; gm[6] = g1.z; gm[7] = g1.w;
     bt[0] = b0.x; bt[1] = b0.y; bt[2] = b0.z; bt[3] = b0.w; bt[4] = b1.x; bt[5] = b1.y; bt[6] = b1.z; bt[7] = b1.w;
   }
-  if (FUSED) {
-    gn_fold_csum(s, n, C, cpg, G, inv_count, eps, csum1, ldc1, csum2, ldc2, sh_sum, sh_sq, sh_mean, sh_rstd);
-    if (blockIdx.x == 0 && threadIdx.x < G) { mean[n * G + threadIdx.x] = sh_mean[threadIdx.x]; rstd[n * G + threadIdx.x] = sh_rstd[threadIdx.x]; }
-  } else {
-    if (threadIdx.x < G) { sh_mean[threadIdx.x] = mean[n * G + threadIdx.x]; sh_rstd[threadIdx.x] = rstd[n * G + threadIdx.x]; }
-    __syncthreads();
-  }
+  gn_fold_csum(s, n, C, cpg, G, inv_count, eps, csum1, ldc1, csum2, ldc2, sh_sum, sh_sq, sh_mean, sh_rstd);
+  if (blockIdx.x == 0 && threadIdx.x < G) { mean[n * G + threadIdx.x] = sh_mean[threadIdx.x]; rstd[n * G + threadIdx.x] = sh_rstd[threadIdx.x]; }
   if (nit == 0) return;
   float sc[8], sh[8];
 #pragma unroll
@@ -256,18 +254,14 @@ __global__ void __launch_bounds__(GNV_MAX_THREADS, 2) gn_apply_ring(GnSrc s, int
   }
 }
 
-// backward pass 1 on raw moments: per channel a1 = sum(e * gamma), ax = sum(e * gamma * x), e = dy * silu'(z); the group
-// fold turns them into s1 = sum a1, s2 = rstd * (sum ax - mean * sum a1) (= sum e*gamma*xhat), so the row loop needs no
-// mean / rstd registers. dgamma = rstd * (sum e*x - mean * sum e), dbeta = sum e.
-template <bool DG>
-__global__ void __launch_bounds__(GNV_MAX_THREADS, 1) gn_bwd_partial_ring(GnSrc s, const bf16* __restrict__ dy, long long lddy, int rows, int rows_per_cta,
-                                                                           int RL, int G, const float* __restrict__ mean, const float* __restrict__ rstd,
-                                                                           const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                                           int fuse_silu, float* ws, float* dgamma, float* dbeta) {
-  __shared__ float sh_s[32 * 2];
+// backward pass 1 on raw moments: sum e, sum e*x per (slab, channel) into sum[outer][2][C] (the gnb_sum layout),
+// e = dy * silu'(x * scale + shift) with scale / shift read from the ab table the apply kernel wrote (only when fuse_silu).
+// gn_bwd_fused_ring folds them into the group sums and derives dgamma / dbeta from them. The row-lane reduction reuses
+// the ring memory, free once every thread has left its loop.
+__global__ void __launch_bounds__(GNV_MAX_THREADS, 1) gn_bwd_sums_ring(GnSrc s, const bf16* __restrict__ dy, long long lddy, int rows, int rows_per_cta,
+                                                                        int RL, const float* __restrict__ ab, int fuse_silu, float* sum) {
   const int C = s.C1 + s.C2;
   const int CV = C / 8;
-  const int cpg = C / G;
   const int n = blockIdx.y;
   const int r0 = blockIdx.x * rows_per_cta;
   const int r1 = min(r0 + rows_per_cta, rows);
@@ -290,20 +284,16 @@ __global__ void __launch_bounds__(GNV_MAX_THREADS, 1) gn_bwd_partial_ring(GnSrc 
     if (d < nit) { cp_async16(&ringx[d * bd], px + d * step); cp_async16(&ringd[d * bd], pd + d * dstep); }
     cp_async_commit();
   }
-  for (int i = threadIdx.x; i < 2 * G; i += bd) sh_s[i] = 0.f;
-  __syncthreads();
+  float S[8], SX[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) { S[k] = SX[k] = 0.f; }
   if (nit > 0) {
-    float gm[8], A[8], B[8];
+    float A[8], B[8];
+    if (fuse_silu) {
+      const float* a = ab + (2LL * n) * C + c0;
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      const int g = (c0 + k) / cpg;
-      gm[k] = gamma[c0 + k];
-      A[k] = rstd[n * G + g] * gm[k];
-      B[k] = beta[c0 + k] - mean[n * G + g] * A[k];
+      for (int k = 0; k < 8; ++k) { A[k] = a[k]; B[k] = a[C + k]; }
     }
-    float a1[8], ax[8], dg[8], db[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) { a1[k] = ax[k] = dg[k] = db[k] = 0.f; }
     for (int i = 0; i < nit; ++i) {
       cp_async_wait<GN_RING - 1>();
       const int slot = (i & (GN_RING - 1)) * bd;
@@ -317,126 +307,18 @@ __global__ void __launch_bounds__(GNV_MAX_THREADS, 1) gn_bwd_partial_ring(GnSrc 
           e0 *= silu_grad_f(fmaf(v.x, A[2 * k], B[2 * k]));
           e1 *= silu_grad_f(fmaf(v.y, A[2 * k + 1], B[2 * k + 1]));
         }
-        const float eg0 = e0 * gm[2 * k], eg1 = e1 * gm[2 * k + 1];
-        a1[2 * k] += eg0; a1[2 * k + 1] += eg1;
-        ax[2 * k] = fmaf(eg0, v.x, ax[2 * k]); ax[2 * k + 1] = fmaf(eg1, v.y, ax[2 * k + 1]);
-        if (DG) {
-          dg[2 * k] = fmaf(e0, v.x, dg[2 * k]); dg[2 * k + 1] = fmaf(e1, v.y, dg[2 * k + 1]);
-          db[2 * k] += e0; db[2 * k + 1] += e1;
-        }
+        S[2 * k] += e0; S[2 * k + 1] += e1;
+        SX[2 * k] = fmaf(e0, v.x, SX[2 * k]); SX[2 * k + 1] = fmaf(e1, v.y, SX[2 * k + 1]);
       }
       if (i + GN_RING < nit) { cp_async16(&ringx[slot], px + (i + GN_RING) * step); cp_async16(&ringd[slot], pd + (i + GN_RING) * dstep); }
       cp_async_commit();
     }
-    int g = c0 / cpg, left = cpg - (c0 - g * cpg);
-    float sa = 0.f, sb = 0.f;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      if (left == 0) { atomicAdd(&sh_s[g], sa); atomicAdd(&sh_s[G + g], sb); sa = sb = 0.f; ++g; left = cpg; }
-      sa += a1[k]; sb += ax[k]; --left;
-    }
-    atomicAdd(&sh_s[g], sa); atomicAdd(&sh_s[G + g], sb);
-    if (DG) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const int gk = (c0 + k) / cpg;
-        const float mu = mean[n * G + gk], rs = rstd[n * G + gk];
-        atomicAdd(&dgamma[c0 + k], rs * (dg[k] - mu * db[k]));
-        atomicAdd(&dbeta[c0 + k], db[k]);
-      }
-    }
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < G; i += bd) {
-    const float mu = mean[n * G + i], rs = rstd[n * G + i];
-    atomicAdd(&ws[(n * G + i) * 2 + 0], sh_s[i]);
-    atomicAdd(&ws[(n * G + i) * 2 + 1], rs * (sh_s[G + i] - mu * sh_s[i]));
-  }
-}
-
-// backward pass 2: dx = rstd*(e*gamma - t1 - xhat*t2) [+ dres] = e*A - x*P + Q [+ dres], A = rstd*gamma, P = rstd^2 * t2,
-// Q = mean*P - rstd*t1 (t1, t2 = s1, s2 / count)
-template <bool DRES>
-__global__ void __launch_bounds__(GNV_MAX_THREADS, 1) gn_bwd_apply_ring(GnSrc s, const bf16* __restrict__ dy, long long lddy, int rows, int rows_per_cta,
-                                                                         int RL, int G, const float* __restrict__ mean, const float* __restrict__ rstd,
-                                                                         const float* __restrict__ gamma, const float* __restrict__ beta, int fuse_silu,
-                                                                         const float* __restrict__ ws, float inv_count, bf16* __restrict__ dx,
-                                                                         long long lddx, bf16* __restrict__ dx2, long long lddx2,
-                                                                         const bf16* __restrict__ dres, long long lddres) {
-  const int C = s.C1 + s.C2;
-  const int CV = C / 8;
-  const int cpg = C / G;
-  const int n = blockIdx.y;
-  const int r0 = blockIdx.x * rows_per_cta;
-  const int r1 = min(r0 + rows_per_cta, rows);
-  const int cv = threadIdx.x % CV, rl = threadIdx.x / CV;
-  const int c0 = cv * 8;
-  const int bd = blockDim.x;
-  const int rr = r0 + rl;
-  const int nit = (rl < RL && rr < r1) ? (r1 - rr + RL - 1) / RL : 0;
-  if (nit == 0) return;
-  uint4* ringx = gn_ring_smem + threadIdx.x;
-  uint4* ringd = ringx + GN_RING * bd;
-  uint4* ringr = ringd + GN_RING * bd;
-  const long long base = (long long)n * rows;
-  const bool first = c0 < s.C1;
-  const long long ld = first ? s.ldx : s.ldx2;
-  const bf16* px = (first ? (s.x + c0) : (s.x2 + (c0 - s.C1))) + (base + rr) * ld;
-  const bf16* pd = dy + (base + rr) * lddy + c0;
-  const bf16* pr = DRES ? dres + (base + rr) * lddres + c0 : nullptr;
-  const long long step = (long long)RL * ld, dstep = (long long)RL * lddy, rstep = (long long)RL * lddres;
-#pragma unroll
-  for (int d = 0; d < GN_RING; ++d) {
-    if (d < nit) {
-      cp_async16(&ringx[d * bd], px + d * step);
-      cp_async16(&ringd[d * bd], pd + d * dstep);
-      if (DRES) cp_async16(&ringr[d * bd], pr + d * rstep);
-    }
-    cp_async_commit();
-  }
-  float A[8], B[8], P[8], Q[8];
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const int g = (c0 + k) / cpg;
-    const float mu = mean[n * G + g], rs = rstd[n * G + g];
-    const float t1 = ws[(n * G + g) * 2] * inv_count, t2 = ws[(n * G + g) * 2 + 1] * inv_count;
-    A[k] = rs * gamma[c0 + k];
-    B[k] = beta[c0 + k] - mu * A[k];
-    P[k] = rs * rs * t2;
-    Q[k] = mu * P[k] - rs * t1;
-  }
-  const long long ols = first ? lddx : lddx2;
-  bf16* po = (first ? (dx + c0) : (dx2 + (c0 - s.C1))) + (base + rr) * ols;
-  const long long ostep = (long long)RL * ols;
-  for (int i = 0; i < nit; ++i) {
-    cp_async_wait<GN_RING - 1>();
-    const int slot = (i & (GN_RING - 1)) * bd;
-    const uint4 ux = ringx[slot], ud = ringd[slot];
-    uint4 ur = make_uint4(0u, 0u, 0u, 0u);
-    if (DRES) ur = ringr[slot];
-    const uint32_t in[4] = {ux.x, ux.y, ux.z, ux.w}, din[4] = {ud.x, ud.y, ud.z, ud.w}, rin[4] = {ur.x, ur.y, ur.z, ur.w};
-    uint32_t out[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float2 v = unpack_bf16x2(in[k]), d = unpack_bf16x2(din[k]);
-      float e0 = d.x, e1 = d.y;
-      if (fuse_silu) {
-        e0 *= silu_grad_f(fmaf(v.x, A[2 * k], B[2 * k]));
-        e1 *= silu_grad_f(fmaf(v.y, A[2 * k + 1], B[2 * k + 1]));
-      }
-      float o0 = fmaf(e0, A[2 * k], fmaf(-v.x, P[2 * k], Q[2 * k]));
-      float o1 = fmaf(e1, A[2 * k + 1], fmaf(-v.y, P[2 * k + 1], Q[2 * k + 1]));
-      if (DRES) { const float2 r2 = unpack_bf16x2(rin[k]); o0 += r2.x; o1 += r2.y; }
-      out[k] = pack_bf16x2(o0, o1);
-    }
-    *reinterpret_cast<uint4*>(po + i * ostep) = make_uint4(out[0], out[1], out[2], out[3]);
-    if (i + GN_RING < nit) {
-      cp_async16(&ringx[slot], px + (i + GN_RING) * step);
-      cp_async16(&ringd[slot], pd + (i + GN_RING) * dstep);
-      if (DRES) cp_async16(&ringr[slot], pr + (i + GN_RING) * rstep);
-    }
-    cp_async_commit();
-  }
+  float* part = reinterpret_cast<float*>(gn_ring_smem);
+  if (active) gn_csum_put(part, C, rl, c0, S, SX);
+  __syncthreads();
+  gn_csum_flush(part, C, RL, sum + (2LL * n) * C, C);
 }
 
 // ------------------------------------------------------------------ LayerNorm
@@ -637,9 +519,11 @@ __global__ void __launch_bounds__(256, SVDX_LN_MINB) ln_bwd_kernel(const bf16* _
   }
 }
 
-// backward pass 2 when pass 1 ran inside the dgrad epilogue (svdx_tapgemm gnb_sum): every CTA folds the per-channel sums
+// backward pass 2, from the per-channel sums of pass 1 (svdx_tapgemm's gnb_sum, or gn_bwd_sums_ring): every CTA folds
 // S_c = sum e, SX_c = sum e*x of its slab into s1_g = sum_c gamma_c S_c and sx_g = sum_c gamma_c SX_c (C values from L2), then
-// streams rows exactly as gn_bwd_apply_ring. CTA x == 0 of a slab also emits dgamma_c += rstd (SX_c - mean S_c), dbeta_c += S_c.
+// streams rows: dx = rstd*(e*gamma - t1 - xhat*t2) [+ dres] = e*A - x*P + Q [+ dres], A = rstd*gamma, P = rstd^2 * t2,
+// Q = mean*P - rstd*t1 (t1 = s1 / count, t2 = rstd * (sx - mean * s1) / count). CTA x == 0 of a slab also emits
+// dgamma_c += rstd (SX_c - mean S_c), dbeta_c += S_c.
 template <bool DRES>
 __global__ void __launch_bounds__(GNV_MAX_THREADS, 1) gn_bwd_fused_ring(GnSrc s, const bf16* __restrict__ dy, long long lddy, int rows, int rows_per_cta,
                                                                          int RL, int G, const float* __restrict__ mean, const float* __restrict__ rstd,
@@ -1036,34 +920,32 @@ __global__ void __launch_bounds__(LnRing<NJ>::W_BWD * 32, 1) ln_bwd_ring(const b
 
 using namespace svdx;
 
-// block = (C/8 channel vectors) x (row lanes) threads; rows per CTA chosen so that ~4 CTAs per SM exist
+// block = (C/8 channel vectors) x (row lanes) threads, ~8 CTAs per SM; each thread streams a multiple of 4 rows (4
+// independent 16-byte loads in flight), and at least 16: a CTA's 2 * C channel-sum reds then stay small next to the rows it
+// read (fewer rows made the reds the bottleneck at C = 640 / 1280)
 static void gn_vec_config(int C, int outer, int rows, int& threads, int& rows_per_cta) {
   const int CV = C / 8;
   int RL = 256 / CV;
   if (RL < 1) RL = 1;
   threads = CV * RL;
-  // ~8 CTAs per SM (tunable for experiments: SVDX_GN_CTAS_PER_SM), each thread streams a multiple of 4 rows (4 independent
-  // 16-byte loads per tensor in flight)
-  static int cps = 0;
-  if (cps == 0) { const char* e = getenv("SVDX_GN_CTAS_PER_SM"); cps = (e && atoi(e) > 0) ? atoi(e) : 8; }
-  const long long want_ctas = (long long)cps * svdx_num_sms();
+  const long long want_ctas = 8LL * svdx_num_sms();
   long long chunks = (want_ctas + outer - 1) / outer;
   if (chunks < 1) chunks = 1;
   rows_per_cta = (int)((rows + chunks - 1) / chunks);
   const int quantum = GN_RIF * RL;
   rows_per_cta = ((rows_per_cta + quantum - 1) / quantum) * quantum;
+  if (rows_per_cta < 4 * quantum) rows_per_cta = 4 * quantum;
 }
 
-// ring kernels: block = RL x CV threads padded to whole warps, ~SVDX_GN_RING_CPS CTAs per SM (each thread then walks
-// enough rows to amortise the ring fill), dynamic shared memory GN_RING slots x 16 B x threads per streamed tensor
+// ring kernels: block = RL x CV threads padded to whole warps, ~2 CTAs per SM (each thread then walks enough rows to amortise
+// the ring fill; in-step A/B on one box: 2 <= 3 < 1 < 4 < 6), dynamic shared memory GN_RING slots x 16 B x threads per
+// streamed tensor
 static void gn_ring_config(int C, int outer, int rows, int& threads, int& RL, int& rows_per_cta) {
   const int CV = C / 8;
   RL = 256 / CV;
   if (RL < 1) RL = 1;
   threads = (CV * RL + 31) & ~31;
-  static int cps = 0;
-  if (cps == 0) { const char* e = getenv("SVDX_GN_RING_CPS"); cps = (e && atoi(e) > 0) ? atoi(e) : 2; }   // in-step A/B (same box): 2 <= 3 < 1 < 4 < 6
-  const long long want_ctas = (long long)cps * svdx_num_sms();
+  const long long want_ctas = 2LL * svdx_num_sms();
   long long chunks = (want_ctas + outer - 1) / outer;
   if (chunks < 1) chunks = 1;
   rows_per_cta = (int)((rows + chunks - 1) / chunks);
@@ -1077,59 +959,31 @@ static void gn_ring_attr(K kernel, bool* done) {
   if (!done[slot]) { cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GN_RING_SMEM_MAX); done[slot] = true; }
 }
 
-static int gn_check(int C1, int C2, int G, int64_t ldx, int64_t ldx2, const void* x, const void* x2) {
+// the one or two bf16 sources: whole 8-channel vectors, at most GNV_MAX_THREADS of them per row, 16-byte aligned rows
+static int gn_check(int C1, int C2, int64_t ldx, int64_t ldx2, const void* x, const void* x2) {
   const int C = C1 + C2;
-  if (!x || G <= 0 || G > 32 || C % G || (C / G) % 2 || C % 8 || C1 % 8 || C2 % 8 || C / 8 > GNV_MAX_THREADS) return 1;
+  if (!x || C <= 0 || C % 8 || C1 % 8 || C2 % 8 || C / 8 > GNV_MAX_THREADS) return 1;
   if (C2 > 0 && !x2) return 1;
   if (ldx % 8 || (C2 > 0 && ldx2 % 8)) return 1;
   if ((reinterpret_cast<uintptr_t>(x) & 15) || (x2 && (reinterpret_cast<uintptr_t>(x2) & 15))) return 1;
   return 0;
 }
 
-extern "C" int svdx_groupnorm_stats(const void* x, int64_t ldx, int32_t C1, const void* x2, int64_t ldx2, int32_t C2, int32_t outer,
-                                    int32_t rows, int32_t num_groups, float eps, float* mean, float* rstd, void* stream_v) {
+// at most 32 groups (the consumers' shared-memory group tables) of an even number of channels
+static int gn_groups_bad(int C, int G) { return G <= 0 || G > 32 || C % G || (C / G) % 2; }
+
+extern "C" int svdx_groupnorm_sums(const void* x, int64_t ldx, int32_t C1, const void* x2, int64_t ldx2, int32_t C2, int32_t outer,
+                                   int32_t rows, float* sums, int64_t ld, void* stream_v) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-  if (gn_check(C1, C2, num_groups, ldx, ldx2, x, x2) || outer <= 0 || rows <= 0 || !mean || !rstd)
-    return svdx_fail(SVDX_E_BADARG, "groupnorm_stats: bad arguments");
+  if (gn_check(C1, C2, ldx, ldx2, x, x2) || outer <= 0 || rows <= 0 || !sums || (reinterpret_cast<uintptr_t>(sums) & 15) || ld < C1 + C2 || ld % 4)
+    return svdx_fail(SVDX_E_BADARG, "groupnorm_sums: bad arguments");
   GnSrc s{reinterpret_cast<const bf16*>(x), ldx, C1, reinterpret_cast<const bf16*>(x2), ldx2, C2};
-  const int total = outer * num_groups;
-  if (rstd == mean + total) {
-    cudaMemsetAsync(mean, 0, sizeof(float) * 2 * total, st);   // adjacent accumulators: one memset node in a captured graph
-  } else {
-    cudaMemsetAsync(mean, 0, sizeof(float) * total, st);
-    cudaMemsetAsync(rstd, 0, sizeof(float) * total, st);
-  }
   int threads, rpc;
   gn_vec_config(C1 + C2, outer, rows, threads, rpc);
-  dim3 grid((rows + rpc - 1) / rpc, outer);
-  gn_stats_partial<<<grid, threads, 0, st>>>(s, rows, rpc, num_groups, mean, rstd);
-  const float inv = 1.0f / ((float)rows * (float)((C1 + C2) / num_groups));
-  gn_stats_finalize<<<(total + 127) / 128, 128, 0, st>>>(mean, rstd, total, inv, eps);
-  SVDX_CHECK_LAUNCH("groupnorm_stats");
+  // row-lane partials: 2 moments x 8 channels per thread
+  gn_sums<<<dim3((rows + rpc - 1) / rpc, outer), threads, (size_t)threads * 16 * sizeof(float), st>>>(s, rows, rpc, sums, ld);
+  SVDX_CHECK_LAUNCH("groupnorm_sums");
   return SVDX_OK;
-}
-
-extern "C" int svdx_groupnorm_apply(const void* x, int64_t ldx, int32_t C1, const void* x2, int64_t ldx2, int32_t C2, int32_t outer,
-                                    int32_t rows, int32_t num_groups, const float* mean, const float* rstd, const float* gamma,
-                                    const float* beta, int32_t fuse_silu, void* y, int64_t ldy, float* ab_out, void* stream_v) {
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-  if (gn_check(C1, C2, num_groups, ldx, ldx2, x, x2) || !y || ldy % 8 || (reinterpret_cast<uintptr_t>(y) & 15) || !mean || !rstd || !gamma || !beta ||
-      (reinterpret_cast<uintptr_t>(gamma) & 15) || (reinterpret_cast<uintptr_t>(beta) & 15) || (ab_out && ((reinterpret_cast<uintptr_t>(ab_out) & 15))))
-    return svdx_fail(SVDX_E_BADARG, "groupnorm_apply: bad arguments");
-  GnSrc s{reinterpret_cast<const bf16*>(x), ldx, C1, reinterpret_cast<const bf16*>(x2), ldx2, C2};
-  int threads, rpc;
-  {
-    static bool attr[SVDX_MAX_DEVICES] = {false};
-    gn_ring_attr(gn_apply_ring<false>, attr);
-    int RL;
-    gn_ring_config(C1 + C2, outer, rows, threads, RL, rpc);
-    const float inv = 1.0f / ((float)rows * (float)((C1 + C2) / num_groups));
-    gn_apply_ring<false><<<dim3((rows + rpc - 1) / rpc, outer), threads, (size_t)GN_RING * threads * 16, st>>>(
-        s, rows, rpc, RL, num_groups, 0.f, inv, nullptr, 0, nullptr, 0, const_cast<float*>(mean), const_cast<float*>(rstd), gamma, beta, fuse_silu,
-        reinterpret_cast<bf16*>(y), ldy, ab_out);
-    SVDX_CHECK_LAUNCH("groupnorm_apply");
-    return SVDX_OK;
-  }
 }
 
 extern "C" int svdx_groupnorm_apply_fused(const void* x, int64_t ldx, int32_t C1, const void* x2, int64_t ldx2, int32_t C2, int32_t outer,
@@ -1137,66 +991,37 @@ extern "C" int svdx_groupnorm_apply_fused(const void* x, int64_t ldx, int32_t C1
                                           const float* csum2, int64_t ldc2, float* mean, float* rstd, const float* gamma,
                                           const float* beta, int32_t fuse_silu, void* y, int64_t ldy, float* ab_out, void* stream_v) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-  if (gn_check(C1, C2, num_groups, ldx, ldx2, x, x2) || !y || ldy % 8 || (reinterpret_cast<uintptr_t>(y) & 15) || !mean || !rstd || !gamma || !beta ||
-      (reinterpret_cast<uintptr_t>(gamma) & 15) || (reinterpret_cast<uintptr_t>(beta) & 15) || (ab_out && ((reinterpret_cast<uintptr_t>(ab_out) & 15))) ||
-      !csum1 || ldc1 < C1 || (C2 > 0 && (!csum2 || ldc2 < C2)) || outer <= 0 || rows <= 0)
+  if (gn_check(C1, C2, ldx, ldx2, x, x2) || gn_groups_bad(C1 + C2, num_groups) || !y || ldy % 8 || (reinterpret_cast<uintptr_t>(y) & 15) || !mean ||
+      !rstd || !gamma || !beta || (reinterpret_cast<uintptr_t>(gamma) & 15) || (reinterpret_cast<uintptr_t>(beta) & 15) ||
+      (ab_out && ((reinterpret_cast<uintptr_t>(ab_out) & 15))) || !csum1 || ldc1 < C1 || (C2 > 0 && (!csum2 || ldc2 < C2)) || outer <= 0 || rows <= 0)
     return svdx_fail(SVDX_E_BADARG, "groupnorm_apply_fused: bad arguments");
   GnSrc s{reinterpret_cast<const bf16*>(x), ldx, C1, reinterpret_cast<const bf16*>(x2), ldx2, C2};
-  int threads, rpc;
-  {
-    static bool attr[SVDX_MAX_DEVICES] = {false};
-    gn_ring_attr(gn_apply_ring<true>, attr);
-    int RLr;
-    gn_ring_config(C1 + C2, outer, rows, threads, RLr, rpc);
-    const float invr = 1.0f / ((float)rows * (float)((C1 + C2) / num_groups));
-    gn_apply_ring<true><<<dim3((rows + rpc - 1) / rpc, outer), threads, (size_t)GN_RING * threads * 16, st>>>(
-        s, rows, rpc, RLr, num_groups, eps, invr, csum1, ldc1, csum2, ldc2, mean, rstd, gamma, beta, fuse_silu, reinterpret_cast<bf16*>(y), ldy, ab_out);
-    SVDX_CHECK_LAUNCH("groupnorm_apply_fused");
-    return SVDX_OK;
-  }
+  static bool attr[SVDX_MAX_DEVICES] = {false};
+  gn_ring_attr(gn_apply_ring, attr);
+  int threads, RL, rpc;
+  gn_ring_config(C1 + C2, outer, rows, threads, RL, rpc);
+  const float inv = 1.0f / ((float)rows * (float)((C1 + C2) / num_groups));
+  gn_apply_ring<<<dim3((rows + rpc - 1) / rpc, outer), threads, (size_t)GN_RING * threads * 16, st>>>(
+      s, rows, rpc, RL, num_groups, eps, inv, csum1, ldc1, csum2, ldc2, mean, rstd, gamma, beta, fuse_silu, reinterpret_cast<bf16*>(y), ldy, ab_out);
+  SVDX_CHECK_LAUNCH("groupnorm_apply_fused");
+  return SVDX_OK;
 }
 
-extern "C" int svdx_groupnorm_bwd(const void* x, int64_t ldx, int32_t C1, const void* x2, int64_t ldx2, int32_t C2, const void* dy,
-                                  int64_t lddy, int32_t outer, int32_t rows, int32_t num_groups, const float* mean, const float* rstd,
-                                  const float* gamma, const float* beta, int32_t fuse_silu, void* dx, int64_t lddx, void* dx2,
-                                  int64_t lddx2, float* dgamma, float* dbeta, float* workspace, int32_t workspace_is_zero, const void* dres,
-                                  int64_t lddres, void* stream_v) {
+extern "C" int svdx_groupnorm_bwd_sums(const void* x, int64_t ldx, int32_t C1, const void* x2, int64_t ldx2, int32_t C2, const void* dy,
+                                       int64_t lddy, int32_t outer, int32_t rows, const float* ab, int32_t fuse_silu, float* sums, void* stream_v) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-  if (gn_check(C1, C2, num_groups, ldx, ldx2, x, x2) || !dy || lddy % 8 || !dx || lddx % 8 || (C2 > 0 && (!dx2 || lddx2 % 8)) || !workspace ||
-      (dgamma && !dbeta) || (dres && (C2 > 0 || lddres % 8 || (reinterpret_cast<uintptr_t>(dres) & 15))))
-    return svdx_fail(SVDX_E_BADARG, "groupnorm_bwd: bad arguments");
+  if (gn_check(C1, C2, ldx, ldx2, x, x2) || !dy || lddy % 8 || (reinterpret_cast<uintptr_t>(dy) & 15) || (fuse_silu && !ab) || !sums ||
+      (reinterpret_cast<uintptr_t>(sums) & 15) || outer <= 0 || rows <= 0)
+    return svdx_fail(SVDX_E_BADARG, "groupnorm_bwd_sums: bad arguments");
   GnSrc s{reinterpret_cast<const bf16*>(x), ldx, C1, reinterpret_cast<const bf16*>(x2), ldx2, C2};
-  const int total = outer * num_groups;
-  if (!workspace_is_zero) cudaMemsetAsync(workspace, 0, sizeof(float) * 2 * total, st);
-  int threads, rpc;
-  {
-    static bool a1[SVDX_MAX_DEVICES] = {false}, a2[SVDX_MAX_DEVICES] = {false}, a3[SVDX_MAX_DEVICES] = {false}, a4[SVDX_MAX_DEVICES] = {false};
-    gn_ring_attr(gn_bwd_partial_ring<true>, a1);
-    gn_ring_attr(gn_bwd_partial_ring<false>, a2);
-    gn_ring_attr(gn_bwd_apply_ring<true>, a3);
-    gn_ring_attr(gn_bwd_apply_ring<false>, a4);
-    int RL;
-    gn_ring_config(C1 + C2, outer, rows, threads, RL, rpc);
-    dim3 gridr((rows + rpc - 1) / rpc, outer);
-    const size_t slab = (size_t)GN_RING * threads * 16;
-    const bf16* dyb = reinterpret_cast<const bf16*>(dy);
-    if (dgamma)
-      gn_bwd_partial_ring<true><<<gridr, threads, 2 * slab, st>>>(s, dyb, lddy, rows, rpc, RL, num_groups, mean, rstd, gamma, beta, fuse_silu, workspace,
-                                                                   dgamma, dbeta);
-    else
-      gn_bwd_partial_ring<false><<<gridr, threads, 2 * slab, st>>>(s, dyb, lddy, rows, rpc, RL, num_groups, mean, rstd, gamma, beta, fuse_silu, workspace,
-                                                                    dgamma, dbeta);
-    const float invr = 1.0f / ((float)rows * (float)((C1 + C2) / num_groups));
-    if (dres)
-      gn_bwd_apply_ring<true><<<gridr, threads, 3 * slab, st>>>(s, dyb, lddy, rows, rpc, RL, num_groups, mean, rstd, gamma, beta, fuse_silu, workspace, invr,
-                                                                 reinterpret_cast<bf16*>(dx), lddx, reinterpret_cast<bf16*>(dx2), lddx2,
-                                                                 reinterpret_cast<const bf16*>(dres), lddres);
-    else
-      gn_bwd_apply_ring<false><<<gridr, threads, 2 * slab, st>>>(s, dyb, lddy, rows, rpc, RL, num_groups, mean, rstd, gamma, beta, fuse_silu, workspace, invr,
-                                                                  reinterpret_cast<bf16*>(dx), lddx, reinterpret_cast<bf16*>(dx2), lddx2, nullptr, 0);
-    SVDX_CHECK_LAUNCH("groupnorm_bwd");
-    return SVDX_OK;
-  }
+  static bool attr[SVDX_MAX_DEVICES] = {false};
+  gn_ring_attr(gn_bwd_sums_ring, attr);
+  int threads, RL, rpc;
+  gn_ring_config(C1 + C2, outer, rows, threads, RL, rpc);
+  gn_bwd_sums_ring<<<dim3((rows + rpc - 1) / rpc, outer), threads, (size_t)2 * GN_RING * threads * 16, st>>>(
+      s, reinterpret_cast<const bf16*>(dy), lddy, rows, rpc, RL, ab, fuse_silu, sums);
+  SVDX_CHECK_LAUNCH("groupnorm_bwd_sums");
+  return SVDX_OK;
 }
 
 extern "C" int svdx_groupnorm_bwd_fused(const void* x, int64_t ldx, int32_t C1, const void* x2, int64_t ldx2, int32_t C2, const void* dy,
@@ -1205,7 +1030,8 @@ extern "C" int svdx_groupnorm_bwd_fused(const void* x, int64_t ldx, int32_t C1, 
                                         void* dx2, int64_t lddx2, float* dgamma, float* dbeta, const void* dres, int64_t lddres,
                                         void* stream_v) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-  if (gn_check(C1, C2, num_groups, ldx, ldx2, x, x2) || !dy || lddy % 8 || (reinterpret_cast<uintptr_t>(dy) & 15) || !dx || lddx % 8 ||
+  if (gn_check(C1, C2, ldx, ldx2, x, x2) || gn_groups_bad(C1 + C2, num_groups) || !dy || lddy % 8 || (reinterpret_cast<uintptr_t>(dy) & 15) || !dx ||
+      lddx % 8 ||
       (reinterpret_cast<uintptr_t>(dx) & 15) || (C2 > 0 && (!dx2 || lddx2 % 8 || (reinterpret_cast<uintptr_t>(dx2) & 15))) || !csum || !mean || !rstd ||
       !gamma || !beta || (dgamma && !dbeta) || (dres && (C2 > 0 || lddres % 8 || (reinterpret_cast<uintptr_t>(dres) & 15))) || outer <= 0 || rows <= 0)
     return svdx_fail(SVDX_E_BADARG, "groupnorm_bwd_fused: bad arguments");

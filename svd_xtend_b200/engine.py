@@ -15,8 +15,6 @@ from __future__ import annotations
 
 from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
-import os
-
 import torch
 
 from . import raw
@@ -143,8 +141,6 @@ class Engine:
         # forward instead of one per GroupNorm (the buffers are consumed before the next forward zeroes them again)
         self._stat_arena: Optional[torch.Tensor] = None
         self._stat_ptr = 0
-        self.fuse_gn_stats = True
-        self.fuse_gn_bwd = os.environ.get("SVDX_GN_BWD_FUSE", "1") != "0"
 
     # ------------------------------------------------------------------ tape
     def begin(self, recording: bool):
@@ -172,8 +168,8 @@ class Engine:
 
     def _gn_sink(self, gn_rows: Optional[int], M: int, N: int, K: int, ntaps: int, device, n_out: Optional[int] = None):
         """channel-sum buffer for the fused GroupNorm statistics of a GEMM / conv output, or None when the launch cannot
-        carry them (split-K path, ragged widths) — the consumer then runs the stand-alone statistics kernel"""
-        if gn_rows is None or not self.fuse_gn_stats or N % 32 or M % gn_rows:
+        carry them (split-K path, ragged widths) — the consumer then runs the stand-alone channel-sum kernel"""
+        if gn_rows is None or N % 32 or M % gn_rows:
             return None
         if raw.split_plan(True, M, N, K, ntaps) is not None:
             return None
@@ -184,7 +180,7 @@ class Engine:
         writer of its gradient: the epilogue then also accumulates pass 1 of the GroupNorm backward (per-channel sums), and
         the GroupNorm's backward is ONE launch with one pass over x and dy. None when the launch cannot carry them."""
         ctx = x.gnb
-        if ctx is None or not self.fuse_gn_bwd or scales is not None or x.grad is not None or N % 32 or M % ctx["rows"] or N != ctx["C"] or M <= 8:
+        if ctx is None or scales is not None or x.grad is not None or N % 32 or M % ctx["rows"] or N != ctx["C"] or M <= 8:
             return None
         if raw.split_plan(True, M, N, K, ntaps) is not None:
             return None
@@ -771,8 +767,8 @@ class Engine:
     # ------------------------------------------------------------------ normalisation
     def groupnorm(self, x: Var, gn, outer: int, rows: int, silu: bool) -> Var:
         """GroupNorm(32) (+SiLU); one statistics group spans `rows` rows (H*W per frame, or T*H*W per clip).
-        When the producer(s) of x accumulated per-channel sums in their epilogues (x.csum, slab = `rows` rows), the group
-        statistics are folded from them inside the apply kernel: ONE launch, no pass over x for the statistics."""
+        The statistics are per-channel sums (slab = `rows` rows), folded into groups inside the apply kernel: those the
+        producer(s) of x accumulated in their epilogues (x.csum), else the stand-alone channel-sum kernel's."""
         C = x.cols
         gamma, beta = self.vec_f32(gn.weight), self.vec_f32(gn.bias)
         out = self.empty(x.rows, C, x.data)
@@ -780,17 +776,17 @@ class Engine:
         p_train = gn.weight.requires_grad
         need = x.needs_grad or p_train
         # per-channel scale / shift table for the backward sums fused into the consumer's dgrad epilogue (see _gnb_for)
-        ab = torch.empty(outer, 2, C, device=out.device, dtype=F32) if (need and self.recording and self.fuse_gn_bwd) else None
-        if cs is not None and cs[0] == rows and len(cs[1]) <= 2 and sum(c for _, c in cs[1]) == C and all(t.shape[0] == outer for t, _ in cs[1]):
-            parts = cs[1]
-            C1 = parts[0][1]
-            x1 = x.data if len(parts) == 1 else x.data[:, :C1]
-            x2 = None if len(parts) == 1 else x.data[:, C1:]
-            mean, rstd = raw.groupnorm_apply_fused(x1, x2, outer, rows, gn.eps, parts[0][0], None if len(parts) == 1 else parts[1][0],
-                                                   gamma, beta, silu, out, gn.num_groups, ab=ab)
-        else:
-            mean, rstd = raw.groupnorm_stats(x.data, None, outer, rows, gn.eps, gn.num_groups)
-            raw.groupnorm_apply(x.data, None, outer, rows, mean, rstd, gamma, beta, silu, out, gn.num_groups, ab=ab)
+        ab = torch.empty(outer, 2, C, device=out.device, dtype=F32) if (need and self.recording) else None
+        if not (cs is not None and cs[0] == rows and len(cs[1]) <= 2 and sum(c for _, c in cs[1]) == C
+                and all(t.shape[0] == outer for t, _ in cs[1])):
+            sums = raw.groupnorm_sums(x.data, None, outer, rows, self.stat_zeros(outer * 2 * C, out.device).view(outer, 2, C))
+            cs = (rows, [(sums, C)])
+        parts = cs[1]
+        C1 = parts[0][1]
+        x1 = x.data if len(parts) == 1 else x.data[:, :C1]
+        x2 = None if len(parts) == 1 else x.data[:, C1:]
+        mean, rstd = raw.groupnorm_apply_fused(x1, x2, outer, rows, gn.eps, parts[0][0], None if len(parts) == 1 else parts[1][0],
+                                               gamma, beta, silu, out, gn.num_groups, ab=ab)
         y = Var(out, need)
         if ab is not None:
             y.gnb = dict(x=x.data, x2=None, ab=ab, rows=rows, silu=silu, C=C)   # x.data is the (already concatenated) [M, C] tensor
@@ -808,12 +804,11 @@ class Engine:
                 dres = x.grad if (x.needs_grad and x.grad is not None and x.grad.dtype == bf16 and x.grad.shape == dx.shape
                                   and x.grad.stride(-1) == 1) else None
                 if fused is not None and fused[1] is dy:
-                    # pass 1 ran inside the dgrad epilogue that wrote dy: one launch, one pass over x and dy
-                    raw.groupnorm_bwd_fused(x.data, None, dy, outer, rows, mean, rstd, gamma, beta, silu, fused[0], dx, None, dg, db,
-                                            gn.num_groups, dres=dres)
+                    sums = fused[0]         # pass 1 ran inside the dgrad epilogue that wrote dy
                 else:
-                    ws = self.stat_zeros(2 * outer * gn.num_groups, dy.device)
-                    raw.groupnorm_bwd(x.data, None, dy, outer, rows, mean, rstd, gamma, beta, silu, dx, None, dg, db, gn.num_groups, ws=ws, dres=dres)
+                    sums = raw.groupnorm_bwd_sums(x.data, None, dy, outer, rows, ab, silu, self.stat_zeros(outer * 2 * C, dy.device).view(outer, 2, C))
+                raw.groupnorm_bwd_fused(x.data, None, dy, outer, rows, mean, rstd, gamma, beta, silu, sums, dx, None, dg, db,
+                                        gn.num_groups, dres=dres)
                 if dres is not None:
                     x.grad, x.owned = dx, True
                 else:

@@ -26,7 +26,7 @@ def dtype_code(t: torch.Tensor, what: str) -> int:
 
 # number of kernels launched through the C ABI since import (each wrapper adds what its entry point launches)
 LAUNCHES = [0]
-_KERNELS_PER_CALL = {"svdx_groupnorm_stats": 2, "svdx_groupnorm_bwd": 2, "svdx_groupnorm_apply_fused": 1, "svdx_attention_bwd": 3, "svdx_adamw_graph": 2, "svdx_adamw_p2p": 2,
+_KERNELS_PER_CALL = {"svdx_groupnorm_apply_fused": 1, "svdx_attention_bwd": 3, "svdx_adamw_graph": 2, "svdx_adamw_p2p": 2,
                      "svdx_adamw_graph_ema": 2, "svdx_adamw_p2p_ema": 2, "svdx_ema_multi": 2}
 
 
@@ -430,32 +430,26 @@ def attention_hd80_fwd(q, k, v, o, *, heads, S, nseq, scale):
 
 
 # ----------------------------------------------------------------------------- norms
-def groupnorm_stats(x, x2, outer, rows, eps, groups=32):
+def groupnorm_sums(x, x2, outer, rows, sums=None):
+    """per-(slab, channel) sum / sum of squares of x (| x2) into a ZEROED fp32 [outer, 2, >= C] (allocated when None): the
+    gn_sum buffer a producing tapgemm epilogue would have written"""
     C1 = x.shape[-1]
     C2 = x2.shape[-1] if x2 is not None else 0
-    stats = torch.empty(2, outer * groups, device=x.device, dtype=torch.float32)   # adjacent: zeroed by ONE memset node
-    mean, rstd = stats[0], stats[1]
+    if sums is None:
+        sums = torch.zeros(outer, 2, C1 + C2, device=x.device, dtype=torch.float32)
     if _fam("groupnorm", 0.0, 2.0 * x.shape[0] * (C1 + C2)):
-        return mean, rstd
-    check(load().svdx_groupnorm_stats(x.data_ptr(), _rowmajor(x, "x"), C1, _ptr(x2), _rowmajor(x2, "x2") if x2 is not None else 0,
-                                      C2, outer, rows, groups, eps, mean.data_ptr(), rstd.data_ptr(), _stream()), "svdx_groupnorm_stats")
-    return mean, rstd
-
-
-def groupnorm_apply(x, x2, outer, rows, mean, rstd, gamma, beta, silu, y, groups=32, ab=None):
-    C1 = x.shape[-1]
-    C2 = x2.shape[-1] if x2 is not None else 0
-    if _fam("groupnorm", 0.0, 4.0 * x.shape[0] * (C1 + C2)):
-        return y
-    check(load().svdx_groupnorm_apply(x.data_ptr(), _rowmajor(x, "x"), C1, _ptr(x2), _rowmajor(x2, "x2") if x2 is not None else 0,
-                                      C2, outer, rows, groups, mean.data_ptr(), rstd.data_ptr(), gamma.data_ptr(), beta.data_ptr(),
-                                      int(silu), y.data_ptr(), _rowmajor(y, "y"), _ptr(ab), _stream()), "groupnorm_apply")
-    return y
+        return sums
+    assert sums.dtype == torch.float32 and sums.dim() == 3 and sums.shape[:2] == (outer, 2) and sums.is_contiguous()
+    check(load().svdx_groupnorm_sums(x.data_ptr(), _rowmajor(x, "x"), C1, _ptr(x2), _rowmajor(x2, "x2") if x2 is not None else 0, C2,
+                                     outer, rows, sums.data_ptr(), sums.shape[2], _stream()), "svdx_groupnorm_sums")
+    return sums
 
 
 def groupnorm_apply_fused(x, x2, outer, rows, eps, csum1, csum2, gamma, beta, silu, y, groups=32, ab=None):
-    """GroupNorm(+SiLU) from the per-channel sums of the producing epilogues; returns (mean, rstd) [outer*groups] for backward.
-    ab: optional fp32 [outer, 2, C] that receives the per-channel scale / shift (for tapgemm's gnb_* backward sums)"""
+    """GroupNorm(+SiLU) from per-channel sums (the producing epilogues' gn_sum, or groupnorm_sums); returns (mean, rstd)
+    [outer*groups] for backward. csum1 / csum2: fp32 [outer, 2, >= C_i] with unit channel stride (csum2 may be a channel
+    slice of one buffer that covers both sources). ab: optional fp32 [outer, 2, C] that receives the per-channel scale / shift
+    (for the backward sums, tapgemm's gnb_* or groupnorm_bwd_sums)"""
     C1 = x.shape[-1]
     C2 = x2.shape[-1] if x2 is not None else 0
     stats = torch.empty(2, outer * groups, device=x.device, dtype=torch.float32)
@@ -463,33 +457,32 @@ def groupnorm_apply_fused(x, x2, outer, rows, eps, csum1, csum2, gamma, beta, si
     if _fam("groupnorm", 0.0, 4.0 * x.shape[0] * (C1 + C2)):
         return mean, rstd
     check(load().svdx_groupnorm_apply_fused(x.data_ptr(), _rowmajor(x, "x"), C1, _ptr(x2), _rowmajor(x2, "x2") if x2 is not None else 0, C2,
-                                            outer, rows, groups, eps, csum1.data_ptr(), csum1.shape[2],
-                                            _ptr(csum2), csum2.shape[2] if csum2 is not None else 0, mean.data_ptr(), rstd.data_ptr(),
+                                            outer, rows, groups, eps, csum1.data_ptr(), csum1.stride(1),
+                                            _ptr(csum2), csum2.stride(1) if csum2 is not None else 0, mean.data_ptr(), rstd.data_ptr(),
                                             gamma.data_ptr(), beta.data_ptr(), int(silu), y.data_ptr(), _rowmajor(y, "y"), _ptr(ab), _stream()),
           "svdx_groupnorm_apply_fused")
     return mean, rstd
 
 
-def groupnorm_bwd(x, x2, dy, outer, rows, mean, rstd, gamma, beta, silu, dx, dx2, dgamma=None, dbeta=None, groups=32, ws=None, dres=None):
-    """ws: optional pre-ZEROED float[2 * outer * groups] workspace (a slice of a zeroed arena: no memset node);
-    dres: gradient already accumulated on x (bf16, same shape), added to dx in the same pass"""
+def groupnorm_bwd_sums(x, x2, dy, outer, rows, ab, silu, sums=None):
+    """backward pass 1: sum e, sum e*x per (slab, channel) into a ZEROED fp32 [outer, 2, C] (allocated when None), e = dy *
+    silu'(x * scale + shift) with scale / shift from groupnorm_apply_fused's ab table: the gnb_sum a dgrad epilogue would have written"""
     C1 = x.shape[-1]
     C2 = x2.shape[-1] if x2 is not None else 0
-    ws_zero = ws is not None
-    if ws is None:
-        ws = torch.empty(outer * groups * 2, device=x.device, dtype=torch.float32)
-    if _fam("groupnorm", 0.0, 6.0 * x.shape[0] * (C1 + C2)):       # minimal traffic: read x, dy once, write dx
-        return
-    check(load().svdx_groupnorm_bwd(x.data_ptr(), _rowmajor(x, "x"), C1, _ptr(x2), _rowmajor(x2, "x2") if x2 is not None else 0, C2,
-                                    dy.data_ptr(), _rowmajor(dy, "dy"), outer, rows, groups, mean.data_ptr(), rstd.data_ptr(),
-                                    gamma.data_ptr(), beta.data_ptr(), int(silu), dx.data_ptr(), _rowmajor(dx, "dx"),
-                                    _ptr(dx2), _rowmajor(dx2, "dx2") if dx2 is not None else 0, _ptr(dgamma), _ptr(dbeta),
-                                    ws.data_ptr(), int(ws_zero), _ptr(dres), _rowmajor(dres, "dres") if dres is not None else 0, _stream()),
-          "svdx_groupnorm_bwd")
+    if sums is None:
+        sums = torch.zeros(outer, 2, C1 + C2, device=x.device, dtype=torch.float32)
+    if _fam("groupnorm", 0.0, 4.0 * x.shape[0] * (C1 + C2)):
+        return sums
+    assert sums.dtype == torch.float32 and sums.shape == (outer, 2, C1 + C2) and sums.is_contiguous()
+    check(load().svdx_groupnorm_bwd_sums(x.data_ptr(), _rowmajor(x, "x"), C1, _ptr(x2), _rowmajor(x2, "x2") if x2 is not None else 0, C2,
+                                         dy.data_ptr(), _rowmajor(dy, "dy"), outer, rows, _ptr(ab), int(silu), sums.data_ptr(), _stream()),
+          "svdx_groupnorm_bwd_sums")
+    return sums
 
 
 def groupnorm_bwd_fused(x, x2, dy, outer, rows, mean, rstd, gamma, beta, silu, csum, dx, dx2, dgamma=None, dbeta=None, groups=32, dres=None):
-    """GroupNorm backward from the per-channel sums the dgrad epilogue accumulated (tapgemm gnb_sum): one launch, one pass"""
+    """GroupNorm backward from the per-channel sums of pass 1 (tapgemm gnb_sum or groupnorm_bwd_sums): one launch, one pass;
+    dres: gradient already accumulated on x (bf16, same shape), added to dx in the same pass"""
     C1 = x.shape[-1]
     C2 = x2.shape[-1] if x2 is not None else 0
     if _fam("groupnorm", 0.0, 6.0 * x.shape[0] * (C1 + C2)):

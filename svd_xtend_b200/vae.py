@@ -394,14 +394,13 @@ class AutoencoderKLTemporalDecoder(nn.Module):
         nimg = g.B * g.T
         M = nimg * g.HW
         out = E.empty(4 * M, O, x.data)
-        sink = E.stat_zeros(nimg * 2 * O, out.device).view(nimg, 2, O) if E.fuse_gn_stats else None
+        sink = E.stat_zeros(nimg * 2 * O, out.device).view(nimg, 2, O)
         b32 = E.vec_f32(conv.bias)
         for i, (ph, pw) in enumerate(PHASES):
             raw.tapgemm(x.data, wf[i], out, M=M, N=O, K=I, mode=raw.A_CONV2D, taps=phase_taps(ph, pw), conv_whn=(g.W, g.H, nimg),
-                        bias=b32, gn_sum=sink, gn_rows=g.HW if sink is not None else 0, phase=(ph, pw))
+                        bias=b32, gn_sum=sink, gn_rows=g.HW, phase=(ph, pw))
         y = Var(out)
-        if sink is not None:
-            y.csum = (4 * g.HW, [(sink, O)])
+        y.csum = (4 * g.HW, [(sink, O)])
         return y
 
     def _run_decode(self, z: torch.Tensor, T: int) -> torch.Tensor:

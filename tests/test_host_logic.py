@@ -146,7 +146,6 @@ def test_groupnorm_backward_fusion_is_decided_per_launch():
     from svd_xtend_b200 import raw
     from svd_xtend_b200.engine import Engine, Var
     E = Engine()
-    E.fuse_gn_bwd = True
     M, rows = 35840, 2560
     x = torch.zeros(M, 320, dtype=torch.bfloat16)
     y = Var(torch.zeros(M, 320, dtype=torch.bfloat16), needs_grad=True)

@@ -92,15 +92,17 @@ def test_attention_temporal_fwd_bwd(raw, B, T, HW, heads):
 
 @pytest.mark.parametrize("outer,rows,C1,C2,silu", [(14, 160, 320, 0, True), (3, 640, 1280, 640, True), (2, 14 * 40, 640, 0, False), (2, 100, 640, 320, True),
                                                   (1, 35841, 320, 0, True), (2, 9001, 320, 320, False)])   # long slabs: the cp.async rings wrap
-def test_groupnorm_fwd_bwd(raw, outer, rows, C1, C2, silu):
+def test_groupnorm_fwd_bwd_through_channel_sums(raw, outer, rows, C1, C2, silu):
+    """the stand-alone channel-sum kernels (one or two sources) feeding the same consumers as the epilogue sums"""
     C = C1 + C2
     x1 = _rand(outer * rows, C1, seed=5).to(bf16) + 0.5
     x2 = _rand(outer * rows, C2, seed=6).to(bf16) if C2 else None
     gamma = _rand(C, seed=7) * 0.2 + 1.0
     beta = _rand(C, seed=8) * 0.1
-    mean, rstd = raw.groupnorm_stats(x1, x2, outer, rows, 1e-5)
+    sums = raw.groupnorm_sums(x1, x2, outer, rows)
     y = torch.empty(outer * rows, C, device=DEV, dtype=bf16)
-    raw.groupnorm_apply(x1, x2, outer, rows, mean, rstd, gamma, beta, silu, y)
+    ab = torch.empty(outer, 2, C, device=DEV)
+    mean, rstd = raw.groupnorm_apply_fused(x1, x2, outer, rows, 1e-5, sums, sums[:, :, C1:] if C2 else None, gamma, beta, silu, y, ab=ab)
     torch.cuda.synchronize()
     xcat = torch.cat([x1, x2], 1) if C2 else x1
     xr = xcat.float().reshape(outer, rows, C).permute(0, 2, 1).requires_grad_(True)  # [outer, C, rows]
@@ -115,7 +117,8 @@ def test_groupnorm_fwd_bwd(raw, outer, rows, C1, C2, silu):
     dx2 = torch.zeros_like(x2) if C2 else None
     dgamma = torch.zeros(C, device=DEV)
     dbeta = torch.zeros(C, device=DEV)
-    raw.groupnorm_bwd(x1, x2, dy, outer, rows, mean, rstd, gamma, beta, silu, dx1, dx2, dgamma, dbeta)
+    bsums = raw.groupnorm_bwd_sums(x1, x2, dy, outer, rows, ab, silu)
+    raw.groupnorm_bwd_fused(x1, x2, dy, outer, rows, mean, rstd, gamma, beta, silu, bsums, dx1, dx2, dgamma, dbeta)
     torch.cuda.synchronize()
     ref.backward(dy.float().view(outer, rows, C).permute(0, 2, 1))
     dxr = xr.grad.permute(0, 2, 1).reshape(outer * rows, C)
@@ -127,7 +130,7 @@ def test_groupnorm_fwd_bwd(raw, outer, rows, C1, C2, silu):
     if not C2:      # residual gradient folded into the same pass (single-source form)
         dres = _rand(outer * rows, C, seed=10).to(bf16)
         dx3 = torch.zeros_like(x1)
-        raw.groupnorm_bwd(x1, None, dy, outer, rows, mean, rstd, gamma, beta, silu, dx3, None, dres=dres)
+        raw.groupnorm_bwd_fused(x1, None, dy, outer, rows, mean, rstd, gamma, beta, silu, bsums, dx3, None, dres=dres)
         torch.cuda.synchronize()
         _close(dx3, dxr + dres.float(), what="groupnorm dx + dres")
 
@@ -326,7 +329,7 @@ def test_multi_transpose_bit_exact(raw):
 
 @pytest.mark.parametrize("outer,rows,C1,C2,silu", [(14, 2560, 320, 0, True), (14, 160, 1280, 640, True), (2, 560, 640, 320, False),
                                                     (3, 40, 1280, 1280, True), (1, 1000, 64, 0, True)])
-def test_groupnorm_apply_fused_from_channel_sums(raw, outer, rows, C1, C2, silu):
+def test_groupnorm_fwd_bwd_from_given_channel_sums(raw, outer, rows, C1, C2, silu):
     """svdx_groupnorm_apply_fused: group statistics folded from per-channel sums (as the GEMM epilogues produce them), one or
     two channel-concatenated sources, against F.group_norm; mean / rstd published for the backward."""
     C = C1 + C2
@@ -340,7 +343,8 @@ def test_groupnorm_apply_fused_from_channel_sums(raw, outer, rows, C1, C2, silu)
         return torch.stack([v.sum(1), (v * v).sum(1)], dim=1).contiguous()      # [outer, 2, Ci]
 
     y = torch.empty(outer * rows, C, device=DEV, dtype=bf16)
-    mean, rstd = raw.groupnorm_apply_fused(x1, x2, outer, rows, 1e-5, sums(x1), sums(x2) if C2 else None, gamma, beta, silu, y)
+    ab = torch.empty(outer, 2, C, device=DEV)
+    mean, rstd = raw.groupnorm_apply_fused(x1, x2, outer, rows, 1e-5, sums(x1), sums(x2) if C2 else None, gamma, beta, silu, y, ab=ab)
     torch.cuda.synchronize()
     xcat = torch.cat([x1, x2], 1) if C2 else x1
     xr = xcat.float().reshape(outer, rows, C).permute(0, 2, 1)
@@ -351,12 +355,12 @@ def test_groupnorm_apply_fused_from_channel_sums(raw, outer, rows, C1, C2, silu)
     v = xr.reshape(outer, 32, -1)
     assert torch.allclose(mean.view(outer, 32), v.mean(-1), atol=1e-4, rtol=1e-4)
     assert torch.allclose(rstd.view(outer, 32), torch.rsqrt(v.var(-1, unbiased=False) + 1e-5), atol=1e-3, rtol=1e-3)
-    # the published statistics drive the (unchanged) backward kernels; zeroed-workspace form
+    # the published statistics and scale / shift table drive the backward kernels
     dy = _rand(outer * rows, C, seed=9).to(bf16)
     dx1 = torch.zeros_like(x1)
     dx2 = torch.zeros_like(x2) if C2 else None
-    ws = torch.zeros(2 * outer * 32, device=DEV)
-    raw.groupnorm_bwd(x1, x2, dy, outer, rows, mean, rstd, gamma, beta, silu, dx1, dx2, ws=ws)
+    bsums = raw.groupnorm_bwd_sums(x1, x2, dy, outer, rows, ab, silu)
+    raw.groupnorm_bwd_fused(x1, x2, dy, outer, rows, mean, rstd, gamma, beta, silu, bsums, dx1, dx2)
     torch.cuda.synchronize()
     xg = xcat.float().reshape(outer, rows, C).permute(0, 2, 1).requires_grad_(True)
     r2 = F.group_norm(xg, 32, gamma, beta, 1e-5)

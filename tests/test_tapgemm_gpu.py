@@ -306,6 +306,11 @@ def test_fused_groupnorm_sums_linear(raw, M, N, K, rows, res):
     ref = a.float() @ w.float().t() + bias + (r1.float() if res else 0)
     _close(out, ref, what="linear + gn_sum")
     _check_gn_sums(sums, out, rows, f"linear {M}x{N}x{K} rows {rows} res {res}")
+    # the stand-alone channel-sum kernel writes the buffer the epilogue wrote
+    alone = raw.groupnorm_sums(out, None, M // rows, rows)
+    _check_gn_sums(alone, out, rows, f"groupnorm_sums {M}x{N} rows {rows}")
+    err = ((alone - sums).abs().amax((0, 2)) / (sums.abs().amax((0, 2)) + 1e-9)).max().item()
+    assert err < 4e-5, f"groupnorm_sums vs the epilogue's gn_sum: {err:.3g}"
 
 
 @pytest.mark.parametrize("N,H,W,Cin,Cout,per_clip", [(14, 40, 64, 64, 320, False), (14, 5, 8, 128, 160, False), (14, 10, 16, 320, 640, True),
@@ -434,7 +439,7 @@ def _gnb_reference(x, dy, outer, rows, gamma, beta, silu):
 @pytest.mark.parametrize("M,N,K,rows,bn", [(35840, 320, 640, 2560, 320), (35840, 320, 640, 2560, 160), (2240, 640, 1280, 160, None),
                                            (560, 1280, 64, 40, None), (280, 320, 128, 40, None), (4480, 1280, 320, 2240, None)])
 @pytest.mark.parametrize("silu,concat", [(True, False), (False, False), (True, True)])
-def test_groupnorm_backward_sums_fused_into_the_dgrad_epilogue(raw, M, N, K, rows, bn, silu, concat):
+def test_groupnorm_backward_sums_of_the_dgrad_epilogue_and_the_standalone_kernel(raw, M, N, K, rows, bn, silu, concat):
     """the GEMM writes dy (the gradient of a GroupNorm output) and accumulates sum e, sum e*x per (slab, channel); the fused
     backward kernel turns them into dx / dgamma / dbeta: compared with F.group_norm's backward on the bf16 dy it stored"""
     outer = M // rows
@@ -446,10 +451,10 @@ def test_groupnorm_backward_sums_fused_into_the_dgrad_epilogue(raw, M, N, K, row
     C1 = N // 2 if concat else N
     x1 = x[:, :C1] if concat else x
     x2 = x[:, C1:] if concat else None
-    mean, rstd = raw.groupnorm_stats(x1, x2, outer, rows, 1e-5)
+    cs = raw.groupnorm_sums(x1, x2, outer, rows)
     y = torch.empty(M, N, device=_dev(), dtype=bf16)
     ab = torch.empty(outer, 2, N, device=_dev())
-    raw.groupnorm_apply(x1, x2, outer, rows, mean, rstd, gamma, beta, silu, y, ab=ab)
+    mean, rstd = raw.groupnorm_apply_fused(x1, x2, outer, rows, 1e-5, cs, cs[:, :, C1:] if concat else None, gamma, beta, silu, y, ab=ab)
     torch.cuda.synchronize()
     cpg = N // 32
     scale = rstd.view(outer, 32).repeat_interleave(cpg, 1) * gamma
@@ -467,6 +472,9 @@ def test_groupnorm_backward_sums_fused_into_the_dgrad_epilogue(raw, M, N, K, row
     SX = (e * x.float()).view(outer, rows, N).sum(1)
     tol = 2e-3 * (e.abs().view(outer, rows, N).sum(1).max().item())
     assert (sums[:, 0] - S).abs().max().item() < tol and (sums[:, 1] - SX).abs().max().item() < 2 * tol
+    # the stand-alone pass 1 on the same dy and scale / shift table writes the epilogue's sums
+    alone = raw.groupnorm_bwd_sums(x1, x2, dy, outer, rows, ab, silu)
+    assert (alone[:, 0] - sums[:, 0]).abs().max().item() < tol and (alone[:, 1] - sums[:, 1]).abs().max().item() < 2 * tol
     dx = torch.full((M, N), float("nan"), device=_dev(), dtype=bf16)
     dgamma = torch.zeros(N, device=_dev())
     dbeta = torch.zeros(N, device=_dev())
@@ -480,7 +488,7 @@ def test_groupnorm_backward_sums_fused_into_the_dgrad_epilogue(raw, M, N, K, row
     _close(dbeta, dbr, what="fused groupnorm dbeta")
 
 
-def test_groupnorm_backward_sums_conv3x3(raw):
+def test_groupnorm_backward_sums_of_a_conv3x3_dgrad(raw):
     Nimg, H, W, Cin, Cout = 14, 20, 32, 128, 640
     M = Nimg * H * W
     g = _rand(Nimg, H, W, Cin, seed=20).to(bf16)
@@ -490,10 +498,9 @@ def test_groupnorm_backward_sums_conv3x3(raw):
     gamma = _rand(Cout, seed=7) * 0.2 + 1.0
     beta = _rand(Cout, seed=8) * 0.1
     rows = H * W
-    mean, rstd = raw.groupnorm_stats(x, None, Nimg, rows, 1e-5)
     y = torch.empty(M, Cout, device=_dev(), dtype=bf16)
     ab = torch.empty(Nimg, 2, Cout, device=_dev())
-    raw.groupnorm_apply(x, None, Nimg, rows, mean, rstd, gamma, beta, True, y, ab=ab)
+    mean, rstd = raw.groupnorm_apply_fused(x, None, Nimg, rows, 1e-5, raw.groupnorm_sums(x, None, Nimg, rows), None, gamma, beta, True, y, ab=ab)
     dy = torch.empty(M, Cout, device=_dev(), dtype=bf16)
     sums = torch.zeros(Nimg, 2, Cout, device=_dev())
     raw.tapgemm(g.view(-1, Cin), wk, dy, M=M, N=Cout, K=Cin, mode=raw.A_CONV2D, taps=raw.CONV3x3_TAPS, conv_whn=(W, H, Nimg),
