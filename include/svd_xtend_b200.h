@@ -34,7 +34,11 @@ extern "C" {
                             the group read as zero (this is the (3,1,1) temporal conv / a linear) */
 #define SVDX_A_CONV2D 1  /* A is [nimg][H][W][K] channels-last; tap t reads pixel (h+tap_d1[t],
                             w+tap_d0[t]) of image n+tap_d2[t]; out-of-image reads are zero
-                            (3x3 conv padding=1, and the parity-plane form of the stride-2 conv) */
+                            (3x3 conv padding=1, and the parity-plane form of the stride-2 conv).
+                            Any width W: when 128 % W == 0 or W % 128 == 0 the tile's pixels are
+                            fetched as shifted row boxes; at every other width as one TMA im2col
+                            load per k-block (taps then need |tap_d0|, |tap_d1| <= 1). The two
+                            forms give bit-identical results; interleave keeps the box widths. */
 
 #define SVDX_OUT_BF16 0
 #define SVDX_OUT_F32 1
@@ -68,7 +72,7 @@ typedef struct SvdxTapGemm {
   int32_t a_mode;       /* SVDX_A_ROWS / SVDX_A_CONV2D */
   int32_t a_major_mn;   /* 0: A[m][k] k contiguous. 1 (ROWS, groups==1 only): memory is [k][m], m contiguous */
   int32_t rows_per_group, groups;      /* ROWS   */
-  int32_t W, H, nimg;                  /* CONV2D: 128 % W == 0, or W % 128 == 0 (wide images: a tile is 128 pixels of one row) */
+  int32_t W, H, nimg;                  /* CONV2D (and b_mode 1): any W > 0; see SVDX_A_CONV2D for how each width is tiled */
   int32_t num_taps;
   int32_t tap_d0[SVDX_MAX_TAPS];
   int32_t tap_d1[SVDX_MAX_TAPS];

@@ -103,6 +103,15 @@ SVDX_DEVINL void tma_load_4d(const CUtensorMap* m, uint32_t bar, uint32_t dst, i
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// im2col mode: c0 = first channel, (c1, c2, c3) = (w, h, n) of the first pixel in the map's start-pixel box; the pixels
+// walk that box (w, then h, then n) and each is read at (w + ow, h + oh, n)
+SVDX_DEVINL void tma_load_4d_im2col(const CUtensorMap* m, uint32_t bar, uint32_t dst, int c0, int c1, int c2, int c3, uint16_t ow,
+                                    uint16_t oh) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
+      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "h"(ow), "h"(oh)
+      : "memory");
+}
 
 // ---- TMA stores (shared -> global through a tensor map, bulk-group completion)
 SVDX_DEVINL void tma_store_3d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2) {

@@ -139,6 +139,48 @@ int svdx_make_tmap(CUtensorMap* out, const void* base, int rank, const uint64_t*
   return svdx_make_tmap_ex(out, base, 0, 128, rank, dims, strides, box);
 }
 
+typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                   const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*, CUtensorMapInterleave,
+                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+static EncodeIm2colFn get_encode_im2col() {
+  static EncodeIm2colFn fn = nullptr;
+  static bool tried = false;
+  if (!tried) {
+    tried = true;
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &p, cudaEnableDefault, &q);
+    if (e == cudaSuccess && q == cudaDriverEntryPointSuccess) fn = reinterpret_cast<EncodeIm2colFn>(p);
+  }
+  return fn;
+}
+
+int svdx_make_tmap_im2col(CUtensorMap* out, const void* base, const uint64_t* dims, const uint64_t* strides, int pixels_per_column) {
+  EncodeIm2colFn enc = get_encode_im2col();
+  if (!enc) return svdx_fail(SVDX_E_NODRIVER, "cuTensorMapEncodeIm2col unavailable (no CUDA driver?)");
+  cuuint64_t gdim[4];
+  cuuint64_t gstr[3];
+  cuuint32_t es[4] = {1, 1, 1, 1};
+  for (int i = 0; i < 4; ++i) gdim[i] = dims[i];
+  for (int i = 0; i < 3; ++i) gstr[i] = strides[i];
+  // the box of start pixels {w, h} runs from -1 to dim - 2: the top-left filter tap of every output pixel of a 3x3 conv
+  // with padding 1; a load adds its tap offset in [0, 2] and reads zero wherever that leaves the tensor
+  const int lower[2] = {-1, -1};
+  const int upper[2] = {-1, -1};
+  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), gdim, gstr, lower, upper, 64,
+                   (cuuint32_t)pixels_per_column, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    char buf[256];
+    snprintf(buf, sizeof(buf), "cuTensorMapEncodeIm2col failed (%d): dims %llu %llu %llu %llu pixels %d stride0 %llu", (int)r,
+             (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3],
+             pixels_per_column, (unsigned long long)strides[0]);
+    return svdx_fail(SVDX_E_CUDA, buf);
+  }
+  return 0;
+}
+
 extern "C" int svdx_struct_size(int which) {
   return which == 0 ? (int)sizeof(SvdxTapGemm) : which == 1 ? (int)sizeof(SvdxAttn) : -1;
 }

@@ -117,7 +117,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
 
   if (warp == PRODUCER_WARP) {
     // =========================== TMA producer ===========================
-    const bool conv_par = (p.a_mode == SVDX_A_CONV2D) && !p.a_mn && !p.b_mn && !p.geglu && !p.wtiles && (BLOCK_M / p.W) <= 32;
+    const bool conv_par = (p.a_mode == SVDX_A_CONV2D) && !p.a_mn && !p.b_mn && !p.geglu && !p.wtiles && !p.im2col && (BLOCK_M / p.W) <= 32;
     if (conv_par) {
       // warp-wide conv producer: lane 0 owns the barriers and the B tile, every lane with a row box issues it
       int stage = 0;
@@ -197,6 +197,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
         const int kb0 = ks * p.kb_per_split;
         const int kb1 = min(kb0 + p.kb_per_split, p.kb_total);
         const int n0 = nt * (p.geglu ? p.block_n / 2 : p.block_n);
+        // im2col A: the tile's first output pixel (n, h, w); one load per k-block walks its 128 pixels across rows and images
+        int iw = 0, ih = 0, in = 0;
+        if (p.im2col && p.a_mode == SVDX_A_CONV2D) {
+          const int row = mt * BLOCK_M / p.W;
+          iw = mt * BLOCK_M - row * p.W;
+          in = row / p.H;
+          ih = row - in * p.H;
+        }
         int tap = kb0 / p.kb_per_tap;
         int kci = kb0 - tap * p.kb_per_tap - 1;
         for (int kb = kb0; kb < kb1; ++kb) {
@@ -224,6 +232,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
             const int g = mt / p.tiles_per_group;
             const int t = mt - g * p.tiles_per_group;
             tma_load_3d(&p.tma, full, dA, kc, t * BLOCK_M + p.tap_d0[tap], g);
+          } else if (p.im2col) {
+            // any width: start pixel (w - 1, h - 1) of the padding-1 box, the tap as offsets; pixels past the last image of
+            // the tensor read as zero (rows past M are never stored)
+            tma_load_4d_im2col(&p.tma, full, dA, kc, iw - 1, ih - 1, in + p.tap_d2[tap], (uint16_t)(p.tap_d0[tap] + 1),
+                               (uint16_t)(p.tap_d1[tap] + 1));
           } else if (p.wtiles) {
             // wide images (VAE encoder, W = 256 / 512): the tile is 128 consecutive pixels of one image row; the shifted
             // box (w0 + dw, h + dh) is zero-filled where it leaves the image, which IS the convolution's padding
@@ -256,7 +269,16 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
             }
           }
           // ---- B
-          if (p.b_mn && p.b_mode == 1) {
+          if (p.b_mn && p.b_mode == 1 && p.im2col) {
+            // the conv weight gradient at any width: a k-block = 64 consecutive output pixels, one 64-pixel im2col load per
+            // 64-channel slab from start pixel (w - 1, h - 1) of the padding-1 box with the tap as offsets
+            const int pix0 = kb * BLOCK_K;
+            const int row = pix0 / p.W;
+            const int n = row / p.H;
+            for (int j = 0; j < p.block_n / 64; ++j)
+              tma_load_4d_im2col(&p.tmb, full, dB + j * 8192, n0 + 64 * j, pix0 - row * p.W - 1, row - n * p.H - 1, n + p.tap_d2[0],
+                                 (uint16_t)(p.tap_d0[0] + 1), (uint16_t)(p.tap_d1[0] + 1));
+          } else if (p.b_mn && p.b_mode == 1) {
             // B rows are the pixels of a channels-last image tensor read at a fixed 2-D shift (conv weight gradient):
             // a k-block = 64 consecutive output pixels; out-of-image reads are zero-filled by TMA
             const int dw = p.tap_d0[0], dh = p.tap_d1[0], dn = p.tap_d2[0];
@@ -433,16 +455,27 @@ int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p) {
     p.m_tiles = p.tiles_per_group * d->groups;
   } else if (d->a_mode == SVDX_A_CONV2D) {
     const bool wide = d->W > 128;
-    if (d->W <= 0 || (wide ? (d->W % 128 != 0) : (128 % d->W != 0)) || d->H <= 0 || d->nimg <= 0)
-      return svdx_fail(SVDX_E_BADARG, "tapgemm: conv2d needs W | 128 or 128 | W");
+    if (d->W <= 0 || d->H <= 0 || d->nimg <= 0) return svdx_fail(SVDX_E_BADARG, "tapgemm: conv2d needs W, H, images > 0");
+    // widths the row boxes tile (W | 128: a tile is whole image rows; 128 | W: a tile is part of one row) take the box
+    // path; every other width takes one im2col load per k-block, which crosses image rows and images
+    const bool boxes = wide ? (d->W % 128 == 0) : (128 % d->W == 0);
+    if (!boxes && d->interleave) return svdx_fail(SVDX_E_BADARG, "tapgemm: conv2d needs W | 128 or 128 | W");
     // M counts output pixels of the first `M / (H*W)` images; the tensor may hold more images (parity planes)
     uint64_t dims[4] = {(uint64_t)d->K, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->nimg};
     uint64_t strides[3] = {(uint64_t)d->lda * 2, (uint64_t)d->lda * 2 * d->W, (uint64_t)d->lda * 2 * d->W * d->H};
     uint32_t box[4] = {64, (uint32_t)(wide ? 128 : d->W), 1, 1};
-    rc = svdx_make_tmap(&p.tma, d->a, 4, dims, strides, box);
     p.max_bh_log2 = 0;
-    p.wtiles = wide ? d->W / 128 : 0;
-    for (int lg = 1; lg <= 4 && !rc && !wide; ++lg) {
+    if (!boxes) {
+      for (int i = 0; i < d->num_taps; ++i)
+        if (d->tap_d0[i] < -1 || d->tap_d0[i] > 1 || d->tap_d1[i] < -1 || d->tap_d1[i] > 1)
+          return svdx_fail(SVDX_E_BADARG, "tapgemm: conv2d at a width with neither W | 128 nor 128 | W needs taps with |dw|, |dh| <= 1");
+      rc = svdx_make_tmap_im2col(&p.tma, d->a, dims, strides, BLOCK_M);
+      p.im2col = 1;
+    } else {
+      rc = svdx_make_tmap(&p.tma, d->a, 4, dims, strides, box);
+    }
+    p.wtiles = (wide && boxes) ? d->W / 128 : 0;
+    for (int lg = 1; lg <= 4 && !rc && !wide && boxes; ++lg) {
       const int bh = 1 << lg;
       if (bh * d->W > BLOCK_M || bh > d->H) break;
       uint32_t boxh[4] = {64, (uint32_t)d->W, (uint32_t)bh, 1};
@@ -459,11 +492,19 @@ int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p) {
   if (rc) return rc;
 
   if (d->b_major_mn && d->b_mode == 1) {
-    if (d->W <= 0 || d->H <= 0 || d->nimg <= 0 || (d->W < 64 && 64 % d->W) || (d->W >= 64 && d->W % 64)) return svdx_fail(SVDX_E_BADARG, "tapgemm: b_mode 1 needs W | 64 or 64 | W");
+    if (d->W <= 0 || d->H <= 0 || d->nimg <= 0) return svdx_fail(SVDX_E_BADARG, "tapgemm: b_mode 1 needs W, H, images > 0");
     uint64_t dims[4] = {(uint64_t)d->N, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->nimg};
     uint64_t strides[3] = {(uint64_t)d->ldb * 2, (uint64_t)d->ldb * 2 * d->W, (uint64_t)d->ldb * 2 * d->W * d->H};
     uint32_t box[4] = {64, (uint32_t)(d->W >= 64 ? 64 : d->W), 1, 1};
-    rc = svdx_make_tmap(&p.tmb, d->b, 4, dims, strides, box);
+    // W | 64 or 64 | W: a k-block is whole rows or part of one row (boxes); any other width: 64-pixel im2col loads
+    if ((d->W < 64 && 64 % d->W) || (d->W >= 64 && d->W % 64)) {
+      if (d->tap_d0[0] < -1 || d->tap_d0[0] > 1 || d->tap_d1[0] < -1 || d->tap_d1[0] > 1)
+        return svdx_fail(SVDX_E_BADARG, "tapgemm: b_mode 1 at a width with neither W | 64 nor 64 | W needs a tap with |dw|, |dh| <= 1");
+      rc = svdx_make_tmap_im2col(&p.tmb, d->b, dims, strides, 64);
+      p.im2col = 1;
+    } else {
+      rc = svdx_make_tmap(&p.tmb, d->b, 4, dims, strides, box);
+    }
     p.W = d->W; p.H = d->H; p.nimg = d->K / (d->W * d->H);   // K = output pixels = images * H * W
     if ((long long)p.nimg * d->W * d->H != d->K) return svdx_fail(SVDX_E_BADARG, "tapgemm: b_mode 1 K must be images*H*W");
   } else if (d->b_major_mn && d->b_mode == 2) {

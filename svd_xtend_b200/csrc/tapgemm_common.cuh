@@ -34,6 +34,8 @@ struct __align__(64) TapGemmKParams {
   int rows_per_group, groups, tiles_per_group;
   int W, H, nimg;
   int wtiles;          // CONV2D with W > 128 (W % 128 == 0): a tile = 128 consecutive pixels of ONE image row, wtiles = W / 128 (else 0)
+  int im2col;          // the image operand (CONV2D A: tma, 128 pixels; b_mode 1 B: tmb, 64 pixels) is an im2col map: widths
+                       // the row boxes cannot tile (neither W | 128 nor 128 | W for A, W | 64 / 64 | W for B)
   int num_taps;
   int tap_d0[SVDX_MAX_TAPS], tap_d1[SVDX_MAX_TAPS], tap_d2[SVDX_MAX_TAPS];
   int M, N, K;

@@ -651,6 +651,7 @@ class UNetSpatioTemporalConditionModel(nn.Module):
     def forward(self, sample: torch.Tensor, timestep: Union[torch.Tensor, float, int], encoder_hidden_states: torch.Tensor,
                 added_time_ids: torch.Tensor, return_dict: bool = True):
         """Same contract as src/unet_spatio_temporal_condition.py:357-490."""
+        self._check_latent_size(sample)
         if not sample.is_cuda:
             raise RuntimeError("svd_xtend_b200: the UNet hot path only runs on a CUDA (sm_90a) device; there is no CPU fallback")
         self._validate(sample)
@@ -669,6 +670,15 @@ class UNetSpatioTemporalConditionModel(nn.Module):
         if not return_dict:
             return (out,)
         return UNetSpatioTemporalConditionOutput(sample=out)
+
+    def _check_latent_size(self, sample: torch.Tensor):
+        """every down block but the last halves the latent, and each up block concatenates the skip of the same size: the
+        latent height and width must be multiples of 2^(down blocks - 1). Any such size runs (the convolutions take any width)."""
+        f = 1 << (len(self.down_blocks) - 1)
+        H, W = sample.shape[-2], sample.shape[-1]
+        if H % f or W % f:
+            raise ValueError(f"svd_xtend_b200: the latent height and width must be multiples of 2^(number of down blocks - 1) = {f} "
+                             f"for the skip connections to line up; got {H}x{W}")
 
     def _validate(self, sample: torch.Tensor):
         """boundary checks, cached on (parameter count, dtype/device signature): every parameter on the sample's device

@@ -269,7 +269,11 @@ class AutoencoderKLTemporalDecoder(nn.Module):
 
     # ------------------------------------------------------------------ the encode path
     def encode(self, x: torch.Tensor, return_dict: bool = True):
-        """x [N, 3, H, W] (H, W multiples of 2^(levels-1); W | 128 or 128 | W at every level) -> object with `.latent_dist`"""
+        """x [N, 3, H, W] (H, W multiples of 2^(levels-1), any such size) -> object with `.latent_dist`"""
+        f = 1 << (len(self.config.block_out_channels) - 1)
+        if x.shape[-2] % f or x.shape[-1] % f:
+            raise ValueError(f"encode: the frame height and width must be multiples of 2^(levels - 1) = {f} (one stride-2 "
+                             f"downsample per level but the last); got {x.shape[-2]}x{x.shape[-1]}")
         if not x.is_cuda:
             raise RuntimeError("svd_xtend_b200: the VAE encode path only runs on a CUDA (sm_90a) device; there is no CPU fallback")
         if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
