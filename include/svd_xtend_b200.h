@@ -38,7 +38,7 @@ extern "C" {
                             Any width W: when 128 % W == 0 or W % 128 == 0 the tile's pixels are
                             fetched as shifted row boxes; at every other width as one TMA im2col
                             load per k-block (taps then need |tap_d0|, |tap_d1| <= 1). The two
-                            forms give bit-identical results; interleave keeps the box widths. */
+                            forms give bit-identical results, with or without interleave. */
 
 #define SVDX_OUT_BF16 0
 #define SVDX_OUT_F32 1
@@ -140,8 +140,9 @@ typedef struct SvdxTapGemm {
    * output row (n, h, w) of the low-res geometry {W, H, nimg} is written to row (n*2H + 2h + phase_h) * 2W + 2w + phase_w of
    * the [nimg][2H][2W][ldo] high-res output, so the four launches fill it without the upsampled input ever existing.
    * gn_sum slabs still count low-res rows (gn_rows = H*W: the four phases of a frame accumulate into one slab).
-   * Requires the plain bf16 TMA-store epilogue (bias only: no rowbias / residual / scales / GEGLU / split-K / gnb sums) and
-   * whole images per 32-row store chunk (W >= 32, or H*W % 32 == 0). */
+   * Requires the plain bf16 TMA-store epilogue (bias only: no rowbias / residual / scales / GEGLU / split-K / gnb sums).
+   * W >= 32: any W and H (a 32-row store chunk that crosses into the next image row or image is stored in two pieces).
+   * W < 32: W | 32 and H*W % 32 == 0 (each 32-row store chunk is whole rows of one image). */
   int32_t interleave;
   int32_t phase_h, phase_w;
   /* Activation epilogue (the MLP fc1 of the CLIP image encoder [transformers CLIPMLP]): out = act(acc + bias), bf16, with

@@ -8,7 +8,10 @@ on the im2col path. Both have identical FLOPs, so the ratio is the cost (or gain
   1. the config-2 train step of bench.py (seeded default-init SVD UNet, as-scripted trainable set, FusedAdamW, one CUDA graph),
      captured twice in one process: 14 x 320x512 (latent 40x64) and 14 x 512x320 (latent 64x40); the two graphs are replayed
      in alternating windows of K replays, medians of 3;
-  2. the VAE encode (no grad, eager) of 14 frames at 576x1024 and at 1024x576, alternating, CUDA events, medians of 3.
+  2. the VAE encode (no grad, eager) of 14 frames at 576x1024 and at 1024x576, alternating, CUDA events, medians of 3;
+  3. the temporal VAE decode (`sampling.decode_latents`, decode_chunk_size 8) of 14 frames at 576x1024 (latent 72x128) and at
+     1024x576 (latent 128x72), alternating, CUDA events, medians of 3. In portrait the phase-form upsample stores cross image
+     rows (widths 72, 144, 288).
 Also reported: the card name, its power limit and SM clock, read in one query. Writes nothing to the source tree.
 """
 import argparse
@@ -44,6 +47,7 @@ def main():
     args = ap.parse_args()
 
     from oracle.svd_vae_oracle import VAE_CONFIG
+    from svd_xtend_b200.sampling import decode_latents
     from svd_xtend_b200.train import FusedAdamW, GraphedStep, ParamArena
     from svd_xtend_b200.unet import UNetSpatioTemporalConditionModel
     from svd_xtend_b200.vae import AutoencoderKLTemporalDecoder
@@ -112,7 +116,7 @@ def main():
     # ---- 2. the VAE encode, landscape vs portrait
     torch.manual_seed(5)
     with torch.device(dev):
-        vae = AutoencoderKLTemporalDecoder(**VAE_CONFIG)
+        vae = AutoencoderKLTemporalDecoder(**VAE_CONFIG, with_decoder=True)
     vae.to(dev).eval().requires_grad_(False)
     g = torch.Generator(device="cpu").manual_seed(11)
     xs = {"landscape": (torch.rand(frames, 3, 576, 1024, generator=g) * 2 - 1).to(dev),
@@ -128,10 +132,28 @@ def main():
     enc = {f"{k}_ms": vmed[k] for k in vmed}
     enc.update({"portrait_over_landscape": vmed["portrait"] / vmed["landscape"], "windows_ms": vms,
                 "what": f"VAE encode of {frames} frames, 576x1024 vs 1024x576, no grad, eager, alternating windows of 3, medians of 3"})
+    del xs
+    torch.cuda.empty_cache()
+
+    # ---- 3. the temporal VAE decode, landscape vs portrait
+    lats = {"landscape": torch.randn(1, frames, 4, 72, 128, generator=g).to(dev),
+            "portrait": torch.randn(1, frames, 4, 128, 72, generator=g).to(dev)}
+    dms = {k: [] for k in lats}
+    with torch.no_grad():
+        for lat in lats.values():
+            decode_latents(vae, lat, 8)
+        for _ in range(3):
+            for k, lat in lats.items():
+                dms[k].append(window(lambda lat=lat: decode_latents(vae, lat, 8), 3))
+    dmed = {k: statistics.median(v) for k, v in dms.items()}
+    dec = {f"{k}_ms": dmed[k] for k in dmed}
+    dec.update({"portrait_over_landscape": dmed["portrait"] / dmed["landscape"], "windows_ms": dms,
+                "what": (f"decode_latents of {frames} frames, decode_chunk_size 8, 576x1024 vs 1024x576, no grad, eager, alternating "
+                         f"windows of 3, medians of 3")})
 
     line = {"metric": "portrait / landscape time of the config-2 train step (same FLOPs)", "value": train["portrait_over_landscape"],
             "unit": "ratio", "higher_is_better": False, "steps": steps, "warmup": warmup,
-            "data": "seeded default-init weights, synthetic batch", **card_details(0), "train_step": train, "vae_encode": enc}
+            "data": "seeded default-init weights, synthetic batch", **card_details(0), "train_step": train, "vae_encode": enc, "vae_decode": dec}
     sys.stdout.flush()
     print(json.dumps(line), flush=True)
 

@@ -459,7 +459,6 @@ int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p) {
     // widths the row boxes tile (W | 128: a tile is whole image rows; 128 | W: a tile is part of one row) take the box
     // path; every other width takes one im2col load per k-block, which crosses image rows and images
     const bool boxes = wide ? (d->W % 128 == 0) : (128 % d->W == 0);
-    if (!boxes && d->interleave) return svdx_fail(SVDX_E_BADARG, "tapgemm: conv2d needs W | 128 or 128 | W");
     // M counts output pixels of the first `M / (H*W)` images; the tensor may hold more images (parity planes)
     uint64_t dims[4] = {(uint64_t)d->K, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->nimg};
     uint64_t strides[3] = {(uint64_t)d->lda * 2, (uint64_t)d->lda * 2 * d->W, (uint64_t)d->lda * 2 * d->W * d->H};
@@ -604,7 +603,11 @@ int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p) {
     if (p.epi_mode != EPI_FAST || p.rowbias || p.split_k > 1 || p.gnb_sum)
       return svdx_fail(SVDX_E_BADARG, "tapgemm: interleave needs the plain bf16 TMA-store epilogue (bias only: no rowbias / residual / "
                                       "scales / GEGLU / split-K / gnb sums; N %% 32 == 0, aligned rows)");
-    if (p.W < 32 && (32 % p.W || (p.H * p.W) % 32))
+    // W >= 32: any width and height (a chunk that crosses into the next image row or image is finished by
+    // il_store_next_row); W < 32: the chunk is 32 / W whole rows of one image
+    if (p.W < 32 && 32 % p.W)
+      return svdx_fail(SVDX_E_BADARG, "tapgemm: interleave with W < 32 needs W | 32 (a store chunk is whole image rows)");
+    if (p.W < 32 && (p.H * p.W) % 32)
       return svdx_fail(SVDX_E_BADARG, "tapgemm: interleave with W < 32 needs H*W %% 32 == 0 (a store chunk must not straddle images)");
     const uint64_t rb = (uint64_t)d->ldo * 2;   // bytes per output row
     uint64_t dims[4] = {(uint64_t)n_out, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.nimg};
@@ -613,6 +616,7 @@ int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p) {
     const bf16* base = reinterpret_cast<const bf16*>(d->out) + (2LL * p.W * d->phase_h + d->phase_w) * d->ldo;
     rc = svdx_make_tmap_ex(&p.tmo, base, 0, 64, 4, dims, strides, box);
     if (rc) return rc;
+    p.il_out = const_cast<bf16*>(base);
     p.interleave = 1;
     p.epi_mode = EPI_FAST_IL;
   }

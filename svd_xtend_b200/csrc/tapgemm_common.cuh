@@ -74,6 +74,7 @@ struct __align__(64) TapGemmKParams {
   int probe;   // dev switch SVDX_EPI_PROBE: 1 = epilogue without global stores, 2 = no epilogue work at all
   int interleave;      // tmo is the 4-D phase view {n_out, W, H, nimg} of a 2x-upsampled output (EPI_FAST_IL*)
   int act;             // SVDX_ACT_GELU / SVDX_ACT_QUICK_GELU applied after the bias (EPI_FAST_ACT)
+  bf16* il_out;        // interleave: output row 0 of the phase (out + (2 W phase_h + phase_w) * ldo), for il_store_next_row
 };
 
 
@@ -236,7 +237,9 @@ SVDX_DEVINL void act32(float (&f)[32], int act) {
 }
 
 // TMA store of one staged 32-row chunk whose first row is row0 of group grp. Interleaved: the chunk is 32 consecutive pixels
-// of the low-res geometry, addressed through the 4-D phase view {column, w, h, image} (whole images per chunk: checked on the host).
+// of the low-res geometry, addressed through the 4-D phase view {column, w, h, image}. W < 32: the box is 32 / W whole rows
+// (whole images per chunk: checked on the host). W >= 32: the box is 32 pixels of one row, clipped at W by the map; the
+// pixels of a chunk that run past the end of the row are written by il_store_next_row.
 template <bool IL>
 SVDX_DEVINL void store_chunk(const TapGemmKParams& p, uint32_t src, int col, int row0, int grp) {
   if constexpr (IL) {
@@ -244,6 +247,25 @@ SVDX_DEVINL void store_chunk(const TapGemmKParams& p, uint32_t src, int col, int
     tma_store_4d(&p.tmo, src, col, w0, r % p.H, r / p.H);
   } else {
     tma_store_3d(&p.tmo, src, col, row0, grp);
+  }
+}
+
+// Interleaved store, W >= 32: a chunk whose first pixel w0 has fewer than 32 pixels left in its row (only at widths that are
+// not multiples of 32) continues in the next row, or in row 0 of the next image. The TMA store above wrote the part in the
+// first row. Each lane whose pixel lies in the next row writes its own 64-byte row from the staged (64B-swizzled) chunk.
+// Low-res pixel row r = n * H + h, column w lands on output row 4 W r + 2 w of the phase base.
+SVDX_DEVINL void il_store_next_row(const TapGemmKParams& p, uint32_t src, int col, int row0, int lane) {
+  const int k = p.W - row0 % p.W;   // pixels of the chunk in its first row
+  if (p.W < 32 || k >= 32 || lane < k || row0 + lane >= p.M) return;
+  const long long orow = 4LL * p.W * (row0 / p.W + 1) + 2 * (lane - k);
+  uint4* dst = reinterpret_cast<uint4*>(p.il_out + orow * p.ldo + col);
+  const uint32_t row = src + lane * 64;
+  const int sw = (lane >> 1) & 3;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    uint4 v;
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(row + ((j ^ sw) << 4)));
+    dst[j] = v;
   }
 }
 
@@ -331,6 +353,10 @@ SVDX_DEVINL void epilogue_fast(const TapGemmKParams& p, uint32_t t_base, long lo
       store_chunk<IL>(p, sbase, colA, row0, grp);
       if (hasB) store_chunk<IL>(p, sbase + 2048, colB, row0, grp);
       bulk_commit();
+    }
+    if constexpr (IL) {
+      il_store_next_row(p, sbase, colA, row0, lane);
+      if (hasB) il_store_next_row(p, sbase + 2048, colB, row0, lane);
     }
     if constexpr (GN) {
       gn_chunk_sums(p, sbase, lane, colA, n_out_total, m0, valid_rows);

@@ -191,10 +191,6 @@ def _mid_attention(E: Engine, a: _Attn, x: Var, g: Geom) -> Var:
     return E.linear(Var(o), a.to_out[0].weight, a.to_out[0].bias, res1=x, gn_rows=S)
 
 
-def _conv_tiles(W: int) -> bool:
-    return W > 0 and (W % 128 == 0 if W > 128 else 128 % W == 0)
-
-
 class DiagonalGaussianDistribution:
     """[D] vae.py DiagonalGaussianDistribution over the [N, 2*latent, h, w] moments (tiny tensors: plain torch ops)."""
 
@@ -357,13 +353,16 @@ class AutoencoderKLTemporalDecoder(nn.Module):
         return SimpleNamespace(sample=sample)
 
     def _check_decode_geometry(self, h: int, w: int):
-        """every level's 3x3 convs tile the width (W | 128 or 128 | W); the phase-form upsample stores whole images per 32-pixel
-        chunk (low-res W >= 32 or H*W % 32 == 0)"""
+        """A level at least 32 pixels wide takes any width and height: the 3x3 convs read widths the row boxes cannot tile
+        through im2col loads, and the phase-form upsample splits a 32-pixel store chunk that crosses image rows. A narrower
+        level needs W | 128 (below 32 the same as W | 32: a store chunk is whole image rows), and if it is upsampled also
+        H*W % 32 == 0 (a chunk is whole images). For latents whose sides are multiples of 8 (every size the UNet takes) this
+        accepts every width except 24, i.e. 192-pixel-wide frames."""
         levels = len(self.config.block_out_channels)
         for lv in range(levels):
             H, W = h << lv, w << lv
-            if not _conv_tiles(W):
-                raise ValueError(f"decode: latent width {w} gives width {W} at level {lv}; every level needs W | 128 or 128 | W")
+            if W < 32 and 128 % W:
+                raise ValueError(f"decode: latent width {w} gives width {W} at level {lv}; a level narrower than 32 pixels needs W | 128")
             if lv < levels - 1 and W < 32 and (H * W) % 32:
                 raise ValueError(f"decode: the 2x upsample at {H}x{W} needs H*W % 32 == 0 when W < 32")
 
