@@ -400,6 +400,23 @@ int svdx_adamw_p2p_ema(float* p, float* m, float* v, const void* const* grads, v
 int svdx_ema_multi(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, double* ema_state,
                    void* stream);
 
+/* Block-wise 8-bit AdamW (train_svd.py --use_8bit_adam: bitsandbytes.optim.AdamW8bit with its defaults; the update is stated
+ * in oracle/svd_adam8bit_oracle.py). One launch over many fp32 parameters, each a job of the DEVICE array
+ *   {float* p; const float* g; void* s1; void* s2; float* absmax1; float* absmax2; bf16* shadow; float* ema; int64 n; int64 quant}
+ * quant != 0: s1 / s2 are uint8 codes [n] into qmap1 (signed dynamic map, for m) / qmap2 (unsigned dynamic map, for v), with
+ * one fp32 absmax per 256-element block and moment (absmax[ceil(n / 256)]); blocks start at the parameter's first element.
+ * quant == 0: s1 / s2 are fp32 m / v [n] (parameters below min_8bit_size). shadow (optional): bf16 copy of the new p.
+ * block_prefix[j] = first 256-element block of job j, total_blocks = sum of ceil(n_j / 256). qmap1 / qmap2: DEVICE float[256],
+ * sorted, shared by every job of the launch. state = svdx_adamw_graph's float[8] (device, advanced by a 1-thread tick first), so
+ * the pair can be captured in a CUDA graph and replayed. Every operation is rounded separately (no FMA); no atomics. Aligned
+ * jobs (p, g, fp32 states, shadow, EMA 16-byte; codes 8-byte) take 16-byte loads, others a scalar path. Two launches. */
+int svdx_adamw8bit(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
+                   const float* qmap2, float* state, float grad_scale, void* stream);
+/* svdx_adamw8bit whose update also advances every job's fp32 EMA buffer (job.ema, required) from the new p
+ * (svdx_adamw_graph_ema's rule; the tick also advances ema_state). Two launches. */
+int svdx_adamw8bit_ema(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
+                       const float* qmap2, float* state, float grad_scale, double* ema_state, void* stream);
+
 /* many bf16 transposes dst[i][o] = src_base[src_off + o*I + i] in one launch (dgrad operands of all trainable linears).
  * jobs: device array of {int64 src_off; void* dst; int32 O; int32 I}; tile_prefix[j] = first 32x32 tile of job j. */
 int svdx_multi_transpose(const void* src_base, const void* jobs, const int32_t* tile_prefix, int32_t njobs, int32_t total_tiles,

@@ -119,6 +119,8 @@ _PROTOS = {
     "svdx_adamw_p2p_ema": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_i64, c_i64, c_void_p, c_float, c_int, c_void_p,
                            c_void_p, c_void_p],
     "svdx_ema_multi": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p],
+    "svdx_adamw8bit": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p],
+    "svdx_adamw8bit_ema": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p],
     "svdx_multi_transpose": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p],
 }
 

@@ -690,6 +690,194 @@ __global__ void __launch_bounds__(256) multi_ema_kernel(const EmaJob* __restrict
   }
 }
 
+// Block-wise 8-bit AdamW (bitsandbytes' AdamW8bit, Dettmers et al. 2022) over many parameters in ONE launch. A job is one
+// parameter; its elements split into 256-element blocks from its first element (the last may be shorter), each block one warp,
+// 8 elements per lane. An 8-bit job keeps m / v as uint8 codes into the signed / unsigned 256-entry maps plus one fp32 absmax
+// per block and moment; a job below min_8bit_size keeps fp32 m / v (the same arithmetic without quantisation). Every
+// operation is rounded separately (no FMA contraction), so results equal oracle/svd_adam8bit_oracle.py's torch ops bit for
+// bit. No atomics: deterministic.
+struct Adam8Job {
+  float* p;
+  const float* g;
+  void* s1;             // uint8 codes (quant) or fp32 m
+  void* s2;             // uint8 codes (quant) or fp32 v
+  float* absmax1;       // [ceil(n / 256)] (quant only)
+  float* absmax2;
+  bf16* shadow;         // optional bf16 copy of p
+  float* ema;           // optional fp32 EMA of p (the _ema entry point)
+  long long n;
+  long long quant;
+};
+constexpr int A8_BLOCK = 256;
+constexpr int A8_WARPS = 8;       // 256 threads per CTA, one warp per block at a time
+
+SVDX_DEVINL int a8_code(const float* mid, float x) {
+  // #{k : mid[k] < x} over 255 sorted midpoints (mid[255] = +inf): a tie goes to the lower code
+  int c = 0;
+#pragma unroll
+  for (int s = 128; s >= 1; s >>= 1)
+    if (mid[c + s - 1] < x) c += s;
+  return c;
+}
+
+template <bool EMA>
+__global__ void __launch_bounds__(256) adamw8bit_kernel(const Adam8Job* __restrict__ jobs, const int* __restrict__ block_prefix, int njobs,
+                                                        int total_blocks, const float* __restrict__ qmap1, const float* __restrict__ qmap2,
+                                                        const float* __restrict__ state, float gscale, const double* __restrict__ ema_state) {
+  __shared__ float q1[256], q2[256], mid1[256], mid2[256];
+  for (int k = threadIdx.x; k < 256; k += blockDim.x) {
+    q1[k] = qmap1[k];
+    q2[k] = qmap2[k];
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k < 256; k += blockDim.x) {
+    mid1[k] = k < 255 ? __fmul_rn(__fadd_rn(q1[k], q1[k + 1]), 0.5f) : INFINITY;
+    mid2[k] = k < 255 ? __fmul_rn(__fadd_rn(q2[k], q2[k + 1]), 0.5f) : INFINITY;
+  }
+  __syncthreads();
+  const float lr = state[0], b1 = state[1], b2 = state[2], eps = state[3], wd = state[4], bc1 = state[6], bc2 = state[7];
+  const float omb1 = __fsub_rn(1.f, b1), omb2 = __fsub_rn(1.f, b2);
+  const float decay = __fsub_rn(1.f, __fmul_rn(lr, wd)), step_size = __fdiv_rn(lr, bc1), sqrt_bc2 = __fsqrt_rn(bc2);
+  float omd = 0.f;
+  if constexpr (EMA) omd = (float)ema_state[8];
+  const int lane = threadIdx.x & 31;
+  for (int b = blockIdx.x * A8_WARPS + (threadIdx.x >> 5); b < total_blocks; b += gridDim.x * A8_WARPS) {
+    int lo = 0, hi = njobs - 1;
+    while (lo < hi) {            // last job whose first block <= b
+      const int mid = (lo + hi + 1) >> 1;
+      if (block_prefix[mid] <= b) lo = mid; else hi = mid - 1;
+    }
+    const Adam8Job j = jobs[lo];
+    const int blk = b - block_prefix[lo];
+    const long long base = (long long)blk * A8_BLOCK + lane * 8;
+    const long long rem = j.n - base;
+    const int cnt = rem >= 8 ? 8 : (rem > 0 ? (int)rem : 0);
+    const bool quant = j.quant != 0;
+    const uintptr_t a16 = reinterpret_cast<uintptr_t>(j.p) | reinterpret_cast<uintptr_t>(j.g) |
+                          (j.shadow ? reinterpret_cast<uintptr_t>(j.shadow) : 0) | (EMA ? reinterpret_cast<uintptr_t>(j.ema) : 0) |
+                          (quant ? 0 : reinterpret_cast<uintptr_t>(j.s1) | reinterpret_cast<uintptr_t>(j.s2));
+    const bool vec = cnt == 8 && (a16 & 15) == 0 &&
+                     (!quant || ((reinterpret_cast<uintptr_t>(j.s1) | reinterpret_cast<uintptr_t>(j.s2)) & 7) == 0);
+    float pp[8], gg[8], mm[8], vv[8];
+    if (vec) {
+      const float4 p0 = *reinterpret_cast<const float4*>(j.p + base), p1 = *reinterpret_cast<const float4*>(j.p + base + 4);
+      const float4 g0 = __ldg(reinterpret_cast<const float4*>(j.g + base)), g1 = __ldg(reinterpret_cast<const float4*>(j.g + base + 4));
+      pp[0] = p0.x; pp[1] = p0.y; pp[2] = p0.z; pp[3] = p0.w; pp[4] = p1.x; pp[5] = p1.y; pp[6] = p1.z; pp[7] = p1.w;
+      gg[0] = g0.x; gg[1] = g0.y; gg[2] = g0.z; gg[3] = g0.w; gg[4] = g1.x; gg[5] = g1.y; gg[6] = g1.z; gg[7] = g1.w;
+      if (quant) {
+        const uint2 c1 = *reinterpret_cast<const uint2*>(reinterpret_cast<const uint8_t*>(j.s1) + base);
+        const uint2 c2 = *reinterpret_cast<const uint2*>(reinterpret_cast<const uint8_t*>(j.s2) + base);
+        const float a1 = j.absmax1[blk], a2 = j.absmax2[blk];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          const uint32_t w1 = k < 4 ? c1.x : c1.y, w2 = k < 4 ? c2.x : c2.y;
+          mm[k] = __fmul_rn(q1[(w1 >> (8 * (k & 3))) & 255], a1);
+          vv[k] = __fmul_rn(q2[(w2 >> (8 * (k & 3))) & 255], a2);
+        }
+      } else {
+        const float* m = reinterpret_cast<const float*>(j.s1) + base;
+        const float* v = reinterpret_cast<const float*>(j.s2) + base;
+        const float4 m0 = *reinterpret_cast<const float4*>(m), m1 = *reinterpret_cast<const float4*>(m + 4);
+        const float4 v0 = *reinterpret_cast<const float4*>(v), v1 = *reinterpret_cast<const float4*>(v + 4);
+        mm[0] = m0.x; mm[1] = m0.y; mm[2] = m0.z; mm[3] = m0.w; mm[4] = m1.x; mm[5] = m1.y; mm[6] = m1.z; mm[7] = m1.w;
+        vv[0] = v0.x; vv[1] = v0.y; vv[2] = v0.z; vv[3] = v0.w; vv[4] = v1.x; vv[5] = v1.y; vv[6] = v1.z; vv[7] = v1.w;
+      }
+    } else {
+      const float a1 = quant && cnt ? j.absmax1[blk] : 0.f, a2 = quant && cnt ? j.absmax2[blk] : 0.f;
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        pp[k] = gg[k] = mm[k] = vv[k] = 0.f;
+        if (k < cnt) {
+          pp[k] = j.p[base + k];
+          gg[k] = j.g[base + k];
+          if (quant) {
+            mm[k] = __fmul_rn(q1[reinterpret_cast<const uint8_t*>(j.s1)[base + k]], a1);
+            vv[k] = __fmul_rn(q2[reinterpret_cast<const uint8_t*>(j.s2)[base + k]], a2);
+          } else {
+            mm[k] = reinterpret_cast<const float*>(j.s1)[base + k];
+            vv[k] = reinterpret_cast<const float*>(j.s2)[base + k];
+          }
+        }
+      }
+    }
+    float amax1 = 0.f, amax2 = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const float gi = __fmul_rn(gg[k], gscale);
+      mm[k] = __fadd_rn(__fmul_rn(b1, mm[k]), __fmul_rn(omb1, gi));
+      vv[k] = __fadd_rn(__fmul_rn(b2, vv[k]), __fmul_rn(__fmul_rn(omb2, gi), gi));
+      const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(vv[k]), sqrt_bc2), eps);
+      pp[k] = __fsub_rn(__fmul_rn(pp[k], decay), __fdiv_rn(__fmul_rn(step_size, mm[k]), denom));
+      if (k < cnt) {
+        amax1 = fmaxf(amax1, fabsf(mm[k]));
+        amax2 = fmaxf(amax2, vv[k]);
+      }
+    }
+    if (quant) {
+#pragma unroll
+      for (int o = 16; o >= 1; o >>= 1) {
+        amax1 = fmaxf(amax1, __shfl_xor_sync(0xffffffffu, amax1, o));
+        amax2 = fmaxf(amax2, __shfl_xor_sync(0xffffffffu, amax2, o));
+      }
+    }
+    if (vec) {
+      *reinterpret_cast<float4*>(j.p + base) = make_float4(pp[0], pp[1], pp[2], pp[3]);
+      *reinterpret_cast<float4*>(j.p + base + 4) = make_float4(pp[4], pp[5], pp[6], pp[7]);
+      if (quant) {
+        uint32_t w1[2] = {0u, 0u}, w2[2] = {0u, 0u};
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          const float x1 = amax1 > 0.f ? __fdiv_rn(mm[k], amax1) : 0.f, x2 = amax2 > 0.f ? __fdiv_rn(vv[k], amax2) : 0.f;
+          w1[k >> 2] |= (uint32_t)a8_code(mid1, x1) << (8 * (k & 3));
+          w2[k >> 2] |= (uint32_t)a8_code(mid2, x2) << (8 * (k & 3));
+        }
+        *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(j.s1) + base) = make_uint2(w1[0], w1[1]);
+        *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(j.s2) + base) = make_uint2(w2[0], w2[1]);
+      } else {
+        float* m = reinterpret_cast<float*>(j.s1) + base;
+        float* v = reinterpret_cast<float*>(j.s2) + base;
+        *reinterpret_cast<float4*>(m) = make_float4(mm[0], mm[1], mm[2], mm[3]);
+        *reinterpret_cast<float4*>(m + 4) = make_float4(mm[4], mm[5], mm[6], mm[7]);
+        *reinterpret_cast<float4*>(v) = make_float4(vv[0], vv[1], vv[2], vv[3]);
+        *reinterpret_cast<float4*>(v + 4) = make_float4(vv[4], vv[5], vv[6], vv[7]);
+      }
+      if (j.shadow)
+        *reinterpret_cast<uint4*>(j.shadow + base) = make_uint4(pack_bf16x2(pp[0], pp[1]), pack_bf16x2(pp[2], pp[3]),
+                                                                pack_bf16x2(pp[4], pp[5]), pack_bf16x2(pp[6], pp[7]));
+      if constexpr (EMA) {
+        float4 e0 = *reinterpret_cast<float4*>(j.ema + base), e1 = *reinterpret_cast<float4*>(j.ema + base + 4);
+        e0.x = ema_update(e0.x, pp[0], omd); e0.y = ema_update(e0.y, pp[1], omd);
+        e0.z = ema_update(e0.z, pp[2], omd); e0.w = ema_update(e0.w, pp[3], omd);
+        e1.x = ema_update(e1.x, pp[4], omd); e1.y = ema_update(e1.y, pp[5], omd);
+        e1.z = ema_update(e1.z, pp[6], omd); e1.w = ema_update(e1.w, pp[7], omd);
+        *reinterpret_cast<float4*>(j.ema + base) = e0;
+        *reinterpret_cast<float4*>(j.ema + base + 4) = e1;
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        if (k < cnt) {
+          j.p[base + k] = pp[k];
+          if (quant) {
+            const float x1 = amax1 > 0.f ? __fdiv_rn(mm[k], amax1) : 0.f, x2 = amax2 > 0.f ? __fdiv_rn(vv[k], amax2) : 0.f;
+            reinterpret_cast<uint8_t*>(j.s1)[base + k] = (uint8_t)a8_code(mid1, x1);
+            reinterpret_cast<uint8_t*>(j.s2)[base + k] = (uint8_t)a8_code(mid2, x2);
+          } else {
+            reinterpret_cast<float*>(j.s1)[base + k] = mm[k];
+            reinterpret_cast<float*>(j.s2)[base + k] = vv[k];
+          }
+          if (j.shadow) j.shadow[base + k] = __float2bfloat16_rn(pp[k]);
+          if constexpr (EMA) j.ema[base + k] = ema_update(j.ema[base + k], pp[k], omd);
+        }
+      }
+    }
+    if (quant && lane == 0) {
+      j.absmax1[blk] = amax1;
+      j.absmax2[blk] = amax2;
+    }
+  }
+}
+
 // row softmax of a bf16 score matrix, y[r][:] = softmax(scale * x[r][:]) (fp32 arithmetic, in place allowed): the single-head,
 // head_dim 512 attention of the VAE encoder's mid block goes through two GEMMs and this kernel (its S x S scores are small).
 // One CTA per row; a row of <= 16 K columns stays L1/L2 resident over the three passes.
@@ -1149,6 +1337,39 @@ extern "C" int svdx_ema_multi(const void* jobs, const int32_t* block_prefix, int
   multi_ema_kernel<<<total_blocks, 256, 0, ST(stream)>>>(reinterpret_cast<const EmaJob*>(jobs), block_prefix, njobs, ema_state);
   SVDX_CHECK_LAUNCH("ema_multi");
   return SVDX_OK;
+}
+
+static int adamw8bit_launch(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
+                            const float* qmap2, float* state, float grad_scale, double* ema_state, bool ema, void* stream) {
+  if (!jobs || !block_prefix || !qmap1 || !qmap2 || !state || njobs <= 0 || total_blocks <= 0 || (reinterpret_cast<uintptr_t>(jobs) & 7) ||
+      (reinterpret_cast<uintptr_t>(block_prefix) & 3) || (reinterpret_cast<uintptr_t>(qmap1) & 3) ||
+      (reinterpret_cast<uintptr_t>(qmap2) & 3) || (reinterpret_cast<uintptr_t>(state) & 3) ||
+      (ema && (!ema_state || (reinterpret_cast<uintptr_t>(ema_state) & 7))))
+    return svdx_fail(SVDX_E_BADARG, ema ? "adamw8bit_ema: bad arguments (device job table, block prefix, maps, state[8], ema_state[9])"
+                                        : "adamw8bit: bad arguments (device job table, block prefix, maps, state[8])");
+  long long blocks = (total_blocks + A8_WARPS - 1) / A8_WARPS;
+  const long long cap = (long long)svdx_num_sms() * 8;      // grid-stride: the maps are staged in shared memory once per CTA
+  if (blocks > cap) blocks = cap;
+  const Adam8Job* j = reinterpret_cast<const Adam8Job*>(jobs);
+  if (ema) {
+    adamw_ema_tick_kernel<<<1, 1, 0, ST(stream)>>>(state, ema_state);
+    adamw8bit_kernel<true><<<(unsigned)blocks, 256, 0, ST(stream)>>>(j, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, ema_state);
+  } else {
+    adamw_tick_kernel<<<1, 1, 0, ST(stream)>>>(state);
+    adamw8bit_kernel<false><<<(unsigned)blocks, 256, 0, ST(stream)>>>(j, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, nullptr);
+  }
+  SVDX_CHECK_LAUNCH(ema ? "adamw8bit_ema" : "adamw8bit");
+  return SVDX_OK;
+}
+
+extern "C" int svdx_adamw8bit(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
+                              const float* qmap2, float* state, float grad_scale, void* stream) {
+  return adamw8bit_launch(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, nullptr, false, stream);
+}
+
+extern "C" int svdx_adamw8bit_ema(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
+                                  const float* qmap2, float* state, float grad_scale, double* ema_state, void* stream) {
+  return adamw8bit_launch(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, ema_state, true, stream);
 }
 
 static int adamw_p2p_launch(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo, int64_t n,

@@ -27,7 +27,8 @@ def dtype_code(t: torch.Tensor, what: str) -> int:
 # number of kernels launched through the C ABI since import (each wrapper adds what its entry point launches)
 LAUNCHES = [0]
 _KERNELS_PER_CALL = {"svdx_groupnorm_apply_fused": 1, "svdx_attention_bwd": 3, "svdx_adamw_graph": 2, "svdx_adamw_p2p": 2,
-                     "svdx_adamw_graph_ema": 2, "svdx_adamw_p2p_ema": 2, "svdx_ema_multi": 2}
+                     "svdx_adamw_graph_ema": 2, "svdx_adamw_p2p_ema": 2, "svdx_ema_multi": 2, "svdx_adamw8bit": 2,
+                     "svdx_adamw8bit_ema": 2}
 
 
 def check(rc: int, what: str = "") -> None:
@@ -759,6 +760,27 @@ def ema_multi(jobs, block_prefix, njobs, total_blocks, ema_state, nelem):
         return
     check(load().svdx_ema_multi(jobs.data_ptr(), block_prefix.data_ptr(), njobs, total_blocks, ema_state.data_ptr(), _stream()),
           "svdx_ema_multi")
+
+
+A8_BLOCK = 256       # elements per quantisation block of adamw8bit_kernel (one warp)
+
+
+def adamw8bit(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale=1.0, ema_state=None, nbytes=0.0):
+    """tick + block-wise 8-bit AdamW over many parameters in one launch (svdx_adamw8bit, svdx_adamw8bit_ema with `ema_state`).
+    jobs: device bytes of the job table (svd_xtend_b200.h); qmap1 / qmap2: device float[256]; state: device float[8];
+    nbytes (the HBM bytes the update moves) is for the byte accounting only."""
+    if qmap1.dtype != torch.float32 or qmap2.dtype != torch.float32 or qmap1.numel() != 256 or qmap2.numel() != 256:
+        raise ValueError("adamw8bit: qmap1 / qmap2 are float32[256]")
+    if _fam("adamw", 0.0, nbytes):
+        return
+    if ema_state is not None:
+        if ema_state.dtype != torch.float64 or ema_state.numel() < 9:
+            raise ValueError("adamw8bit: ema_state is float64[9] (svd_xtend_b200.h)")
+        check(load().svdx_adamw8bit_ema(jobs.data_ptr(), block_prefix.data_ptr(), njobs, total_blocks, qmap1.data_ptr(), qmap2.data_ptr(),
+                                        state.data_ptr(), float(grad_scale), ema_state.data_ptr(), _stream()), "svdx_adamw8bit_ema")
+        return
+    check(load().svdx_adamw8bit(jobs.data_ptr(), block_prefix.data_ptr(), njobs, total_blocks, qmap1.data_ptr(), qmap2.data_ptr(),
+                                state.data_ptr(), float(grad_scale), _stream()), "svdx_adamw8bit")
 
 
 def multi_transpose(src_base, jobs, tile_prefix, njobs, total_tiles):

@@ -6,7 +6,8 @@
 Before the script body runs, the replacement class is installed under the two names the reference
 imports the UNet from: `diffusers.UNetSpatioTemporalConditionModel` (train_svd.py:49) and
 `src.unet_spatio_temporal_condition.UNetSpatioTemporalConditionModel` (train_svd_lora.py:60), and the EMA as
-`diffusers.training_utils.EMAModel` (train_svd.py:52, used with --use_ema). Where transformers is
+`diffusers.training_utils.EMAModel` (train_svd.py:52, used with --use_ema), and, for a run with --use_8bit_adam, the 8-bit
+AdamW as `bitsandbytes.optim.AdamW8bit` (train_svd.py:746-773). Where transformers is
 importable, the image encoder is also installed as `transformers.CLIPVisionModelWithProjection` (train_svd.py:646-647).
 diffusers / accelerate are NOT part of this image (no network), so this shim is exercised only where a
 user's environment provides them; it fails loudly when they are missing.
@@ -14,12 +15,21 @@ user's environment provides them; it fails loudly when they are missing.
 from __future__ import annotations
 
 import importlib
+import importlib.machinery
 import runpy
 import sys
 import types
 
 
-def install() -> None:
+def wants_8bit_adam(argv) -> bool:
+    """the script's arguments ask for the 8-bit optimizer (`--use_8bit_adam`, a store_true flag, or a prefix argparse accepts
+    for it: no other flag of the scripts starts with `--use_8`)"""
+    return any(a.startswith("--use_8") and "--use_8bit_adam".startswith(a) for a in argv)
+
+
+def install(use_8bit_adam: bool | None = None) -> None:
+    """use_8bit_adam: also install the 8-bit AdamW (install_adam8bit); None reads `--use_8bit_adam` from sys.argv. Without
+    it bitsandbytes is left alone: no import of an installed one, no stand-in that other libraries' probes would find."""
     from .unet import UNetSpatioTemporalConditionModel
     try:
         diffusers = importlib.import_module("diffusers")
@@ -48,7 +58,38 @@ def install() -> None:
         tu.EMAModel = EMAModel
     except ModuleNotFoundError:
         pass
+    if wants_8bit_adam(sys.argv[1:]) if use_8bit_adam is None else use_8bit_adam:
+        install_adam8bit()
     install_clip()
+
+
+def install_adam8bit():
+    """install the block-wise 8-bit AdamW on this package's kernels as `bitsandbytes.optim.AdamW8bit` (train_svd.py:746-773 and
+    train_svd_lora.py:732-740 build it for --use_8bit_adam). Where bitsandbytes is importable its module is patched: its own
+    update writes the parameters from a kernel that may leave their version counters alone, and the model would then run
+    on stale operands. Otherwise a minimal stand-in `bitsandbytes` package (marked `__svdx_standin__ = True`) is registered
+    in sys.modules, so the scripts' `import bitsandbytes as bnb` succeeds. The stand-in carries a real module spec, so
+    `importlib.util.find_spec("bitsandbytes")` keeps working, and the version "0.0.0+svdx.standin", so libraries that gate
+    their bitsandbytes integrations on a minimum version (transformers' `is_bitsandbytes_available`) keep them off: it
+    provides the optimizer only. Returns the module."""
+    from .optim8bit import AdamW8bit
+    try:
+        bnb = importlib.import_module("bitsandbytes")
+        optim = importlib.import_module("bitsandbytes.optim")
+    except ModuleNotFoundError:
+        bnb = types.ModuleType("bitsandbytes")
+        bnb.__spec__ = importlib.machinery.ModuleSpec("bitsandbytes", None, is_package=True)
+        bnb.__path__ = []
+        bnb.__version__ = "0.0.0+svdx.standin"
+        bnb.__svdx_standin__ = True
+        optim = types.ModuleType("bitsandbytes.optim")
+        optim.__spec__ = importlib.machinery.ModuleSpec("bitsandbytes.optim", None, is_package=True)
+        optim.__path__ = []
+        bnb.optim = optim
+        sys.modules["bitsandbytes"] = bnb
+        sys.modules["bitsandbytes.optim"] = optim
+    optim.AdamW8bit = AdamW8bit
+    return bnb
 
 
 def install_clip() -> bool:
@@ -72,7 +113,7 @@ def main(argv=None) -> None:
     argv = list(sys.argv[1:] if argv is None else argv)
     if not argv:
         raise SystemExit("usage: python -m svd_xtend_b200.shim <train_svd.py|train_svd_lora.py> [args...]")
-    install()
+    install(use_8bit_adam=wants_8bit_adam(argv[1:]))
     script = argv[0]
     sys.argv = argv
     runpy.run_path(script, run_name="__main__")

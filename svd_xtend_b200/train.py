@@ -233,6 +233,167 @@ class FusedAdamW:
         return ts + self._ema_tensors()
 
 
+class FusedAdamW8bit:
+    """FusedAdamW with block-wise 8-bit moments (bitsandbytes' AdamW8bit, train_svd.py --use_8bit_adam; the update is stated in
+    oracle/svd_adam8bit_oracle.py): a parameter with at least `min_8bit_size` elements keeps m / v as uint8 codes plus one fp32
+    absmax per 256-element block counted from its own arena offset (arena padding belongs to no block); a smaller one keeps
+    fp32 m / v. ONE tick + ONE launch over every parameter (`svdx_adamw8bit`), with the same device `state` float[8] as
+    FusedAdamW, so a captured GraphedStep replays the right sequence. About 2.03 bytes of state per parameter instead of 8.
+    The update is deterministic, so under GradReducer every rank's replica stays identical."""
+
+    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, min_8bit_size: int = 4096):
+        from .optim8bit import dynamic_map, num_blocks
+        self.arena = arena
+        self.betas, self.weight_decay, self.eps, self.min_8bit_size = betas, weight_decay, eps, int(min_8bit_size)
+        dev = arena.data.device
+        self.qmap1, self.qmap2 = dynamic_map(True).to(dev), dynamic_map(False).to(dev)
+        # per parameter: (param, arena offset, quant, state offset (codes / fp32 elements), absmax offset)
+        self.layout: List[tuple] = []
+        codes, blocks, f32 = 0, 0, 0
+        for p in arena.params:
+            n = p.numel()
+            if n >= self.min_8bit_size:
+                self.layout.append((p, arena.offset_of[p], True, codes, blocks))
+                codes += num_blocks(n) * 256
+                blocks += num_blocks(n)
+            else:
+                self.layout.append((p, arena.offset_of[p], False, f32, 0))
+                f32 += (n + 63) // 64 * 64
+        self.codes1 = torch.zeros(codes, dtype=torch.uint8, device=dev)
+        self.codes2 = torch.zeros(codes, dtype=torch.uint8, device=dev)
+        self.absmax1 = torch.zeros(blocks, dtype=F32, device=dev)
+        self.absmax2 = torch.zeros(blocks, dtype=F32, device=dev)
+        self.m32 = torch.zeros(f32, dtype=F32, device=dev)
+        self.v32 = torch.zeros(f32, dtype=F32, device=dev)
+        self._lr = float(lr)
+        self.state = torch.tensor([float(lr), betas[0], betas[1], eps, weight_decay, 0.0, 1.0, 1.0], device=dev, dtype=F32)
+        self._lr_host = torch.empty(1, dtype=F32).pin_memory() if arena.data.is_cuda else torch.empty(1, dtype=F32)
+        self.on_updated = None
+        self.param_groups = [{"lr": float(lr), "params": arena.params}]
+        self.ema = None
+        self._table = None
+        self._index = {p: i for i, (p, *_r) in enumerate(self.layout)}
+
+    lr = FusedAdamW.lr
+    sync_lr = FusedAdamW.sync_lr
+    t = FusedAdamW.t
+    _ema_tensors = FusedAdamW._ema_tensors
+
+    def attach_ema(self, ema):
+        """FusedAdamW.attach_ema for the 8-bit update: the EMA of the new masters is advanced in the same launch"""
+        ema._attach(self, sharded=False)
+        self.ema = ema
+        self._table = None
+
+    def state_views(self, p: torch.nn.Parameter) -> Dict[str, torch.Tensor]:
+        """this parameter's optimizer state as views into the flat buffers (bitsandbytes' keys, without step)"""
+        _, _, quant, so, bo = self.layout[self._index[p]]
+        n = p.numel()
+        if quant:
+            nb = (n + 255) // 256
+            return {"state1": self.codes1[so:so + n].view(p.shape), "state2": self.codes2[so:so + n].view(p.shape),
+                    "qmap1": self.qmap1, "qmap2": self.qmap2, "absmax1": self.absmax1[bo:bo + nb], "absmax2": self.absmax2[bo:bo + nb]}
+        return {"state1": self.m32[so:so + n].view(p.shape), "state2": self.v32[so:so + n].view(p.shape)}
+
+    def job_rows(self):
+        """the launch's job table as an int64 array [params, 10] (svd_xtend_b200.h, svdx_adamw8bit)"""
+        import numpy as np
+        from .optim8bit import job_row
+        a = self.arena
+        pb, gb = a.data.data_ptr(), a.grad.data_ptr()
+        sb = a.shadow.data_ptr() if a.shadow is not None else 0
+        eb = self.ema._flat.data_ptr() if self.ema is not None else 0
+        rows = []
+        for p, off, quant, so, bo in self.layout:
+            if quant:
+                s1, s2 = self.codes1.data_ptr() + so, self.codes2.data_ptr() + so
+                a1, a2 = self.absmax1.data_ptr() + 4 * bo, self.absmax2.data_ptr() + 4 * bo
+            else:
+                s1, s2, a1, a2 = self.m32.data_ptr() + 4 * so, self.v32.data_ptr() + 4 * so, 0, 0
+            rows.append(job_row(pb + 4 * off, gb + 4 * off, s1, s2, a1, a2, sb + 2 * off if sb else 0, eb + 4 * off if eb else 0,
+                                p.numel(), quant))
+        return np.array(rows, dtype=np.int64).reshape(-1, 10)
+
+    def step(self, grad_scale: float = 1.0):
+        from .optim8bit import JobTable, update_bytes
+        if self._table is None:
+            self._table = JobTable(self.arena.data.device)
+            self._table.set(self.job_rows())
+            n8 = sum(p.numel() for p, _, q, _, _ in self.layout if q)
+            self._nbytes = update_bytes(n8, sum(p.numel() for p in self.arena.params) - n8, self.arena.shadow is not None, self.ema is not None)
+        tb = self._table
+        raw.adamw8bit(tb.dev, tb.prefix, tb.njobs, tb.blocks, self.qmap1, self.qmap2, self.state, grad_scale,
+                      ema_state=None if self.ema is None else self.ema._state, nbytes=self._nbytes)
+        if self.on_updated is not None:
+            self.on_updated()
+
+    def zero_grad(self, set_to_none: bool = False):
+        self.arena.zero_grad()
+
+    def snapshot_tensors(self) -> List[torch.Tensor]:
+        ts = [self.arena.data, self.codes1, self.codes2, self.absmax1, self.absmax2, self.m32, self.v32, self.state]
+        if self.arena.shadow is not None:
+            ts.append(self.arena.shadow)
+        return ts + self._ema_tensors()
+
+    # ---- checkpoints in bitsandbytes' per-parameter layout (svd_xtend_b200.optim8bit.AdamW8bit loads them too) ----
+    def state_dict(self) -> dict:
+        step = int(self.state[5].item())
+        st = {}
+        for i, (p, *_r) in enumerate(self.layout):
+            d = {k: (v if k.startswith("qmap") else v.clone()) for k, v in self.state_views(p).items()}
+            d["step"] = step
+            st[i] = d
+        group = {"lr": self._lr, "betas": tuple(self.betas), "eps": self.eps, "weight_decay": self.weight_decay, "amsgrad": False,
+                 "optim_bits": 8, "min_8bit_size": self.min_8bit_size, "percentile_clipping": 100, "block_wise": True,
+                 "is_paged": False, "params": list(range(len(self.layout)))}
+        return {"state": st, "param_groups": [group]}
+
+    @torch.no_grad()
+    def load_state_dict(self, sd: dict) -> None:
+        groups = sd["param_groups"]
+        if len(groups) != 1 or len(groups[0]["params"]) != len(self.layout):
+            raise ValueError("FusedAdamW8bit.load_state_dict: one group over the arena's parameters expected")
+        g = groups[0]
+        if int(g.get("min_8bit_size", self.min_8bit_size)) != self.min_8bit_size:
+            raise ValueError("FusedAdamW8bit.load_state_dict: saved with a different min_8bit_size")
+        from .optim8bit import check_param_state
+        steps = set()
+        maps_done = False
+        missing = [i for i in g["params"] if i not in sd["state"]]
+        if missing:
+            raise ValueError(f"FusedAdamW8bit.load_state_dict: no state for parameters {missing[:8]} (they never had a gradient in "
+                             "the saved run); the fused form keeps one step count for all parameters and needs every one")
+        for (p, *_r), i in zip(self.layout, g["params"]):
+            src = {k: (v.contiguous() if isinstance(v, torch.Tensor) else v) for k, v in sd["state"][i].items()}
+            check_param_state(src, p, self.min_8bit_size, f"FusedAdamW8bit.load_state_dict: parameter {i}")
+            dst = self.state_views(p)
+            for k in ("state1", "state2", "absmax1", "absmax2"):
+                if (k in dst) != (k in src):
+                    raise ValueError(f"FusedAdamW8bit.load_state_dict: parameter {i} has a different state form")
+                if k in dst:
+                    if src[k].shape != dst[k].shape or src[k].dtype != dst[k].dtype:
+                        raise ValueError(f"FusedAdamW8bit.load_state_dict: {k} of parameter {i} has shape {tuple(src[k].shape)} "
+                                         f"{src[k].dtype}, expected {tuple(dst[k].shape)} {dst[k].dtype}")
+                    dst[k].copy_(src[k])
+            if "qmap1" in src:
+                if not maps_done:
+                    self.qmap1.copy_(src["qmap1"])
+                    self.qmap2.copy_(src["qmap2"])
+                    maps_done = True
+                elif not (torch.equal(src["qmap1"].to(self.qmap1.device), self.qmap1) and torch.equal(src["qmap2"].to(self.qmap2.device), self.qmap2)):
+                    raise ValueError("FusedAdamW8bit.load_state_dict: parameters carry different quantisation maps")
+            steps.add(int(src.get("step", 0)))
+        if len(steps) > 1:
+            raise ValueError("FusedAdamW8bit.load_state_dict: parameters at different step counts (one device counter here)")
+        b1, b2 = g.get("betas", self.betas)
+        self.betas, self.eps, self.weight_decay = (b1, b2), g.get("eps", self.eps), g.get("weight_decay", self.weight_decay)
+        step = steps.pop() if steps else 0
+        self.state.copy_(torch.tensor([float(g.get("lr", self._lr)), b1, b2, self.eps, self.weight_decay, float(step), 1.0, 1.0], dtype=F32))
+        self._lr = float(g.get("lr", self._lr))
+        self.param_groups[0]["lr"] = self._lr
+
+
 class ShardedAdamW:
     """Data-parallel update with the optimizer state SHARDED over the ranks (ZeRO-1 on the flat arenas), all in NCCL
     collectives that capture into the step's CUDA graph:
