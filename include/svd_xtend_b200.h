@@ -70,7 +70,8 @@ typedef struct SvdxTapGemm {
   const void* a;
   int64_t lda;          /* elements between consecutive rows/pixels */
   int32_t a_mode;       /* SVDX_A_ROWS / SVDX_A_CONV2D */
-  int32_t a_major_mn;   /* 0: A[m][k] k contiguous. 1 (ROWS, groups==1 only): memory is [k][m], m contiguous */
+  int32_t a_major_mn;   /* 0: A[m][k] k contiguous. 1 (ROWS, groups==1 only): memory is [k][m], m contiguous; runs the
+                           generic epilogue, so no gn_sum / gnb sums / act / interleave / block_n 320 */
   int32_t rows_per_group, groups;      /* ROWS   */
   int32_t W, H, nimg;                  /* CONV2D (and b_mode 1): any W > 0; see SVDX_A_CONV2D for how each width is tiled */
   int32_t num_taps;
@@ -80,7 +81,8 @@ typedef struct SvdxTapGemm {
   /* B operand (bf16): [N][num_taps*K] (k contiguous), or if b_major_mn: memory [K][N], n contiguous */
   const void* b;
   int64_t ldb;
-  int32_t b_major_mn;
+  int32_t b_major_mn;   /* 1: with a bf16 output, bias / rowbias only (with res1 / res2 / scales it runs the generic epilogue);
+                           no gn_sum / gnb sums / act / interleave / GEGLU */
   int32_t b_mode;       /* weight-gradient forms (a_major_mn = b_major_mn = 1): 0 plain [K][N];
                            1: B is a channels-last image tensor [nimg][H][W][N], contraction row p (an output
                               pixel) reads pixel shifted by (tap_d0[0], tap_d1[0]) of image +tap_d2[0], zero outside

@@ -5,9 +5,10 @@
 // One persistent, warp-specialised kernel:
 //   warp 8      : TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
 //   warps 0..7  : two consumer warpgroups; warpgroup g multiplies rows [64g, 64g + 64) of the 128-row tile with wgmma,
-//                 then both park the fp32 tile in shared memory and run the epilogue on it (bias / rowbias / GEGLU /
-//                 residual / blend, staged TMA stores). The producer keeps filling the ring meanwhile, so the next
-//                 tile's operands are resident when the epilogue ends.
+//                 then runs the epilogue (bias / rowbias / GEGLU / residual / blend, staged TMA stores) straight from
+//                 the accumulator registers (bf16 outputs, 5-stage ring) or, in EPI_GENERIC, from the fp32 tile parked
+//                 in shared memory (3-stage ring). The producer keeps filling the ring meanwhile, so the next tile's
+//                 operands are resident when the epilogue ends.
 //
 // A-operand modes (see include/svd_xtend_b200.h): plain/grouped rows with row-shifted taps
 // (linear, (3,1,1) temporal conv [D: TemporalResnetBlock]) and channels-last images with 2-D
@@ -18,11 +19,14 @@
 namespace svdx {
 
 // Main loop of one tile for one consumer warpgroup: rows [64 wg, 64 wg + 64) x BN columns, k-blocks [kb0, kb1) of the
-// ring, then the accumulator is written to the shared tile sAcc (row-major, ACC_LD floats per row).
-template <int BN, int TA, int TB>
-__device__ __forceinline__ void tile_mainloop(int kb0, int kb1, uint32_t sA, uint32_t sB, uint32_t bar_full, uint32_t bar_empty,
-                                           uint32_t sAcc, int wg, int& stage, uint32_t& phase) {
-  float acc[BN / 2];
+// STG-stage ring, into the wgmma accumulator fragments acc.
+struct Ring {
+  uint32_t sA, sB, bar_full, bar_empty;
+  int stage;
+  uint32_t phase;
+};
+template <int BN, int TA, int TB, int STG>
+__device__ __forceinline__ void tile_mainloop(float (&acc)[BN / 2], int kb0, int kb1, Ring& rg, int wg) {
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
   const int lane = threadIdx.x & 31;
@@ -30,9 +34,9 @@ __device__ __forceinline__ void tile_mainloop(int kb0, int kb1, uint32_t sA, uin
   const uint32_t astep = TA ? (2048 >> 4) : (32 >> 4), bstep = TB ? (2048 >> 4) : (32 >> 4);
   int prev_stage = -1;
   for (int kb = kb0; kb < kb1; ++kb) {
-    mbar_wait_mma(bar_full + 8 * stage, phase);
-    const uint32_t aaddr = sA + stage * A_STAGE_BYTES + wg * 8192;   // 64 rows: 8 KB in either major
-    const uint32_t baddr = sB + stage * B_STAGE_BYTES;
+    mbar_wait_mma(rg.bar_full + 8 * rg.stage, rg.phase);
+    const uint32_t aaddr = rg.sA + rg.stage * A_STAGE_BYTES + wg * 8192;   // 64 rows: 8 KB in either major
+    const uint32_t baddr = rg.sB + rg.stage * B_STAGE_BYTES;
     const uint64_t ad0 = make_smem_desc_sw128(aaddr, 8192, 1024);
     const uint64_t bd0 = make_smem_desc_sw128(baddr, 8192, 1024);
     wgmma_fence();
@@ -51,17 +55,24 @@ __device__ __forceinline__ void tile_mainloop(int kb0, int kb1, uint32_t sA, uin
     reg_fence(acc);
     if (prev_stage >= 0) {
       __syncwarp();
-      if (lane == 0) mbar_arrive(bar_empty + 8 * prev_stage);
+      if (lane == 0) mbar_arrive(rg.bar_empty + 8 * prev_stage);
     }
-    prev_stage = stage;
-    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    prev_stage = rg.stage;
+    if (++rg.stage == STG) { rg.stage = 0; rg.phase ^= 1; }
   }
   wgmma_wait<0>();
   reg_fence(acc);
   __syncwarp();
-  if (lane == 0 && prev_stage >= 0) mbar_arrive(bar_empty + 8 * prev_stage);
+  if (lane == 0 && prev_stage >= 0) mbar_arrive(rg.bar_empty + 8 * prev_stage);
+}
 
-  // D fragment -> shared tile: register 4j + 2h + e is row 16 * warp + lane / 4 + 8h, column 8j + 2 * (lane % 4) + e
+// EPI_GENERIC: main loop, then the fragments -> the shared tile sAcc (row-major, ACC_LD floats per row)
+template <int BN, int TA, int TB>
+SVDX_DEVINL void tile_parked_bn(int kb0, int kb1, Ring& rg, uint32_t sAcc, int wg) {
+  float acc[BN / 2];
+  tile_mainloop<BN, TA, TB, STAGES_PARKED>(acc, kb0, kb1, rg, wg);
+  // register 4j + 2h + e is row 16 * warp + lane / 4 + 8h, column 8j + 2 * (lane % 4) + e
+  const int lane = threadIdx.x & 31;
   const int r0 = wg * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
   const uint32_t base = sAcc + (uint32_t)(r0 * ACC_LD + 2 * (lane & 3)) * 4u;
 #pragma unroll
@@ -74,25 +85,61 @@ __device__ __forceinline__ void tile_mainloop(int kb0, int kb1, uint32_t sA, uin
 }
 
 template <int TA, int TB>
-SVDX_DEVINL void tile_mainloop_bn(int bn, int kb0, int kb1, uint32_t sA, uint32_t sB, uint32_t bar_full, uint32_t bar_empty, uint32_t sAcc,
-                                  int wg, int& stage, uint32_t& phase) {
+SVDX_DEVINL void tile_parked(int bn, int kb0, int kb1, Ring& rg, uint32_t sAcc, int wg) {
   switch (bn) {
-    case 32: tile_mainloop<32, TA, TB>(kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase); break;
-    case 64: tile_mainloop<64, TA, TB>(kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase); break;
-    case 96: tile_mainloop<96, TA, TB>(kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase); break;
-    case 128: tile_mainloop<128, TA, TB>(kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase); break;
-    default: tile_mainloop<160, TA, TB>(kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase); break;
+    case 32: tile_parked_bn<32, TA, TB>(kb0, kb1, rg, sAcc, wg); break;
+    case 64: tile_parked_bn<64, TA, TB>(kb0, kb1, rg, sAcc, wg); break;
+    case 96: tile_parked_bn<96, TA, TB>(kb0, kb1, rg, sAcc, wg); break;
+    case 128: tile_parked_bn<128, TA, TB>(kb0, kb1, rg, sAcc, wg); break;
+    default: tile_parked_bn<160, TA, TB>(kb0, kb1, rg, sAcc, wg); break;
+  }
+}
+
+// register epilogues: main loop, then the epilogue straight from the fragments. A is K-major (the host sends MN-major A
+// to EPI_GENERIC); MN-major B comes with 64 / 128-wide tiles only, and only to EPI_FAST; GEGLU tiles are 64 / 128 wide.
+template <int EPI, int BN, int TB>
+SVDX_DEVINL void tile_regs_bn(const TapGemmKParams& p, int kb0, int kb1, Ring& rg, int wg, PairStage& ps, const EpiTile& t, int lane,
+                              float s_acc, float s_r1, float s_r2) {
+  float acc[BN / 2];
+  tile_mainloop<BN, 0, TB, STAGES_REGS>(acc, kb0, kb1, rg, wg);
+  epilogue_regs<EPI, BN>(p, acc, ps, t, lane, s_acc, s_r1, s_r2);
+}
+
+template <int EPI>
+SVDX_DEVINL void tile_regs(const TapGemmKParams& p, int kb0, int kb1, Ring& rg, int wg, PairStage& ps, const EpiTile& t, int lane,
+                           float s_acc, float s_r1, float s_r2) {
+  if constexpr (EPI == EPI_GEGLU) {
+    if (p.block_n == 64) tile_regs_bn<EPI, 64, 0>(p, kb0, kb1, rg, wg, ps, t, lane, s_acc, s_r1, s_r2);
+    else tile_regs_bn<EPI, 128, 0>(p, kb0, kb1, rg, wg, ps, t, lane, s_acc, s_r1, s_r2);
+  } else {
+    if constexpr (EPI == EPI_FAST) {
+      // MN-major B (the VAE attention's P·V) reaches only the plain epilogue: the host sends it nowhere else
+      if (p.b_mn) {
+        if (p.block_n == 64) tile_regs_bn<EPI, 64, 1>(p, kb0, kb1, rg, wg, ps, t, lane, s_acc, s_r1, s_r2);
+        else tile_regs_bn<EPI, 128, 1>(p, kb0, kb1, rg, wg, ps, t, lane, s_acc, s_r1, s_r2);
+        return;
+      }
+    }
+    switch (p.block_n) {
+      case 32: tile_regs_bn<EPI, 32, 0>(p, kb0, kb1, rg, wg, ps, t, lane, s_acc, s_r1, s_r2); break;
+      case 64: tile_regs_bn<EPI, 64, 0>(p, kb0, kb1, rg, wg, ps, t, lane, s_acc, s_r1, s_r2); break;
+      case 96: tile_regs_bn<EPI, 96, 0>(p, kb0, kb1, rg, wg, ps, t, lane, s_acc, s_r1, s_r2); break;
+      case 128: tile_regs_bn<EPI, 128, 0>(p, kb0, kb1, rg, wg, ps, t, lane, s_acc, s_r1, s_r2); break;
+      default: tile_regs_bn<EPI, 160, 0>(p, kb0, kb1, rg, wg, ps, t, lane, s_acc, s_r1, s_r2); break;
+    }
   }
 }
 
 template <int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_constant__ TapGemmKParams p) {
+  constexpr bool PARKED = EPI == EPI_GENERIC;
+  constexpr int STAGES = PARKED ? STAGES_PARKED : STAGES_REGS;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sA = smem_base;
   const uint32_t sB = smem_base + STAGES * A_STAGE_BYTES;
-  const uint32_t sAcc = sB + STAGES * B_STAGE_BYTES;     // the finished fp32 tile, read by the epilogue
-  const uint32_t sEpi = sAcc + ACC_BYTES;                // epilogue staging (TMA stores), 4 KB per epilogue warp
+  const uint32_t sAcc = sB + STAGES * B_STAGE_BYTES;     // EPI_GENERIC: the finished fp32 tile, read by the epilogue
+  const uint32_t sEpi = sAcc + (PARKED ? ACC_BYTES : 0); // epilogue staging (TMA stores), 4 KB per epilogue warp
   const uint32_t sBar = sEpi + NUM_EPI_WARPS * EPI_STAGE_BYTES;
   // barrier layout (8 B each): full[STAGES], empty[STAGES]
   const uint32_t bar_full = sBar;
@@ -322,10 +369,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
   } else {
     // =========================== consumer warpgroups: main loop + epilogue ===========================
     const int wg = warp >> 2;
-    const int q = warp & 3;            // 32-row quarter of the tile this warp's epilogue writes
-    const int half = warp >> 2;        // which of the two warps of the quarter: takes chunks half, half+2, ...
-    int stage = 0;
-    uint32_t phase = 0;
+    // parked: warp takes 32-row quarter warp % 4 and the chunks half, half + 2, ... of it; registers: the pair of warps
+    // 2q, 2q + 1 holds quarter q (16 rows each) and stages every chunk of it
+    const int q = PARKED ? (warp & 3) : (warp >> 1);
+    const int half = PARKED ? (warp >> 2) : (warp & 1);
+    Ring rg{sA, sB, bar_full, bar_empty, 0, 0u};
     float s_acc = 1.f, s_r1 = 1.f, s_r2 = 1.f;
     if (p.scales) { s_acc = p.scales[0]; s_r1 = p.scales[1]; s_r2 = p.scales[2]; }
     const int n_out_total = p.geglu ? p.N / 2 : p.N;
@@ -333,6 +381,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
     EpiStage st;
     st.base = sEpi + warp * EPI_STAGE_BYTES;
     st.off = 0;
+    PairStage ps{sEpi + q * 2 * EPI_STAGE_BYTES, 2 + q, half, 0u};
     const uint32_t t_base = sAcc + (uint32_t)((q * 32 + lane) * ACC_LD) * 4u;   // this thread's accumulator row
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int nt = tile % p.n_tiles;
@@ -363,20 +412,22 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
       }
       if constexpr (EPI == EPI_RES || EPI == EPI_RES_GN || EPI == EPI_FAST_GNB)
         prefetch_epilogue_operands(p, EPI, m0, valid_rows, n0, bn_out, n_out_total, lane, half);
-      // every warp has finished reading the previous tile's accumulator before it is overwritten
-      named_bar_sync(1, 32 * NUM_EPI_WARPS);
-      if (p.a_mn && p.b_mn) tile_mainloop_bn<1, 1>(p.block_n, kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase);
-      else if (p.a_mn) tile_mainloop_bn<1, 0>(p.block_n, kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase);
-      else if (p.b_mn) tile_mainloop_bn<0, 1>(p.block_n, kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase);
-      else tile_mainloop_bn<0, 0>(p.block_n, kb0, kb1, sA, sB, bar_full, bar_empty, sAcc, wg, stage, phase);
-      named_bar_sync(1, 32 * NUM_EPI_WARPS);
-      if constexpr (EPI == EPI_FAST || EPI == EPI_FAST_GN) epilogue_fast<EPI == EPI_FAST_GN>(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, st.base, st.row0, st.grp, lane, m0, valid_rows);
-      else if constexpr (EPI == EPI_FAST_IL || EPI == EPI_FAST_IL_GN) epilogue_fast<EPI == EPI_FAST_IL_GN, true>(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, st.base, st.row0, st.grp, lane, m0, valid_rows);
-      else if constexpr (EPI == EPI_FAST_ACT) epilogue_fast<false, false, true>(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, st.base, st.row0, st.grp, lane, m0, valid_rows);
-      else if constexpr (EPI == EPI_RES || EPI == EPI_RES_GN) epilogue_res<EPI == EPI_RES_GN>(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, s_acc, s_r1, s_r2, st.base, st.off, st.row0, st.grp, lane, m0, valid_rows);
-      else if constexpr (EPI == EPI_GEGLU) epilogue_geglu(p, t_base, n0, half, bn_out, st.base, st.row0, st.grp, lane);
-      else if constexpr (EPI == EPI_FAST_GNB) epilogue_fast_gnb(p, t_base, m, row_ok, n0, half, 0, bn_out, n_out_total, st.base, st.row0, st.grp, lane, m0, valid_rows);
-      else epilogue_tile(p, t_base, m, row_ok, n0, half, bn_out, n_out_total, s_acc, s_r1, s_r2, st, lane);
+      if constexpr (PARKED) {
+        // every warp has finished reading the previous tile's accumulator before it is overwritten
+        named_bar_sync(1, 32 * NUM_EPI_WARPS);
+        if (p.a_mn && p.b_mn) tile_parked<1, 1>(p.block_n, kb0, kb1, rg, sAcc, wg);
+        else if (p.a_mn) tile_parked<1, 0>(p.block_n, kb0, kb1, rg, sAcc, wg);
+        else if (p.b_mn) tile_parked<0, 1>(p.block_n, kb0, kb1, rg, sAcc, wg);
+        else tile_parked<0, 0>(p.block_n, kb0, kb1, rg, sAcc, wg);
+        named_bar_sync(1, 32 * NUM_EPI_WARPS);
+        epilogue_tile(p, t_base, m, row_ok, n0, half, bn_out, n_out_total, s_acc, s_r1, s_r2, st, lane);
+      } else {
+        EpiTile et;
+        et.n0 = n0; et.n_out_total = n_out_total; et.row0 = st.row0; et.grp = st.grp; et.valid_rows = valid_rows; et.m0 = m0;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) tile_row(p, mt, q * 32 + half * 16 + (lane >> 2) + 8 * h, et.m[h], et.ok[h]);
+        tile_regs<EPI>(p, kb0, kb1, rg, wg, ps, et, lane, s_acc, s_r1, s_r2);
+      }
     }
     if (lane == 0) bulk_wait<0>();   // staged stores must have left shared memory (and landed) before the CTA exits
   }
@@ -582,8 +633,10 @@ int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p) {
     p.epi_mode = EPI_GENERIC;
     const bool vec_ok = (reinterpret_cast<uintptr_t>(d->bias) & 15) == 0
                         && (!d->rowbias || ((reinterpret_cast<uintptr_t>(d->rowbias) & 15) == 0 && d->ldrb % 4 == 0));
-    if (p.tma_store && !f32 && n_out % 32 == 0 && vec_ok && !p.probe && use != 2)
-      p.epi_mode = d->geglu ? EPI_GEGLU : (d->res1 || d->res2 || d->scales) ? EPI_RES : EPI_FAST;
+    // the register epilogues are built for K-major A, and for MN-major B only in the plain form
+    const bool has_res = d->res1 || d->res2 || d->scales;
+    if (p.tma_store && !f32 && n_out % 32 == 0 && vec_ok && !d->a_major_mn && !(d->b_major_mn && has_res) && !p.probe && use != 2)
+      p.epi_mode = d->geglu ? EPI_GEGLU : has_res ? EPI_RES : EPI_FAST;
   }
   if (p.split_k > 1 && (p.bias || p.rowbias || p.res1 || p.res2 || p.geglu)) return svdx_fail(SVDX_E_BADARG, "tapgemm: split_k with epilogue operands");
   if (p.gnb_sum) {
@@ -628,6 +681,8 @@ int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p) {
     p.act = d->act;
     p.epi_mode = EPI_FAST_ACT;
   }
+  if (d->b_major_mn && p.epi_mode != EPI_GENERIC && (p.epi_mode != EPI_FAST || p.gn_sum))
+    return svdx_fail(SVDX_E_BADARG, "tapgemm: MN-major B takes the plain epilogue only (no gn_sum / gnb sums / act)");
   if (wide320 && p.epi_mode != EPI_FAST && p.epi_mode != EPI_RES && p.epi_mode != EPI_FAST_GNB && p.epi_mode != EPI_FAST_IL && p.epi_mode != EPI_FAST_ACT)
     return svdx_fail(SVDX_E_BADARG, "tapgemm: block_n 320 needs a bf16 output through the TMA-store epilogues (N % 320 == 0, aligned rows)");
   if (p.gn_sum) {
@@ -646,6 +701,18 @@ int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p) {
   return SVDX_OK;
 }
 
+// shared memory of an instantiation: EPI_GENERIC keeps the parked tile and 3 stages, the register epilogues 5 stages
+static constexpr int kernel_smem(int epi) { return epi == EPI_GENERIC ? smem_bytes(STAGES_PARKED, true) : smem_bytes(STAGES_REGS, false); }
+
+template <int EPI>
+static cudaError_t set_smem() {
+  return cudaFuncSetAttribute(tapgemm_kernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, kernel_smem(EPI));
+}
+template <int EPI>
+static void launch(int grid, cudaStream_t stream, const TapGemmKParams& p) {
+  tapgemm_kernel<EPI><<<grid, NUM_THREADS, kernel_smem(EPI), stream>>>(p);
+}
+
 extern "C" int svdx_tapgemm(const SvdxTapGemm* d, void* stream_v) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
   TapGemmKParams p;
@@ -654,32 +721,32 @@ extern "C" int svdx_tapgemm(const SvdxTapGemm* d, void* stream_v) {
   static bool attr_done[SVDX_MAX_DEVICES] = {false};
   const int slot = svdx_device_slot();
   if (!attr_done[slot]) {
-    cudaError_t e = cudaFuncSetAttribute(tapgemm_kernel<EPI_GENERIC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_FAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_GEGLU>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_FAST_GN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_RES_GN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_FAST_GNB>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_FAST_IL>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_FAST_IL_GN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tapgemm_kernel<EPI_FAST_ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    cudaError_t e = set_smem<EPI_GENERIC>();
+    if (e == cudaSuccess) e = set_smem<EPI_FAST>();
+    if (e == cudaSuccess) e = set_smem<EPI_GEGLU>();
+    if (e == cudaSuccess) e = set_smem<EPI_RES>();
+    if (e == cudaSuccess) e = set_smem<EPI_FAST_GN>();
+    if (e == cudaSuccess) e = set_smem<EPI_RES_GN>();
+    if (e == cudaSuccess) e = set_smem<EPI_FAST_GNB>();
+    if (e == cudaSuccess) e = set_smem<EPI_FAST_IL>();
+    if (e == cudaSuccess) e = set_smem<EPI_FAST_IL_GN>();
+    if (e == cudaSuccess) e = set_smem<EPI_FAST_ACT>();
     if (e != cudaSuccess) return svdx_fail_cuda(e, "tapgemm: set smem attribute");
     attr_done[slot] = true;
   }
   const int total_tiles = p.m_tiles * p.n_tiles * p.split_k;
   int grid = svdx_num_sms();
   if (grid > total_tiles) grid = total_tiles;
-  if (p.epi_mode == EPI_FAST_ACT) tapgemm_kernel<EPI_FAST_ACT><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
-  else if (p.epi_mode == EPI_FAST_IL && p.gn_sum) tapgemm_kernel<EPI_FAST_IL_GN><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
-  else if (p.epi_mode == EPI_FAST_IL) tapgemm_kernel<EPI_FAST_IL><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
-  else if (p.epi_mode == EPI_FAST_GNB) tapgemm_kernel<EPI_FAST_GNB><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
-  else if (p.epi_mode == EPI_FAST && p.gn_sum) tapgemm_kernel<EPI_FAST_GN><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
-  else if (p.epi_mode == EPI_RES && p.gn_sum) tapgemm_kernel<EPI_RES_GN><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
-  else if (p.epi_mode == EPI_FAST) tapgemm_kernel<EPI_FAST><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
-  else if (p.epi_mode == EPI_GEGLU) tapgemm_kernel<EPI_GEGLU><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
-  else if (p.epi_mode == EPI_RES) tapgemm_kernel<EPI_RES><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
-  else tapgemm_kernel<EPI_GENERIC><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(p);
+  if (p.epi_mode == EPI_FAST_ACT) launch<EPI_FAST_ACT>(grid, stream, p);
+  else if (p.epi_mode == EPI_FAST_IL && p.gn_sum) launch<EPI_FAST_IL_GN>(grid, stream, p);
+  else if (p.epi_mode == EPI_FAST_IL) launch<EPI_FAST_IL>(grid, stream, p);
+  else if (p.epi_mode == EPI_FAST_GNB) launch<EPI_FAST_GNB>(grid, stream, p);
+  else if (p.epi_mode == EPI_FAST && p.gn_sum) launch<EPI_FAST_GN>(grid, stream, p);
+  else if (p.epi_mode == EPI_RES && p.gn_sum) launch<EPI_RES_GN>(grid, stream, p);
+  else if (p.epi_mode == EPI_FAST) launch<EPI_FAST>(grid, stream, p);
+  else if (p.epi_mode == EPI_GEGLU) launch<EPI_GEGLU>(grid, stream, p);
+  else if (p.epi_mode == EPI_RES) launch<EPI_RES>(grid, stream, p);
+  else launch<EPI_GENERIC>(grid, stream, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return svdx_fail_cuda(e, "tapgemm: launch");
   return SVDX_OK;

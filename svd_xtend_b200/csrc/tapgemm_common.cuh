@@ -9,20 +9,26 @@ namespace svdx {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;
-constexpr int STAGES = 3;
 constexpr int MAX_BN = 160;                           // widest tile: 80 accumulator registers per thread
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
 constexpr int B_STAGE_BYTES = MAX_BN * BLOCK_K * 2;   // 20 KB
 constexpr int NUM_EPI_WARPS = 8;   // the two consumer warpgroups: wgmma main loop, then the epilogue of the tile
 constexpr int PRODUCER_WARP = NUM_EPI_WARPS;
 constexpr int NUM_THREADS = 32 * NUM_EPI_WARPS + 32;
-// the finished fp32 accumulator tile in shared memory, one 128-row x MAX_BN tile; rows padded by 16 bytes so that the
-// epilogue's row-per-lane 16-byte reads are conflict-free
+// EPI_GENERIC parks the finished fp32 accumulator tile in shared memory, one 128-row x MAX_BN tile; rows padded by 16 bytes
+// so that the epilogue's row-per-lane 16-byte reads are conflict-free
 constexpr int ACC_LD = MAX_BN + 4;
 constexpr int ACC_BYTES = BLOCK_M * ACC_LD * 4;
 constexpr int EPI_STAGE_BYTES = 4096;  // per epilogue warp: 2 x (32 rows x 64 B) bf16 halves or 1 x (32 rows x 128 B) fp32
-constexpr int SMEM_BYTES = 1024 + STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + ACC_BYTES + NUM_EPI_WARPS * EPI_STAGE_BYTES + 256;
-static_assert(SMEM_BYTES <= 227 * 1024, "tapgemm shared memory exceeds the 227 KB a block may use");
+// operand ring depth: the parked tile leaves room for 3 stages; the register epilogues give its 84 KB to two more
+constexpr int STAGES_PARKED = 3;
+constexpr int STAGES_REGS = 5;
+constexpr int smem_bytes(int stages, bool parked) {
+  return 1024 + stages * (A_STAGE_BYTES + B_STAGE_BYTES) + (parked ? ACC_BYTES : 0) + NUM_EPI_WARPS * EPI_STAGE_BYTES + 256;
+}
+static_assert(smem_bytes(STAGES_PARKED, true) <= 227 * 1024, "tapgemm shared memory exceeds the 227 KB a block may use");
+static_assert(smem_bytes(STAGES_REGS, false) <= 227 * 1024, "tapgemm shared memory exceeds the 227 KB a block may use");
+static_assert(16 * STAGES_REGS <= 256, "ring barriers must fit their 256-byte region");
 static_assert((ACC_BYTES % 1024) == 0 && (B_STAGE_BYTES % 1024) == 0, "staging buffers must stay 1024-byte aligned");
 
 struct __align__(64) TapGemmKParams {
@@ -212,9 +218,9 @@ SVDX_DEVINL void gn_chunk_sums(const TapGemmKParams& p, uint32_t buf, int lane, 
 }
 
 // ---- specialised epilogues (kernel template parameter EPI): the hot shapes have short K, so the per-chunk instruction
-// count of the epilogue decides their speed. EPI_FAST / EPI_GEGLU assume a bf16 output
-// written through TMA, whole 32-column chunks (n_out % 32 == 0) and 16-byte aligned bias rows; everything else takes
-// the generic epilogue_tile below.
+// count of the epilogue decides their speed. Every EPI but EPI_GENERIC assumes a bf16 output written through TMA, whole
+// 32-column chunks (n_out % 32 == 0), 16-byte aligned bias rows and a K-major A operand, and reads the accumulator straight
+// from the wgmma registers (epilogue_regs); everything else parks the tile and takes the generic epilogue_tile below.
 constexpr int EPI_GENERIC = 0, EPI_FAST = 1, EPI_GEGLU = 2, EPI_RES = 3;
 // + fused GroupNorm statistics of the output (separate instantiations: the plain ones keep their register budget)
 constexpr int EPI_FAST_GN = 4, EPI_RES_GN = 5;
@@ -226,13 +232,14 @@ constexpr int EPI_FAST_IL = 7, EPI_FAST_IL_GN = 8;
 constexpr int EPI_FAST_ACT = 9;
 
 // the activations of EPI_FAST_ACT: GELU (erf) and quick_gelu x * sigmoid(1.702 x)
-SVDX_DEVINL void act32(float (&f)[32], int act) {
+template <int N>
+SVDX_DEVINL void act_n(float (&f)[N], int act) {
   if (act == SVDX_ACT_GELU) {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) f[i] = gelu_erf_f(f[i]);
+    for (int i = 0; i < N; ++i) f[i] = gelu_erf_f(f[i]);
   } else {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) f[i] = __fdividef(f[i], 1.0f + __expf(-1.702f * f[i]));
+    for (int i = 0; i < N; ++i) f[i] = __fdividef(f[i], 1.0f + __expf(-1.702f * f[i]));
   }
 }
 
@@ -269,30 +276,6 @@ SVDX_DEVINL void il_store_next_row(const TapGemmKParams& p, uint32_t src, int co
   }
 }
 
-SVDX_DEVINL void add_vec32(float (&f)[32], const float* __restrict__ src) {
-  const float4* bp = reinterpret_cast<const float4*>(src);
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const float4 b4 = __ldg(bp + k);
-    f[4 * k] += b4.x; f[4 * k + 1] += b4.y; f[4 * k + 2] += b4.z; f[4 * k + 3] += b4.w;
-  }
-}
-SVDX_DEVINL void axpy_bf16x32(float (&f)[32], float s, const uint4 (&r)[4]) {
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const float2 a = unpack_bf16x2(r[k].x), b = unpack_bf16x2(r[k].y), c = unpack_bf16x2(r[k].z), d = unpack_bf16x2(r[k].w);
-    f[8 * k] += s * a.x; f[8 * k + 1] += s * a.y; f[8 * k + 2] += s * b.x; f[8 * k + 3] += s * b.y;
-    f[8 * k + 4] += s * c.x; f[8 * k + 5] += s * c.y; f[8 * k + 6] += s * d.x; f[8 * k + 7] += s * d.y;
-  }
-}
-// one lane's 32 values -> its 64-byte row of a staging half (64B-swizzled)
-SVDX_DEVINL void stage_row_bf16(uint32_t row, int sw, const float (&f)[32]) {
-#pragma unroll
-  for (int j = 0; j < 4; ++j)
-    st_shared_v4(row + ((j ^ sw) << 4), pack_bf16x2(f[8 * j], f[8 * j + 1]), pack_bf16x2(f[8 * j + 2], f[8 * j + 3]),
-                 pack_bf16x2(f[8 * j + 4], f[8 * j + 5]), pack_bf16x2(f[8 * j + 6], f[8 * j + 7]));
-}
-
 // Epilogue operands that are read per chunk (the residual of EPI_RES, the GroupNorm input of EPI_FAST_GNB) are usually not in L2
 // any more; a warp has ONE chunk's loads in flight, so the fetch is latency-bound. Each epilogue warp therefore requests its 32 rows x bn columns of the tile
 // into L2 BEFORE its main loop: the lines arrive while the tensor cores work. Lane = row; the two warps of a lane
@@ -319,58 +302,14 @@ SVDX_DEVINL void prefetch_epilogue_operands(const TapGemmKParams& p, int epi, lo
   }
 }
 
-// plain epilogue (bias / row-bias only): two 32-column chunks per round (both staging halves), one proxy fence and one
-// bulk group per round. IL: interleaved (upsample phase) store. ACT: activation after the bias (p.act).
-template <bool GN, bool IL = false, bool ACT = false>
-SVDX_DEVINL void epilogue_fast(const TapGemmKParams& p, uint32_t t_base, long long m, bool row_ok, int n0, int half, int c_lo, int c_hi,
-                               int n_out_total, uint32_t sbase, int row0, int grp, int lane, long long m0, int valid_rows) {
-  const float* bias = p.bias;
-  const float* rb = (p.rowbias && row_ok) ? p.rowbias + (m / p.rowbias_div) * p.ldrb : nullptr;
-  const uint32_t rowX = sbase + lane * 64, rowY = rowX + 2048;
-  const int sw = (lane >> 1) & 3;
-#pragma unroll 1
-  for (int c = c_lo + half * 32; c < c_hi; c += 128) {           // accumulator columns [c_lo, c_hi) of the tile
-    const int colA = n0 + c;
-    if (colA >= n_out_total) break;
-    const int colB = colA + 64;
-    const bool hasB = (c + 64 < c_hi) && (colB < n_out_total);     // warp-uniform
-    uint32_t va[32], vb[32];
-    acc_ld32(t_base, c, va);
-    if (hasB) acc_ld32(t_base, c + 64, vb);
-    float fa[32], fb[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) { fa[i] = __uint_as_float(va[i]); fb[i] = __uint_as_float(vb[i]); }
-    if (bias) { add_vec32(fa, bias + colA); if (hasB) add_vec32(fb, bias + colB); }
-    if (rb) { add_vec32(fa, rb + colA); if (hasB) add_vec32(fb, rb + colB); }
-    if constexpr (ACT) { act32(fa, p.act); if (hasB) act32(fb, p.act); }
-    if (lane == 0) bulk_wait_read<0>();   // the previous round's stores have drained both halves
-    __syncwarp();
-    stage_row_bf16(rowX, sw, fa);
-    if (hasB) stage_row_bf16(rowY, sw, fb);
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) {
-      store_chunk<IL>(p, sbase, colA, row0, grp);
-      if (hasB) store_chunk<IL>(p, sbase + 2048, colB, row0, grp);
-      bulk_commit();
-    }
-    if constexpr (IL) {
-      il_store_next_row(p, sbase, colA, row0, lane);
-      if (hasB) il_store_next_row(p, sbase + 2048, colB, row0, lane);
-    }
-    if constexpr (GN) {
-      gn_chunk_sums(p, sbase, lane, colA, n_out_total, m0, valid_rows);
-      if (hasB) gn_chunk_sums(p, sbase + 2048, lane, colB, n_out_total, m0, valid_rows);
-    }
-  }
-}
-
 // ---- GroupNorm backward, pass 1, fused into the epilogue that WRITES dy (the dgrad conv / GEMM whose input was the
 // GroupNorm(+SiLU) output): per (slab, channel) S = sum_rows e and SX = sum_rows e * x with e = dy * act'(x * scale + shift),
 // from the staged bf16 dy chunk (exactly the values stored) and the matching 32 x 32 chunk of the GroupNorm input x staged
 // beside it. The consumer (svdx_groupnorm_bwd_fused) folds channels into groups: s1 = sum_c gamma_c S_c,
 // s2 = rstd * (sum_c gamma_c SX_c - mean * s1); dgamma_c = rstd * (SX_c - mean * S_c), dbeta_c = S_c. Same lane layout as
 // gn_chunk_sums (lane = column pair x row parity), slabs walked segment by segment.
+// ROWS: the rows the buffers hold (a 32-row chunk, or one warp's 16-row half of it).
+template <int ROWS = 32>
 SVDX_DEVINL void gnb_chunk_sums(const TapGemmKParams& p, uint32_t buf_dy, uint32_t buf_x, int lane, int col0, int n_out_total, long long m0,
                                 int valid_rows) {
   const int pr = lane & 15, h = lane >> 4;
@@ -389,11 +328,11 @@ SVDX_DEVINL void gnb_chunk_sums(const TapGemmKParams& p, uint32_t buf_dy, uint32
       B = *reinterpret_cast<const float2*>(p.gnb_ab + (2 * slab + 1) * p.N + col);
     }
     float s0 = 0.f, s1 = 0.f, x0 = 0.f, x1 = 0.f;
-    if (r == 0 && seg_end == 32) {
-      // the common case (a whole 32-row chunk inside one slab): rows h, h + 2, ... in two unrolled batches of 8 so that the
+    if (r == 0 && seg_end == ROWS) {
+      // the common case (all ROWS rows inside one slab): rows h, h + 2, ... in unrolled batches of 8 so that the
       // sigmoid chains (ex2 -> rcp) of different rows overlap; the rolled loop below ran one dependent chain at a time
 #pragma unroll
-      for (int b = 0; b < 2; ++b) {
+      for (int b = 0; b < ROWS / 16; ++b) {
         uint32_t wd[8], wx[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
@@ -446,174 +385,201 @@ SVDX_DEVINL void gnb_chunk_sums(const TapGemmKParams& p, uint32_t buf_dy, uint32
   }
 }
 
-// plain epilogue + gnb_chunk_sums: one chunk per round, staging half X = the dy chunk (TMA-store source), half Y = the x chunk
-SVDX_DEVINL void epilogue_fast_gnb(const TapGemmKParams& p, uint32_t t_base, long long m, bool row_ok, int n0, int half, int c_lo, int c_hi,
-                                   int n_out_total, uint32_t sbase, int row0, int grp, int lane, long long m0, int valid_rows) {
-  const float* bias = p.bias;
-  const float* rb = (p.rowbias && row_ok) ? p.rowbias + (m / p.rowbias_div) * p.ldrb : nullptr;
-  const uint32_t rowX = sbase + lane * 64;
-  const int sw = (lane >> 1) & 3;
-  const int prow = lane >> 2, ppc = lane & 3;
-#pragma unroll 1
-  for (int c = c_lo + half * 32; c < c_hi; c += 64) {
-    const int col0 = n0 + c;
-    if (col0 >= n_out_total) break;
-    // the matching chunk of the GroupNorm input, fetched coalesced (8 rows x 64 B per instruction) before the accumulator read
-    const bool src1 = col0 < p.gnb_c1;
-    const long long xld = src1 ? p.gnb_ldx : p.gnb_ldx2;
-    const bf16* xs = (src1 ? p.gnb_x + col0 : p.gnb_x2 + (col0 - p.gnb_c1)) + m0 * xld + ppc * 8;
-    uint4 xa[4];
+// ---- register epilogues (every EPI but EPI_GENERIC): the accumulator stays in the wgmma fragment registers. Consumer warp
+// w holds tile rows 16 w + lane / 4 + 8 h (h = 0, 1); its register 4 j + 2 h + e is column 8 j + 2 (lane % 4) + e. The two
+// warps of a pair (w = 2 q, 2 q + 1) own the 32-row quarter q: per 32-column chunk each stages its 16 rows as bf16 with
+// stmatrix into one 2 KB slot (32 rows x 64 B, 64B swizzle) of the pair's 8 KB, they meet on the pair's named barrier and
+// lane 0 of the first warp issues the 32 x 32 TMA store. The fused GroupNorm sums and the interleaved next-row stores read
+// the staged chunk as the parked epilogue did: each warp sums its own 16 rows, and the next-row stores alternate between the
+// two warps. Per element the arithmetic is the
+// parked epilogue's: bias, row-bias, scale, residuals, GEGLU / activation, round to bf16, in that order.
+struct PairStage {
+  uint32_t slots;   // the pair's 8 KB staging region: four 2 KB slots
+  int bar;          // the pair's named barrier (2..5)
+  int sub;          // 0: rows 0-15 of the quarter, issues the stores; 1: rows 16-31
+  uint32_t round;   // chunks staged so far: the slot ring position, carried across tiles
+};
+struct EpiTile {
+  int n0, n_out_total, row0, grp, valid_rows;   // row0 / grp: tensor-map coordinates of the quarter's first row
+  long long m0;                                 // global row of the quarter's first row; valid_rows of its 32 exist
+  long long m[2];                               // global rows 16 w + lane / 4 + 8 h of this thread
+  bool ok[2];
+};
+
+// byte offset of row r, 16-byte column piece j, in a 64B-swizzled slot (rows 64 B apart: 16 r and 16 (r & ~15) swizzle alike)
+SVDX_DEVINL uint32_t sw64(int r, int j) { return (uint32_t)(r * 64 + ((j ^ ((r >> 1) & 3)) << 4)); }
+// the row this lane addresses for stmatrix / ldmatrix x4 number x of a warp's 16 x 32 chunk: matrix lane / 8 of the four
+// covers column piece 2 x + (lane / 8) / 2 and rows 8 ((lane / 8) % 2) + [0, 8); register k of the x4 is fragment
+// register pair (j, h) = (2 x + k / 2, k % 2)
+SVDX_DEVINL uint32_t frag_row_addr(uint32_t base16, int lane, int x) {
+  const int mi = lane >> 3;
+  return base16 + sw64(8 * (mi & 1) + (lane & 7), 2 * x + (mi >> 1));
+}
+SVDX_DEVINL void stmatrix_x4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+SVDX_DEVINL void ldmatrix_x4(uint32_t addr, uint32_t& a, uint32_t& b, uint32_t& c, uint32_t& d) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d) : "r"(addr) : "memory");
+}
+// a chunk's 16 fragment values (f[4 j + 2 h + e]) -> this warp's 16 rows of a slot, bf16 (cvt.rn.bf16x2)
+SVDX_DEVINL void stage_frag16(uint32_t base16, int lane, const float (&f)[16]) {
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int rr = prow + 8 * j;
-      xa[j] = (rr < valid_rows) ? *reinterpret_cast<const uint4*>(xs + (long long)rr * xld) : make_uint4(0u, 0u, 0u, 0u);
-    }
-    uint32_t v[32];
-    acc_ld32(t_base, c, v);
-    float f[32];
+  for (int x = 0; x < 2; ++x)
+    stmatrix_x4(frag_row_addr(base16, lane, x), pack_bf16x2(f[8 * x], f[8 * x + 1]), pack_bf16x2(f[8 * x + 2], f[8 * x + 3]),
+                pack_bf16x2(f[8 * x + 4], f[8 * x + 5]), pack_bf16x2(f[8 * x + 6], f[8 * x + 7]));
+}
+// 16 rows x 32 bf16 columns of a row-major operand, fetched coalesced (lane: 16-byte piece lane % 4 of rows lane / 4 and
+// lane / 4 + 8, 8 rows x 64 B per instruction); rows >= nrows read as zero
+SVDX_DEVINL void load_rows16(const bf16* base, long long ld, int nrows, int lane, uint4 (&v)[2]) {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
-    if (bias) add_vec32(f, bias + col0);
-    if (rb) add_vec32(f, rb + col0);
-    if (lane == 0) bulk_wait_read<0>();   // the previous round's store has drained half X
-    __syncwarp();
-    stage_row_bf16(rowX, sw, f);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int rr = prow + 8 * j;
-      st_shared_v4(sbase + 2048 + rr * 64 + ((ppc ^ ((rr >> 1) & 3)) << 4), xa[j].x, xa[j].y, xa[j].z, xa[j].w);
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) { tma_store_3d(&p.tmo, sbase, col0, row0, grp); bulk_commit(); }
-    gnb_chunk_sums(p, sbase, sbase + 2048, lane, col0, n_out_total, m0, valid_rows);
-    __syncwarp();                          // all lanes are done with half Y before the next round overwrites it
+  for (int j = 0; j < 2; ++j) {
+    const int rr = (lane >> 2) + 8 * j;
+    v[j] = rr < nrows ? *reinterpret_cast<const uint4*>(base + (long long)rr * ld + (lane & 3) * 8) : make_uint4(0u, 0u, 0u, 0u);
   }
 }
-
-// residual / AlphaBlender epilogue: out = s_acc*(acc + bias + rowbias) + s_r1*res1 + s_r2*res2; one chunk per round,
-// alternating staging halves; the residual rows are requested before the accumulator read.
-template <bool GN>
-SVDX_DEVINL void epilogue_res(const TapGemmKParams& p, uint32_t t_base, long long m, bool row_ok, int n0, int half, int c_lo, int c_hi,
-                              int n_out_total, float s_acc, float s_r1, float s_r2, uint32_t sbase, uint32_t& off, int row0, int grp, int lane,
-                              long long m0, int valid_rows) {
-  const float* bias = p.bias;
-  const float* rb = (p.rowbias && row_ok) ? p.rowbias + (m / p.rowbias_div) * p.ldrb : nullptr;
-  // res1 (every residual add of the network) is fetched COALESCED: lane l loads the 16-byte piece l % 4 of rows l / 4 + 8 j
-  // (8 rows x 64 B = 8 cache lines per instruction instead of one line per lane: the row-per-lane form cost 32 L1 tag
-  // cycles per load and made the K = 320 / 640 residual GEMMs LSU-bound), the pieces are transposed through the staging half
-  // that is about to receive this chunk's output, and every lane reads back its own row. res2 (AlphaBlender only) stays direct.
-  const bf16* r1 = p.res1 ? p.res1 + m0 * p.ldr1 : nullptr;
-  const bf16* r2 = (p.res2 && row_ok) ? p.res2 + m * p.ldr2 : nullptr;
-  const bool scaled = p.scales != nullptr;
-  const uint32_t row = sbase + lane * 64;
-  const int sw = (lane >> 1) & 3;
-  const int prow = lane >> 2, ppc = lane & 3;
-  // `off` (which staging half comes next) lives in the caller across tiles: bulk_wait_read<1> only guarantees that the
-  // half written TWO stores ago has been read out
-#pragma unroll 1
-  for (int c = c_lo + half * 32; c < c_hi; c += 64) {
-    const int col0 = n0 + c;
-    if (col0 >= n_out_total) break;
-    uint4 a1[4], a2[4];
-    if (r1) {
+SVDX_DEVINL void stage_rows16(uint32_t base16, int lane, const uint4 (&v)[2]) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int rr = prow + 8 * j;
-        a1[j] = (rr < valid_rows) ? *reinterpret_cast<const uint4*>(r1 + (long long)rr * p.ldr1 + col0 + ppc * 8) : make_uint4(0u, 0u, 0u, 0u);
-      }
-    }
-    if (r2) {
-      const uint4* q = reinterpret_cast<const uint4*>(r2 + col0);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) a2[k] = q[k];
-    }
-    uint32_t v[32];
-    acc_ld32(t_base, c, v);
-    float f[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
-    if (bias) add_vec32(f, bias + col0);
-    if (rb) add_vec32(f, rb + col0);
-    if (scaled) {
-#pragma unroll
-      for (int i = 0; i < 32; ++i) f[i] *= s_acc;
-    }
-    if (lane == 0) bulk_wait_read<1>();
-    __syncwarp();
-    if (r1) {
-      // transpose the coalesced pieces through the (now free) staging half: same 64B swizzle as the output rows
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int rr = prow + 8 * j;
-        st_shared_v4(sbase + off + rr * 64 + ((ppc ^ ((rr >> 1) & 3)) << 4), a1[j].x, a1[j].y, a1[j].z, a1[j].w);
-      }
-      __syncwarp();
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(a1[k].x), "=r"(a1[k].y), "=r"(a1[k].z), "=r"(a1[k].w) : "r"(row + off + ((k ^ sw) << 4)));
-      axpy_bf16x32(f, s_r1, a1);
-    }
-    if (r2) axpy_bf16x32(f, s_r2, a2);
-    stage_row_bf16(row + off, sw, f);
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) { tma_store_3d(&p.tmo, sbase + off, col0, row0, grp); bulk_commit(); }
-    if constexpr (GN) gn_chunk_sums(p, sbase + off, lane, col0, n_out_total, m0, valid_rows);
-    off ^= 2048;
-  }
+  for (int j = 0; j < 2; ++j) st_shared_v4(base16 + sw64((lane >> 2) + 8 * j, lane & 3), v[j].x, v[j].y, v[j].z, v[j].w);
 }
 
-// GEGLU epilogue: value | gate column halves of the accumulator; optionally saves the bf16 pre-activation for backward.
-SVDX_DEVINL void epilogue_geglu(const TapGemmKParams& p, uint32_t t_base, int n0, int half, int bn_out, uint32_t sbase, int row0,
-                                int grp, int lane) {
+template <int EPI, int BN>
+SVDX_DEVINL void epilogue_regs(const TapGemmKParams& p, const float (&acc)[BN / 2], PairStage& ps, const EpiTile& t, int lane, float s_acc,
+                               float s_r1, float s_r2) {
+  constexpr bool GEGLU = EPI == EPI_GEGLU;
+  constexpr bool RES = EPI == EPI_RES || EPI == EPI_RES_GN;
+  constexpr bool GN = EPI == EPI_FAST_GN || EPI == EPI_RES_GN || EPI == EPI_FAST_IL_GN;
+  constexpr bool IL = EPI == EPI_FAST_IL || EPI == EPI_FAST_IL_GN;
+  constexpr bool GNB = EPI == EPI_FAST_GNB;
+  constexpr int BN_OUT = GEGLU ? BN / 2 : BN;
+  const int cq = 2 * (lane & 3);
+  const bool issuer = ps.sub == 0 && lane == 0;
+  const bool save_pre = GEGLU && p.pre != nullptr;
+  const int vr = t.valid_rows - 16 * ps.sub;             // rows of this warp's 16 that exist
+  const long long mw = t.m0 + 16 * ps.sub;               // global row of this warp's first row
   const float* bias = p.bias;
-  const bool save_pre = p.pre != nullptr;
-  const int nh = p.N / 2;
-  const uint32_t rowX = sbase + lane * 64, rowY = rowX + 2048;
-  const int sw = (lane >> 1) & 3;
-  uint32_t off = 0;
-#pragma unroll 1
-  for (int c = half * 32; c < bn_out; c += 64) {
-    const int col0 = n0 + c;
-    uint32_t v[32], gte[32];
-    acc_ld32(t_base, c, v);
-    acc_ld32(t_base, bn_out + c, gte);
-    float f[32], g[32];
+  // rows past the end read row 0's operands: they are clipped by the store and skipped by the sums
+  const float* rb[2] = {nullptr, nullptr};
+  const bf16* r2[2] = {nullptr, nullptr};
 #pragma unroll
-    for (int i = 0; i < 32; ++i) { f[i] = __uint_as_float(v[i]); g[i] = __uint_as_float(gte[i]); }
-    if (bias) { add_vec32(f, bias + col0); add_vec32(g, bias + nh + col0); }
-    if (save_pre) {
-      if (lane == 0) bulk_wait_read<0>();
-      __syncwarp();
-      stage_row_bf16(rowX, sw, f);
-      stage_row_bf16(rowY, sw, g);
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-        tma_store_3d(&p.tmpre, sbase, col0, row0, grp);
-        tma_store_3d(&p.tmpre, sbase + 2048, nh + col0, row0, grp);
-        bulk_commit();
+  for (int h = 0; h < 2; ++h) {
+    if (!GEGLU && p.rowbias) rb[h] = p.rowbias + (t.ok[h] ? t.m[h] / p.rowbias_div : 0) * p.ldrb;
+    if (RES && p.res2) r2[h] = p.res2 + (t.ok[h] ? t.m[h] : 0) * p.ldr2;
+  }
+#pragma unroll
+  for (int ch = 0; ch < BN_OUT / 32; ++ch) {
+    const int col0 = t.n0 + 32 * ch;
+    if (col0 >= t.n_out_total) break;                     // pair-uniform
+    // slots: a ring of four single-chunk slots (wait until the store three chunks back has been read before the barrier
+    // that frees its slot); GNB: dy | x slot pairs, alternating; GEGLU with pre: value | gate | output, fixed
+    const uint32_t slot = ps.slots + 2048u * (GNB ? 2 * (ps.round & 1) : save_pre ? 2 : (ps.round & 3));
+    const uint32_t mine = slot + 1024u * ps.sub;
+    uint4 xa[2];                                          // RES: res1 rows; GNB: the GroupNorm input rows
+    if constexpr (RES) {
+      if (p.res1) load_rows16(p.res1 + mw * p.ldr1 + col0, p.ldr1, vr, lane, xa);
+    }
+    if constexpr (GNB) {
+      const bool src1 = col0 < p.gnb_c1;
+      const long long xld = src1 ? p.gnb_ldx : p.gnb_ldx2;
+      load_rows16((src1 ? p.gnb_x + col0 : p.gnb_x2 + (col0 - p.gnb_c1)) + mw * xld, xld, vr, lane, xa);
+    }
+    uint32_t a2[8];
+    if constexpr (RES) {
+      if (p.res2) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) a2[k] = *reinterpret_cast<const uint32_t*>(r2[k & 1] + col0 + 8 * (k >> 1) + cq);
       }
     }
-    // the reference applies GEGLU on the bf16-rounded projection (autocast F.linear output)
+    float f[16], g[16];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const float fv = __bfloat162float(__float2bfloat16(f[i]));
-      const float gv = __bfloat162float(__float2bfloat16(g[i]));
-      f[i] = fv * gelu_erf_f(gv);
+    for (int i = 0; i < 16; ++i) {
+      f[i] = acc[16 * ch + i];
+      if constexpr (GEGLU) g[i] = acc[BN_OUT / 2 + 16 * ch + i];
     }
-    if (save_pre) {
-      if (lane == 0) bulk_wait_read<0>();
-    } else {
-      if (lane == 0) bulk_wait_read<1>();
+    if (bias) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col0 + 8 * j + cq));
+        f[4 * j] += b.x; f[4 * j + 1] += b.y; f[4 * j + 2] += b.x; f[4 * j + 3] += b.y;
+        if constexpr (GEGLU) {
+          const float2 bg = __ldg(reinterpret_cast<const float2*>(bias + p.N / 2 + col0 + 8 * j + cq));
+          g[4 * j] += bg.x; g[4 * j + 1] += bg.y; g[4 * j + 2] += bg.x; g[4 * j + 3] += bg.y;
+        }
+      }
     }
-    __syncwarp();
-    stage_row_bf16(save_pre ? rowX : rowX + off, sw, f);
+    if (!GEGLU && p.rowbias) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const float2 b = __ldg(reinterpret_cast<const float2*>(rb[k & 1] + col0 + 8 * (k >> 1) + cq));
+        f[2 * k] += b.x; f[2 * k + 1] += b.y;
+      }
+    }
+    if constexpr (EPI == EPI_FAST_ACT) act_n(f, p.act);
+    if constexpr (RES) {
+      if (p.scales) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) f[i] = __fmul_rn(f[i], s_acc);
+      }
+      if (p.res1) {
+        // the coalesced rows go through this warp's half of the slot that is about to receive its output, back in
+        // fragment order
+        uint32_t a1[8];
+        stage_rows16(mine, lane, xa);
+        __syncwarp();
+        ldmatrix_x4(frag_row_addr(mine, lane, 0), a1[0], a1[1], a1[2], a1[3]);
+        ldmatrix_x4(frag_row_addr(mine, lane, 1), a1[4], a1[5], a1[6], a1[7]);
+        __syncwarp();
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          const float2 a = unpack_bf16x2(a1[k]);
+          f[2 * k] = __fmaf_rn(s_r1, a.x, f[2 * k]); f[2 * k + 1] = __fmaf_rn(s_r1, a.y, f[2 * k + 1]);
+        }
+      }
+      if (p.res2) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          const float2 a = unpack_bf16x2(a2[k]);
+          f[2 * k] = __fmaf_rn(s_r2, a.x, f[2 * k]); f[2 * k + 1] = __fmaf_rn(s_r2, a.y, f[2 * k + 1]);
+        }
+      }
+    }
+    if constexpr (GEGLU) {
+      if (save_pre) {
+        // the bf16 pre-activation: value and gate columns through slots 0 and 1
+        stage_frag16(ps.slots + 1024u * ps.sub, lane, f);
+        stage_frag16(ps.slots + 2048u + 1024u * ps.sub, lane, g);
+        fence_proxy_async_smem();
+        if (issuer) bulk_wait_read<0>();                 // the previous chunk's output store has left slot 2
+        named_bar_sync(ps.bar, 64);
+        if (issuer) {
+          tma_store_3d(&p.tmpre, ps.slots, col0, t.row0, t.grp);
+          tma_store_3d(&p.tmpre, ps.slots + 2048u, p.N / 2 + col0, t.row0, t.grp);
+          bulk_commit();
+        }
+      }
+      // the reference applies GEGLU on the bf16-rounded projection (autocast F.linear output)
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const float fv = __bfloat162float(__float2bfloat16(f[i]));
+        const float gv = __bfloat162float(__float2bfloat16(g[i]));
+        f[i] = fv * gelu_erf_f(gv);
+      }
+    }
+    stage_frag16(mine, lane, f);
+    if constexpr (GNB) stage_rows16(mine + 2048u, lane, xa);
     fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) { tma_store_3d(&p.tmo, save_pre ? sbase : sbase + off, col0, row0, grp); bulk_commit(); }
-    off ^= 2048;
+    if (issuer) {
+      if (GNB || save_pre) bulk_wait_read<0>();
+      else bulk_wait_read<2>();
+    }
+    named_bar_sync(ps.bar, 64);
+    if (issuer) { store_chunk<IL>(p, slot, col0, t.row0, t.grp); bulk_commit(); }
+    if constexpr (IL) {
+      if ((ps.round & 1) == (uint32_t)ps.sub) il_store_next_row(p, slot, col0, t.row0, lane);
+    }
+    // each warp sums its own 16 rows of the staged chunk, so the two warps of a pair run their sums at the same time
+    if constexpr (GN) gn_chunk_sums(p, mine, lane, col0, t.n_out_total, mw, max(0, min(16, vr)));
+    if constexpr (GNB) gnb_chunk_sums<16>(p, mine, mine + 2048u, lane, col0, t.n_out_total, mw, max(0, min(16, vr)));
+    ++ps.round;
   }
 }
 

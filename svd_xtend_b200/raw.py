@@ -59,6 +59,11 @@ def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
 
+def _layout(t: torch.Tensor) -> dict:
+    """shape / strides / dtype of a launch operand (SHAPE_LOG): enough to rebuild a view of the same layout"""
+    return dict(shape=list(t.shape), stride=list(t.stride()), dtype=str(t.dtype).replace("torch.", ""))
+
+
 def _rowmajor(t: torch.Tensor, name: str) -> int:
     """leading dimension (elements) of a 2-D-like view whose last dim is contiguous."""
     if t.stride(-1) != 1:
@@ -228,7 +233,20 @@ def tapgemm(
         SHAPE_LOG.append(dict(M=M, N=N, K=K, taps=len(taps), conv2d=int(mode == A_CONV2D), geglu=int(geglu), a_mn=int(a_mn), b_mode=b_mode,
                               split_k=split_k, block_n=block_n, f32out=int(out.dtype != bf16), bias=int(bias is not None),
                               rowbias=int(rowbias is not None), res=int(res1 is not None) + int(res2 is not None),
-                              scales=int(scales is not None), pre=int(pre is not None)))
+                              scales=int(scales is not None), pre=int(pre is not None),
+                              # enough to rebuild the launch from seeded operands (scripts/bench_tapgemm_shapes.py)
+                              launch=dict(M=M, N=N, K=K, mode=mode, taps=[[int(v) for v in t] for t in taps], rows_per_group=rows_per_group,
+                                          groups=groups, conv_whn=None if conv_whn is None else [int(v) for v in conv_whn], lda=lda, ldb=ldb,
+                                          ldo=ldo, a_mn=bool(a_mn), b_mn=bool(b_mn), b_mode=b_mode, block_n=block_n, split_k=split_k,
+                                          out_dtype=out_dtype, geglu=bool(geglu), rowbias_div=rowbias_div, gn_rows=gn_rows,
+                                          phase=None if phase is None else [int(v) for v in phase], act=int(act),
+                                          gnb=None if gnb is None else dict(rows=int(gnb["rows"]), silu=bool(gnb["silu"])),
+                                          tensors={k: _layout(t) for k, t in (
+                                              ("a", a), ("b", b), ("out", out), ("bias", bias), ("rowbias", rowbias), ("res1", res1),
+                                              ("res2", res2), ("scales", scales), ("pre", pre), ("gn_sum", gn_sum),
+                                              ("gnb_x", None if gnb is None else gnb["x"]), ("gnb_x2", None if gnb is None else gnb.get("x2")),
+                                              ("gnb_ab", None if gnb is None else gnb.get("ab")), ("gnb_sum", None if gnb is None else gnb["sum"]))
+                                              if t is not None})))
     d = SvdxTapGemm()
     assert a.dtype == bf16 and b.dtype == bf16
     d.a = a.data_ptr()
