@@ -424,6 +424,18 @@ int svdx_adamw8bit_ema(const void* jobs, const int32_t* block_prefix, int32_t nj
 int svdx_multi_transpose(const void* src_base, const void* jobs, const int32_t* tile_prefix, int32_t njobs, int32_t total_tiles,
                          void* stream);
 
+/* LoRA fuse / unfuse (UNet fuse_lora / unfuse_lora): many base weights W [N, K] updated in place in one launch,
+ *   W[n,k] = round(fl(W[n,k] + tot)),  tot = sum over the job's terms, in order, of fl(scale * acc),
+ *   acc = sum over j < r, in order, of fl(B[n,j] * A[j,k])   (every product and sum rounded separately, no FMA; the
+ *   final rounding to bf16 / fp16 is to nearest even). oracle/svd_lora_oracle.py states the same in torch ops.
+ * jobs: device array of {void* w; int64 n; int64 k; int32 dtype; int32 term0; int32 nterms; int32 pad} (40 bytes);
+ * terms: device array of {const void* a [r, K]; const void* b [N, r]; int32 r (>= 1); int32 dtype; float scale; int32 pad}
+ * (32 bytes); job j uses terms[term0 .. term0 + nterms). dtype codes as above (0 fp32, 1 bf16, 2 fp16), a and b of one term
+ * share one. tile_prefix[j] = first 64x64 tile of job j, total_tiles = sum of ceil(n/64) * ceil(k/64). An unfuse is a
+ * fuse with negated scales: it restores W to within one unit in the last place of its dtype. */
+int svdx_lora_merge(const void* jobs, const void* terms, const int32_t* tile_prefix, int32_t njobs, int32_t total_tiles,
+                    void* stream);
+
 #ifdef __cplusplus
 }
 #endif

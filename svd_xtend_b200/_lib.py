@@ -122,6 +122,7 @@ _PROTOS = {
     "svdx_adamw8bit": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p],
     "svdx_adamw8bit_ema": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p],
     "svdx_multi_transpose": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p],
+    "svdx_lora_merge": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p],
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOS) + ("svdx_last_error",)

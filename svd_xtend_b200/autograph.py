@@ -58,7 +58,8 @@ class GraphRunner:
     def key(self, record, sample, timesteps, enc, added_time_ids) -> Tuple:
         m = self.model
         return (bool(record), bool(m.training), tuple(sample.shape), sample.dtype, tuple(enc.shape), enc.dtype, tuple(added_time_ids.shape),
-                timesteps.dtype, m.is_gradient_checkpointing, id(m._arena), sum(1 for p in m.parameters() if p.requires_grad))
+                timesteps.dtype, m.is_gradient_checkpointing, id(m._arena), sum(1 for p in m.parameters() if p.requires_grad),
+                getattr(m, "lora_stamp", 0))
 
     def busy(self) -> bool:
         return any(e.pending_backward for e in self.entries.values())
@@ -68,6 +69,11 @@ class GraphRunner:
         """returns (out, entry) when the call was served by a graph, else None (caller runs the eager tape)"""
         m = self.model
         k = self.key(record, sample, timesteps, enc, added_time_ids)
+        # graphs captured under an earlier adapter state can never be served again: drop them and their pools (one still
+        # waiting for its backward is dropped at a later call, once that backward has run)
+        stale = [old for old, ent in self.entries.items() if old[-1] != k[-1] and not ent.pending_backward]
+        for old in stale:
+            del self.entries[old]
         e = self.entries.get(k)
         if e is None:
             e = self.entries[k] = _Captured()

@@ -1058,6 +1058,99 @@ __global__ void multi_transpose_kernel(const bf16* __restrict__ src_base, const 
   }
 }
 
+// LoRA fuse / unfuse: W[n,k] += sum over terms of s_a * (B_a A_a)[n,k], in place, for many base weights in ONE launch.
+// block -> (job, 64x64 tile) through a tile prefix table (as multi_transpose_kernel). Per term, the tile's B rows and A
+// columns are staged in shared memory as fp32, LM_RC ranks at a time. Every product and sum is rounded separately (no FMA):
+//   acc = fl(acc + fl(B[n,j] * A[j,k])) over j;  tot = fl(tot + fl(s * acc)) over terms;  W = rn(fl(W + tot)).
+struct LoraMergeTerm {
+  const void* a;     // [r, K]
+  const void* b;     // [N, r]
+  int32_t r;
+  int32_t dtype;     // of a and b
+  float scale;
+  int32_t pad;
+};
+struct LoraMergeJob {
+  void* w;           // [N, K]
+  int64_t n, k;
+  int32_t dtype;
+  int32_t term0, nterms;
+  int32_t pad;
+};
+constexpr int LM_TILE = 64;
+constexpr int LM_RC = 64;                        // ranks per shared-memory chunk
+constexpr int LM_ROWS = LM_TILE / 4;             // rows per thread (256 threads = 64 columns x 4 row groups)
+
+SVDX_DEVINL float ld_any(const void* p, int dtype, long long i) {
+  if (dtype == 0) return reinterpret_cast<const float*>(p)[i];
+  if (dtype == 1) return __bfloat162float(reinterpret_cast<const bf16*>(p)[i]);
+  return __half2float(reinterpret_cast<const __half*>(p)[i]);
+}
+
+__global__ void __launch_bounds__(256) lora_merge_kernel(const LoraMergeJob* __restrict__ jobs, const LoraMergeTerm* __restrict__ terms,
+                                                         const int* __restrict__ tile_prefix, int njobs) {
+  __shared__ float bs[LM_TILE][LM_RC + 1];
+  __shared__ float as[LM_RC][LM_TILE];
+  int lo = 0, hi = njobs - 1;
+  const int blk = blockIdx.x;
+  while (lo < hi) {            // last job whose first tile <= blk
+    const int mid = (lo + hi + 1) >> 1;
+    if (tile_prefix[mid] <= blk) lo = mid; else hi = mid - 1;
+  }
+  const LoraMergeJob j = jobs[lo];
+  const int t = blk - tile_prefix[lo];
+  const long long tiles_k = (j.k + LM_TILE - 1) / LM_TILE;
+  const long long n0 = (t / tiles_k) * LM_TILE, k0 = (t % tiles_k) * LM_TILE;
+  const int tx = threadIdx.x % LM_TILE, ty = threadIdx.x / LM_TILE;
+  float tot[LM_ROWS];
+#pragma unroll
+  for (int i = 0; i < LM_ROWS; ++i) tot[i] = 0.f;
+  for (int q = 0; q < j.nterms; ++q) {
+    const LoraMergeTerm tm = terms[j.term0 + q];
+    float acc[LM_ROWS];
+#pragma unroll
+    for (int i = 0; i < LM_ROWS; ++i) acc[i] = 0.f;
+    for (int j0 = 0; j0 < tm.r; j0 += LM_RC) {
+      const int rc = tm.r - j0 < LM_RC ? tm.r - j0 : LM_RC;
+      __syncthreads();         // the previous chunk's readers are done
+      for (int e = threadIdx.x; e < LM_TILE * LM_RC; e += blockDim.x) {
+        const int c = e % LM_RC, row = e / LM_RC;      // B: consecutive threads walk the rank axis of one row
+        const long long n = n0 + row;
+        bs[row][c] = (c < rc && n < j.n) ? ld_any(tm.b, tm.dtype, n * tm.r + j0 + c) : 0.f;
+        const int kk = e % LM_TILE, jr = e / LM_TILE;  // A: consecutive threads walk K
+        const long long k = k0 + kk;
+        as[jr][kk] = (jr < rc && k < j.k) ? ld_any(tm.a, tm.dtype, (long long)(j0 + jr) * j.k + k) : 0.f;
+      }
+      __syncthreads();
+      for (int c = 0; c < rc; ++c) {
+        const float a = as[c][tx];
+#pragma unroll
+        for (int i = 0; i < LM_ROWS; ++i) acc[i] = __fadd_rn(acc[i], __fmul_rn(bs[ty + 4 * i][c], a));
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < LM_ROWS; ++i) tot[i] = __fadd_rn(tot[i], __fmul_rn(tm.scale, acc[i]));
+  }
+  const long long k = k0 + tx;
+  if (k >= j.k) return;
+#pragma unroll
+  for (int i = 0; i < LM_ROWS; ++i) {
+    const long long n = n0 + ty + 4 * i;
+    if (n >= j.n) break;
+    const long long o = n * j.k + k;
+    if (j.dtype == 0) {
+      float* w = reinterpret_cast<float*>(j.w);
+      w[o] = __fadd_rn(w[o], tot[i]);
+    } else if (j.dtype == 1) {
+      bf16* w = reinterpret_cast<bf16*>(j.w);
+      w[o] = __float2bfloat16_rn(__fadd_rn(__bfloat162float(w[o]), tot[i]));
+    } else {
+      __half* w = reinterpret_cast<__half*>(j.w);
+      w[o] = __float2half_rn(__fadd_rn(__half2float(w[o]), tot[i]));
+    }
+  }
+}
+
 }  // namespace svdx
 
 using namespace svdx;
@@ -1418,6 +1511,17 @@ extern "C" int svdx_multi_transpose(const void* src_base, const void* jobs, cons
   multi_transpose_kernel<<<total_tiles, dim3(32, 8), 0, ST(stream)>>>(reinterpret_cast<const bf16*>(src_base),
                                                                      reinterpret_cast<const TransposeJob*>(jobs), tile_prefix, njobs);
   SVDX_CHECK_LAUNCH("multi_transpose");
+  return SVDX_OK;
+}
+
+extern "C" int svdx_lora_merge(const void* jobs, const void* terms, const int32_t* tile_prefix, int32_t njobs, int32_t total_tiles,
+                               void* stream) {
+  if (!jobs || !terms || !tile_prefix || njobs <= 0 || total_tiles <= 0 || (reinterpret_cast<uintptr_t>(jobs) & 7) ||
+      (reinterpret_cast<uintptr_t>(terms) & 7) || (reinterpret_cast<uintptr_t>(tile_prefix) & 3))
+    return svdx_fail(SVDX_E_BADARG, "lora_merge: bad arguments (device job and term tables, tile prefix)");
+  lora_merge_kernel<<<total_tiles, 256, 0, ST(stream)>>>(reinterpret_cast<const LoraMergeJob*>(jobs),
+                                                         reinterpret_cast<const LoraMergeTerm*>(terms), tile_prefix, njobs);
+  SVDX_CHECK_LAUNCH("lora_merge");
   return SVDX_OK;
 }
 

@@ -48,6 +48,35 @@ class ImageToVideoPipeline:
             m.to(device)
         return self
 
+    # ---- LoRA adapters of the UNet (diffusers' pipeline method names; the file format lives in svd_xtend_b200.lora)
+    def load_lora_weights(self, pretrained_model_name_or_path_or_dict, adapter_name: Optional[str] = None,
+                          weight_name: Optional[str] = None) -> str:
+        return self.unet.load_lora_adapter(pretrained_model_name_or_path_or_dict, adapter_name=adapter_name, weight_name=weight_name)
+
+    @staticmethod
+    def save_lora_weights(save_directory: str, unet_lora_layers, weight_name: Optional[str] = None, safe_serialization: bool = True,
+                          **kwargs) -> str:
+        from .lora import save_lora_weights
+        return save_lora_weights(save_directory, unet_lora_layers, weight_name=weight_name, safe_serialization=safe_serialization)
+
+    def set_adapters(self, adapter_names, adapter_weights=None):
+        self.unet.set_adapters(adapter_names, adapter_weights)
+
+    def fuse_lora(self, lora_scale: float = 1.0, adapter_names=None):
+        self.unet.fuse_lora(lora_scale=lora_scale, adapter_names=adapter_names)
+
+    def unfuse_lora(self):
+        self.unet.unfuse_lora()
+
+    def unload_lora_weights(self):
+        self.unet.unload_lora()
+
+    def disable_lora(self):
+        self.unet.disable_lora()
+
+    def enable_lora(self):
+        self.unet.enable_lora()
+
     @torch.no_grad()
     def __call__(self, image: torch.Tensor, *, num_frames: Optional[int] = None, num_inference_steps: int = 25,
                  min_guidance_scale: float = 1.0, max_guidance_scale: float = 3.0, fps: int = 7, motion_bucket_id: int = 127,

@@ -808,6 +808,18 @@ def multi_transpose(src_base, jobs, tile_prefix, njobs, total_tiles):
           "svdx_multi_transpose")
 
 
+LM_TILE = 64         # tile edge of lora_merge_kernel
+
+
+def lora_merge(jobs, terms, tile_prefix, njobs, total_tiles, flops=0.0, nbytes=0.0):
+    """in-place LoRA fuse / unfuse of many base weights in one launch (svdx_lora_merge). jobs / terms: device bytes of the
+    tables (svd_xtend_b200.h); flops / nbytes are for the accounting only."""
+    if _fam("elementwise", flops, nbytes):
+        return
+    check(load().svdx_lora_merge(jobs.data_ptr(), terms.data_ptr(), tile_prefix.data_ptr(), njobs, total_tiles, _stream()),
+          "svdx_lora_merge")
+
+
 def unprep_conv_grad(src, dst, O, I, taps, i_pad):
     check(load().svdx_unprep_conv_grad(src.data_ptr(), dst.data_ptr(), O, I, taps, i_pad, _stream()), "svdx_unprep_conv_grad")
     return dst

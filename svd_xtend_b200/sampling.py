@@ -38,6 +38,7 @@ class VideoLatentSampler:
         self.use_cuda_graph = use_cuda_graph
         self._graph = None
         self._key = None
+        self._wstamp = None
 
     def _step(self, st):
         """one denoising step on the static buffers `st` (all device tensors; scal = [sigma, sigma_next, timestep])"""
@@ -81,6 +82,11 @@ class VideoLatentSampler:
             self._st = dict(latents=torch.empty(B, num_frames, 4, h, w, device=dev, dtype=F32), cond=torch.empty_like(cond),
                             emb=torch.empty_like(emb), ids=torch.empty_like(ids), scal=torch.zeros(3, device=dev, dtype=F32),
                             gs=torch.empty(1, num_frames, 1, 1, 1, device=dev, dtype=F32), cfg=cfg)
+        # the captured step replays the weight operands and LoRA scales of its capture: rewritten weights (load_state_dict,
+        # fuse_lora) or a changed adapter state need a new capture
+        wstamp = (getattr(self.unet, "lora_stamp", 0), tuple(p._version for p in self.unet.parameters()))
+        if self._graph is not None and self._wstamp != wstamp:
+            self._graph = None
         st = self._st
         st["latents"].copy_(noise.float() * math.sqrt(float(sigmas[0]) ** 2 + 1.0))
         st["cond"].copy_(cond)
@@ -112,7 +118,7 @@ class VideoLatentSampler:
                     with torch.cuda.graph(g):
                         self._step(st)
                     st["latents"].copy_(saved)
-                    self._graph = g
+                    self._graph, self._wstamp = g, wstamp
                 self._graph.replay()
         finally:
             self.unet.train(was_training)

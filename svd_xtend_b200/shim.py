@@ -61,6 +61,18 @@ def install(use_8bit_adam: bool | None = None) -> None:
     if wants_8bit_adam(sys.argv[1:]) if use_8bit_adam is None else use_8bit_adam:
         install_adam8bit()
     install_clip()
+    install_lora_writer(getattr(diffusers, "StableVideoDiffusionPipeline", None))
+
+
+def install_lora_writer(pipeline_cls) -> bool:
+    """train_svd_lora.py:1064-1074 and :1146-1153 call `StableVideoDiffusionPipeline.save_lora_weights(...)`, which some
+    diffusers releases lack. Where the class lacks it, the writer of svd_xtend_b200.lora (diffusers' file layout) is set;
+    an existing one is left alone. Returns whether it was set."""
+    if pipeline_cls is None or hasattr(pipeline_cls, "save_lora_weights"):
+        return False
+    from .lora import save_lora_weights
+    pipeline_cls.save_lora_weights = staticmethod(save_lora_weights)
+    return True
 
 
 def install_adam8bit():

@@ -293,26 +293,50 @@ class UNetSpatioTemporalConditionOutput:
 class LoraLinear(nn.Module):
     """PEFT-compatible LoRA wrapper layout (base_layer + lora_A/lora_B ModuleDicts keyed by adapter name), so that
     parameter names match what `unet.add_adapter(LoraConfig)` of train_svd_lora.py:659-671 produces:
-    `<linear>.base_layer.weight`, `<linear>.lora_A.default.weight` [r,in], `<linear>.lora_B.default.weight` [out,r]."""
+    `<linear>.base_layer.weight`, `<linear>.lora_A.default.weight` [r,in], `<linear>.lora_B.default.weight` [out,r].
+    Per adapter, under PEFT's names: `r`, `lora_alpha`, `scaling` (= lora_alpha / r), the user weight of `set_adapters`
+    (`adapter_weights`, default 1.0), and whether it is merged into the base weight (`merged_adapters`, with the fp32 scale it
+    was merged with in `merged_scales`, so that an unmerge subtracts the same term)."""
 
     def __init__(self, base: nn.Linear, r: int, lora_alpha: float, adapter_name: str = "default", init: str = "gaussian"):
         super().__init__()
         self.base_layer = base
         self.in_features, self.out_features = base.in_features, base.out_features
-        self.lora_A = nn.ModuleDict({adapter_name: nn.Linear(base.in_features, r, bias=False)})
-        self.lora_B = nn.ModuleDict({adapter_name: nn.Linear(r, base.out_features, bias=False)})
-        self.scaling = {adapter_name: lora_alpha / r}
-        self.active_adapters = [adapter_name]
-        self.r = {adapter_name: r}
+        self.lora_A = nn.ModuleDict()
+        self.lora_B = nn.ModuleDict()
+        self.r, self.lora_alpha, self.scaling, self.adapter_weights = {}, {}, {}, {}
+        self.active_adapters: List[str] = []
+        self.merged_adapters: List[str] = []
+        self.merged_scales: Dict[str, float] = {}
+        self.disable_adapters = False
+        self.add(adapter_name, r, lora_alpha, init)
+
+    def add(self, adapter_name: str, r: int, lora_alpha: float, init: str = "gaussian"):
+        A = nn.Linear(self.in_features, r, bias=False)
+        B = nn.Linear(r, self.out_features, bias=False)
         with torch.no_grad():
             if init == "gaussian":
-                nn.init.normal_(self.lora_A[adapter_name].weight, std=1.0 / r)
+                nn.init.normal_(A.weight, std=1.0 / r)
             else:
-                nn.init.kaiming_uniform_(self.lora_A[adapter_name].weight, a=math.sqrt(5))
-            nn.init.zeros_(self.lora_B[adapter_name].weight)
-        dev, dt = base.weight.device, base.weight.dtype
-        self.lora_A.to(device=dev, dtype=dt)
-        self.lora_B.to(device=dev, dtype=dt)
+                nn.init.kaiming_uniform_(A.weight, a=math.sqrt(5))
+            nn.init.zeros_(B.weight)
+        dev, dt = self.base_layer.weight.device, self.base_layer.weight.dtype
+        self.lora_A[adapter_name] = A.to(device=dev, dtype=dt)
+        self.lora_B[adapter_name] = B.to(device=dev, dtype=dt)
+        self.r[adapter_name], self.lora_alpha[adapter_name] = r, lora_alpha
+        self.scaling[adapter_name] = lora_alpha / r
+        self.adapter_weights[adapter_name] = 1.0
+
+    def remove(self, adapter_name: str):
+        for d in (self.lora_A, self.lora_B):
+            del d[adapter_name]
+        for d in (self.r, self.lora_alpha, self.scaling, self.adapter_weights):
+            d.pop(adapter_name)
+        self.active_adapters = [n for n in self.active_adapters if n != adapter_name]
+
+    @property
+    def merged(self) -> bool:
+        return bool(self.merged_adapters)
 
     @property
     def weight(self):
@@ -323,19 +347,15 @@ class LoraLinear(nn.Module):
         return self.base_layer.bias
 
 
-def _lora_of(lin: nn.Module, off: int = 0):
-    """(col_offset, out_features, A, B, scale) of a LoRA-wrapped linear (ours or PEFT's), else None."""
-    if not hasattr(lin, "lora_A") or not hasattr(lin, "base_layer"):
-        return None
-    names = [n for n in getattr(lin, "active_adapters", list(lin.lora_A.keys())) if n in lin.lora_A]
-    if not names:
-        return None
-    if len(names) > 1:
-        raise NotImplementedError("svd_xtend_b200: one active LoRA adapter per layer is supported")
-    n = names[0]
-    if getattr(lin, "merged", False):
-        return None
-    return (off, lin.lora_B[n].weight.shape[0], lin.lora_A[n].weight, lin.lora_B[n].weight, float(lin.scaling[n]))
+def _lora_of(lin: nn.Module, off: int = 0) -> list:
+    """[(col_offset, out_features, A, B, scaling * weight)] of a LoRA-wrapped linear (ours or PEFT's): one term per active,
+    unmerged adapter; none when the layer is plain or its adapters are disabled."""
+    if not hasattr(lin, "lora_A") or not hasattr(lin, "base_layer") or getattr(lin, "disable_adapters", False):
+        return []
+    merged = set(getattr(lin, "merged_adapters", ()))
+    weights = getattr(lin, "adapter_weights", {})
+    return [(off, lin.lora_B[n].weight.shape[0], lin.lora_A[n].weight, lin.lora_B[n].weight, float(lin.scaling[n]) * weights.get(n, 1.0))
+            for n in getattr(lin, "active_adapters", list(lin.lora_A.keys())) if n in lin.lora_A and n not in merged]
 
 
 def _sinusoid(t: torch.Tensor, dim: int) -> torch.Tensor:
@@ -465,6 +485,10 @@ class UNetSpatioTemporalConditionModel(nn.Module):
         self.grad_hook = None   # callable(list_of_params) invoked as soon as parameter gradients are final (DDP overlap)
         self._arena = None
         self._graphs = None     # autograph.GraphRunner: shape-keyed CUDA graphs of this module's forward / backward
+        self.peft_config: Dict[str, object] = {}     # adapter name -> the config object add_adapter was given (PEFT's attribute)
+        self.lora_stamp = 0     # moves on every change of adapter state: captured graphs keyed on it are re-captured
+        self._active_adapters: List[str] = []
+        self._fuse_calls: List[list] = []    # per fuse_lora call: (LoraLinear, [(name, -scale)]), what unfuse_lora subtracts
 
     # ------------------------------------------------------------------ training plumbing (svd_xtend_b200.train)
     def attach_arena(self, arena):
@@ -576,24 +600,198 @@ class UNetSpatioTemporalConditionModel(nn.Module):
 
     def add_adapter(self, adapter_config, adapter_name: str = "default"):
         """LoRA injection with the surface of diffusers' PeftAdapterMixin.add_adapter (train_svd_lora.py:671): wraps
-        every nn.Linear whose name ends with one of `target_modules` (to_k, to_q, to_v, to_out.0 at :659-664),
-        freezes the base model and leaves only lora_A / lora_B trainable."""
+        every nn.Linear whose name ends with one of `target_modules` (to_k, to_q, to_v, to_out.0 at :659-664), or adds the
+        adapter to such a layer that is already wrapped, freezes the base model and leaves only the new adapter's lora_A /
+        lora_B trainable. The config object is kept as `peft_config[adapter_name]`; the new adapter becomes the active one."""
+        self._check_new_adapter_name(adapter_name)
         targets = list(getattr(adapter_config, "target_modules"))
         r = int(getattr(adapter_config, "r"))
         alpha = float(getattr(adapter_config, "lora_alpha", r))
         init = getattr(adapter_config, "init_lora_weights", True)
-        self.requires_grad_(False)
-        n = 0
-        for parent_name, parent in list(self.named_modules()):
-            for child_name, child in list(parent.named_children()):
-                full = f"{parent_name}.{child_name}" if parent_name else child_name
-                if isinstance(child, nn.Linear) and any(full == t or full.endswith("." + t) for t in targets):
-                    setattr(parent, child_name, LoraLinear(child, r, alpha, adapter_name, "gaussian" if init == "gaussian" else "kaiming"))
-                    n += 1
-        if n == 0:
+        init = "gaussian" if init == "gaussian" else "kaiming"
+        slots = [(full, parent, child_name, child) for full, parent, child_name, child in self._linear_slots()
+                 if any(full == t or full.endswith("." + t) for t in targets)]
+        if not slots:
             raise ValueError(f"add_adapter: no module matched target_modules={targets}")
+        adaptable = self._adaptable()
+        refused = [full for full, _, _, _ in slots if full not in adaptable]
+        if refused:
+            raise ValueError(f"add_adapter: target_modules={targets} match linears without a LoRA side path on this build "
+                             f"(only the attention projections to_q / to_k / to_v / to_out.0 take one): {refused[:8]}")
+        matched = [(parent, child_name, child) for _, parent, child_name, child in slots]
+        self.requires_grad_(False)
+        self._inject(adapter_name, [(parent, child_name, child, r, alpha, init) for parent, child_name, child in matched])
+        self.peft_config[adapter_name] = adapter_config
+        return len(matched)
+
+    # ------------------------------------------------------------------ LoRA adapters (diffusers' adapter API)
+    def _linear_slots(self):
+        """(full name, parent, attribute, module) of every nn.Linear or LoraLinear of the model (not the linears inside a
+        LoraLinear)"""
+        inside = tuple(n + "." for n, m in self.named_modules() if isinstance(m, LoraLinear))
+        out = []
+        for parent_name, parent in list(self.named_modules()):
+            if isinstance(parent, LoraLinear) or (inside and (parent_name + ".").startswith(inside)):
+                continue
+            for child_name, child in list(parent.named_children()):
+                if isinstance(child, (nn.Linear, LoraLinear)):
+                    out.append((f"{parent_name}.{child_name}" if parent_name else child_name, parent, child_name, child))
+        return out
+
+    def _adaptable(self) -> set:
+        """full names of the linears that take a LoRA side path in forward and backward (`_lora_of` call sites): the
+        attention projections. attn2.to_q / to_k are among them: their output never reaches the result (one key), in the
+        reference as here, so an adapter on them changes nothing either way."""
+        out = set()
+        for name, m in self.named_modules():
+            if isinstance(m, Attention):
+                out.update(f"{name}.{p}" for p in ("to_q", "to_k", "to_v", "to_out.0"))
+        return out
+
+    def _lora_layers(self) -> List[LoraLinear]:
+        return [m for m in self.modules() if isinstance(m, LoraLinear)]
+
+    def _check_new_adapter_name(self, adapter_name: str):
+        if not isinstance(adapter_name, str) or not adapter_name or "." in adapter_name:
+            raise ValueError(f"adapter name must be a non-empty string without '.', got {adapter_name!r}")
+        if adapter_name in self.peft_config:
+            raise ValueError(f"adapter {adapter_name!r} already exists; delete_adapters it first or choose another name")
+
+    def _inject(self, adapter_name: str, slots):
+        """slots: (parent, attribute, nn.Linear or LoraLinear, r, lora_alpha, init). Adds the adapter to every slot and makes
+        it the only active adapter."""
+        for parent, child_name, child, r, alpha, init in slots:
+            if isinstance(child, LoraLinear):
+                child.add(adapter_name, r, alpha, init)
+            else:
+                setattr(parent, child_name, LoraLinear(child, r, alpha, adapter_name, init))
         self._engine.wc.clear()
-        return n
+        self._set_active([adapter_name])
+
+    def _set_active(self, names: List[str], weights: Optional[List[float]] = None):
+        for layer in self._lora_layers():
+            layer.active_adapters = [n for n in names if n in layer.lora_A]
+            if weights is not None:
+                for n, w in zip(names, weights):
+                    if n in layer.adapter_weights:
+                        layer.adapter_weights[n] = float(w)
+        self._active_adapters = list(names)
+        self.lora_stamp += 1
+
+    def _check_known(self, names, what: str):
+        unknown = [n for n in names if n not in self.peft_config]
+        if unknown:
+            raise ValueError(f"{what}: unknown adapter(s) {unknown}; present: {list(self.peft_config)}")
+
+    def _check_not_fused(self, names, what: str):
+        fused = sorted({n for layer in self._lora_layers() for n in layer.merged_adapters if n in names})
+        if fused:
+            raise ValueError(f"{what}: adapter(s) {fused} are fused into the base weights; unfuse_lora() first")
+
+    def active_adapters(self) -> List[str]:
+        """names of the active adapters (empty when there are none)"""
+        return [n for n in getattr(self, "_active_adapters", []) if n in self.peft_config]
+
+    def set_adapters(self, adapter_names, weights=None):
+        """make `adapter_names` (a name or a list) the active adapters, each with its weight (a number for all, a list, or
+        None for 1.0): the layer output is W x + sum over active adapters of weight * scaling * B A x"""
+        names = [adapter_names] if isinstance(adapter_names, str) else list(adapter_names)
+        if weights is None:
+            weights = [1.0] * len(names)
+        elif not isinstance(weights, (list, tuple)):
+            weights = [weights] * len(names)
+        if len(weights) != len(names):
+            raise ValueError(f"set_adapters: {len(names)} adapter names but {len(weights)} weights")
+        self._check_known(names, "set_adapters")
+        self._check_not_fused(names, "set_adapters")
+        self._set_active(names, [float(w) for w in weights])
+
+    def disable_lora(self):
+        """run the base model alone (adapters already fused stay in the base weights)"""
+        for layer in self._lora_layers():
+            layer.disable_adapters = True
+        self.lora_stamp += 1
+
+    def enable_lora(self):
+        for layer in self._lora_layers():
+            layer.disable_adapters = False
+        self.lora_stamp += 1
+
+    def delete_adapters(self, adapter_names):
+        names = [adapter_names] if isinstance(adapter_names, str) else list(adapter_names)
+        self._check_known(names, "delete_adapters")
+        self._check_not_fused(names, "delete_adapters")
+        for layer in self._lora_layers():
+            for n in names:
+                if n in layer.lora_A:
+                    layer.remove(n)
+        for n in names:
+            self.peft_config.pop(n)
+        self._engine.wc.clear()
+        self._set_active([n for n in self.active_adapters() if n not in names])
+
+    def unload_lora(self):
+        """remove every LoRA wrapper and put the plain nn.Linear back; adapters fused into the base weights stay there"""
+        for _, parent, child_name, child in self._linear_slots():
+            if isinstance(child, LoraLinear):
+                setattr(parent, child_name, child.base_layer)
+        self.peft_config.clear()
+        self._fuse_calls = []
+        self._engine.wc.clear()
+        self._set_active([])
+
+    def _merge(self, items, what: str):
+        """items: (LoraLinear, [(adapter name, fp32-rounded scale)]) -> one svdx_lora_merge launch over their base weights"""
+        from . import lora
+        for layer, _ in items:
+            w = layer.base_layer.weight
+            if not w.is_cuda:
+                raise RuntimeError(f"svd_xtend_b200: {what} runs on the CUDA kernels only; there is no CPU fallback (move the UNet to the GPU)")
+            if w.requires_grad:
+                raise ValueError(f"{what}: a base weight is trainable; fusing into a trainable base is not supported")
+        lora.merge_into_base([(layer.base_layer.weight, [(layer.lora_A[n].weight, layer.lora_B[n].weight, s) for n, s in terms])
+                              for layer, terms in items])
+        torch.autograd.graph.increment_version([layer.base_layer.weight for layer, _ in items])
+        self.lora_stamp += 1
+
+    def fuse_lora(self, lora_scale: float = 1.0, adapter_names=None):
+        """merge the active (or named) adapters into the base weights in place, in one kernel launch: each layer then holds
+        W + lora_scale * weight * scaling * B A, so state_dict / save_pretrained see the merged weights. Adapters already
+        fused are skipped."""
+        names = self.active_adapters() if adapter_names is None else \
+            ([adapter_names] if isinstance(adapter_names, str) else list(adapter_names))
+        self._check_known(names, "fuse_lora")
+        items = []
+        for layer in self._lora_layers():
+            terms = [(n, float(torch.tensor(float(lora_scale) * layer.adapter_weights[n] * layer.scaling[n], dtype=F32)))
+                     for n in names if n in layer.lora_A and n not in layer.merged_adapters]
+            if terms:
+                items.append((layer, terms))
+        if not items:
+            return
+        self._merge(items, "fuse_lora")
+        for layer, terms in items:
+            for n, s in terms:
+                layer.merged_adapters.append(n)
+                layer.merged_scales[n] = s
+        self._fuse_calls.append([(layer, [(n, -s) for n, s in terms]) for layer, terms in items])
+
+    def unfuse_lora(self):
+        """subtract every fused adapter from the base weights again, undoing the fuse_lora calls last first, one launch each:
+        each call's terms are subtracted with exactly the negated sum that call added, so every call leaves at most one ulp of
+        the base dtype behind (at the larger of the weight's magnitudes before and after that fuse)"""
+        calls, self._fuse_calls = self._fuse_calls, []
+        for items in reversed(calls):
+            self._merge(items, "unfuse_lora")
+        for layer in self._lora_layers():
+            layer.merged_adapters, layer.merged_scales = [], {}
+
+    def load_lora_adapter(self, pretrained_model_name_or_path_or_dict, adapter_name: Optional[str] = None,
+                          weight_name: Optional[str] = None):
+        """load a LoRA file written by save_lora_weights (or a directory holding one, or its state dict) as a new adapter
+        (svd_xtend_b200.lora.load_into); it becomes the active adapter. Returns the adapter name."""
+        from . import lora
+        return lora.load_into(self, pretrained_model_name_or_path_or_dict, adapter_name, weight_name)
 
     def register_to_config(self, **kwargs):
         for k, v in kwargs.items():
@@ -815,14 +1013,14 @@ class UNetSpatioTemporalConditionModel(nn.Module):
     @staticmethod
     def _qkv_lora(attn: Attention):
         C = attn.inner_dim
-        return [_lora_of(attn.to_q, 0), _lora_of(attn.to_k, C), _lora_of(attn.to_v, 2 * C)]
+        return _lora_of(attn.to_q, 0) + _lora_of(attn.to_k, C) + _lora_of(attn.to_v, 2 * C)
 
     def _cross_vec(self, E: Engine, attn2: Attention, enc: Var) -> Var:
         """Image cross-attention has ONE key/value token (train_svd.py:1000-1001), so softmax == 1 and the
         attention output is to_out(to_v(e)) for every query of the clip (SURVEY.md §0 quirk 3): a [B, C]
         vector, added through the row-bias epilogue. to_q / to_k / norm2 receive exactly zero gradient."""
-        v = E.linear(enc, attn2.to_v.weight, lora=[_lora_of(attn2.to_v)])
-        c = E.linear(v, attn2.to_out[0].weight, attn2.to_out[0].bias, lora=[_lora_of(attn2.to_out[0])])
+        v = E.linear(enc, attn2.to_v.weight, lora=_lora_of(attn2.to_v))
+        c = E.linear(v, attn2.to_out[0].weight, attn2.to_out[0].bias, lora=_lora_of(attn2.to_out[0]))
         return E.cast_to_f32(c)
 
     def _frame_emb(self, E: Engine, tr: TransformerSpatioTemporalModel, g: Geom):
@@ -858,7 +1056,7 @@ class UNetSpatioTemporalConditionModel(nn.Module):
             qkv = E.linear(n1, None, fused=[sb.attn1.to_q.weight, sb.attn1.to_k.weight, sb.attn1.to_v.weight], lora=self._qkv_lora(sb.attn1))
             a = E.attention(qkv, heads, g, temporal=False)
             x1 = E.linear(a, sb.attn1.to_out[0].weight, sb.attn1.to_out[0].bias, res1=x0,
-                          rowbias=self._cross_vec(E, sb.attn2, enc), rowbias_div=per_clip, lora=[_lora_of(sb.attn1.to_out[0])])
+                          rowbias=self._cross_vec(E, sb.attn2, enc), rowbias_div=per_clip, lora=_lora_of(sb.attn1.to_out[0]))
             _, n3 = E.layernorm(x1, sb.norm3)
             ff = E.linear(n3, sb.ff.net[0].proj.weight, sb.ff.net[0].proj.bias, geglu=True)
             return E.linear(ff, sb.ff.net[2].weight, sb.ff.net[2].bias, res1=x1)
@@ -876,7 +1074,7 @@ class UNetSpatioTemporalConditionModel(nn.Module):
         qkv = E.linear(n1, None, fused=[tb.attn1.to_q.weight, tb.attn1.to_k.weight, tb.attn1.to_v.weight], lora=self._qkv_lora(tb.attn1))
         a = E.attention(qkv, heads, g, temporal=True)
         y2 = E.linear(a, tb.attn1.to_out[0].weight, tb.attn1.to_out[0].bias, res1=y1,
-                      rowbias=self._cross_vec(E, tb.attn2, enc), rowbias_div=per_clip, lora=[_lora_of(tb.attn1.to_out[0])])
+                      rowbias=self._cross_vec(E, tb.attn2, enc), rowbias_div=per_clip, lora=_lora_of(tb.attn1.to_out[0]))
         _, n3 = E.layernorm(y2, tb.norm3)
         ff = E.linear(n3, tb.ff.net[0].proj.weight, tb.ff.net[0].proj.bias, geglu=True)
         s8 = self._blend(E, tr.time_mixer)
