@@ -43,6 +43,9 @@ extern "C" {
 #define SVDX_OUT_BF16 0
 #define SVDX_OUT_F32 1
 #define SVDX_OUT_F32_ATOMIC 2  /* out += result (fp32 red.add), used by split-K weight gradients */
+/* fp32 outputs (SVDX_OUT_F32 / SVDX_OUT_F32_ATOMIC) without bias / rowbias / res1 / res2 / GEGLU run an epilogue from the
+ * accumulator registers (scales[0] applied; any operand majors and b_mode, any N, split-K); fp32 outputs with those operands
+ * run the generic epilogue. Both give bit-identical stores. fp32 rows must be 16-byte aligned (ldo % 4 == 0). */
 
 /*
  * svdx_tapgemm — the one tensor-core contraction of the path (wgmma, register accumulators,
@@ -70,8 +73,8 @@ typedef struct SvdxTapGemm {
   const void* a;
   int64_t lda;          /* elements between consecutive rows/pixels */
   int32_t a_mode;       /* SVDX_A_ROWS / SVDX_A_CONV2D */
-  int32_t a_major_mn;   /* 0: A[m][k] k contiguous. 1 (ROWS, groups==1 only): memory is [k][m], m contiguous; runs the
-                           generic epilogue, so no gn_sum / gnb sums / act / interleave / block_n 320 */
+  int32_t a_major_mn;   /* 0: A[m][k] k contiguous. 1 (ROWS, groups==1 only): memory is [k][m], m contiguous; a bf16 output runs
+                           the generic epilogue, so no gn_sum / gnb sums / act / interleave / block_n 320 */
   int32_t rows_per_group, groups;      /* ROWS   */
   int32_t W, H, nimg;                  /* CONV2D (and b_mode 1): any W > 0; see SVDX_A_CONV2D for how each width is tiled */
   int32_t num_taps;

@@ -59,7 +59,9 @@ def epilogue_name(L, raw):
     f32 = L["out_dtype"] not in (None, raw.OUT_BF16) or t["out"]["dtype"] != "bfloat16"
     n_out = L["N"] // 2 if L["geglu"] else L["N"]
     res = any(k in t for k in ("res1", "res2", "scales"))
-    if f32 or L["split_k"] > 1 or L["a_mn"] or n_out % 32 or (L["b_mn"] and res):
+    if f32:
+        return "GENERIC" if any(k in t for k in ("bias", "rowbias", "res1", "res2")) else "F32"
+    if L["split_k"] > 1 or L["a_mn"] or n_out % 32 or (L["b_mn"] and res):
         return "GENERIC"
     if L["act"]:
         return "FAST_ACT"

@@ -6,9 +6,9 @@
 //   warp 8      : TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
 //   warps 0..7  : two consumer warpgroups; warpgroup g multiplies rows [64g, 64g + 64) of the 128-row tile with wgmma,
 //                 then runs the epilogue (bias / rowbias / GEGLU / residual / blend, staged TMA stores) straight from
-//                 the accumulator registers (bf16 outputs, 5-stage ring) or, in EPI_GENERIC, from the fp32 tile parked
-//                 in shared memory (3-stage ring). The producer keeps filling the ring meanwhile, so the next tile's
-//                 operands are resident when the epilogue ends.
+//                 the accumulator registers (bf16 outputs and plain / scaled fp32 outputs, 5-stage ring) or, in
+//                 EPI_GENERIC, from the fp32 tile parked in shared memory (3-stage ring). The producer keeps filling the
+//                 ring meanwhile, so the next tile's operands are resident when the epilogue ends.
 //
 // A-operand modes (see include/svd_xtend_b200.h): plain/grouped rows with row-shifted taps
 // (linear, (3,1,1) temporal conv [D: TemporalResnetBlock]) and channels-last images with 2-D
@@ -127,6 +127,32 @@ SVDX_DEVINL void tile_regs(const TapGemmKParams& p, int kb0, int kb1, Ring& rg, 
       case 128: tile_regs_bn<EPI, 128, 0>(p, kb0, kb1, rg, wg, ps, t, lane, s_acc, s_r1, s_r2); break;
       default: tile_regs_bn<EPI, 160, 0>(p, kb0, kb1, rg, wg, ps, t, lane, s_acc, s_r1, s_r2); break;
     }
+  }
+}
+
+// EPI_F32: any operand majors; MN-major B comes with 64 / 128-wide tiles only (block_n % 64, at most 128)
+template <int BN, int TA, int TB>
+SVDX_DEVINL void tile_f32_bn(const TapGemmKParams& p, int kb0, int kb1, Ring& rg, int wg, EpiStage& st, const EpiTile& t, int sub, int lane,
+                             float s_acc) {
+  float acc[BN / 2];
+  tile_mainloop<BN, TA, TB, STAGES_REGS>(acc, kb0, kb1, rg, wg);
+  epilogue_f32<BN>(p, acc, st, t, sub, lane, s_acc);
+}
+
+template <int TA>
+SVDX_DEVINL void tile_f32(const TapGemmKParams& p, int kb0, int kb1, Ring& rg, int wg, EpiStage& st, const EpiTile& t, int sub, int lane,
+                          float s_acc) {
+  if (p.b_mn) {
+    if (p.block_n == 64) tile_f32_bn<64, TA, 1>(p, kb0, kb1, rg, wg, st, t, sub, lane, s_acc);
+    else tile_f32_bn<128, TA, 1>(p, kb0, kb1, rg, wg, st, t, sub, lane, s_acc);
+    return;
+  }
+  switch (p.block_n) {
+    case 32: tile_f32_bn<32, TA, 0>(p, kb0, kb1, rg, wg, st, t, sub, lane, s_acc); break;
+    case 64: tile_f32_bn<64, TA, 0>(p, kb0, kb1, rg, wg, st, t, sub, lane, s_acc); break;
+    case 96: tile_f32_bn<96, TA, 0>(p, kb0, kb1, rg, wg, st, t, sub, lane, s_acc); break;
+    case 128: tile_f32_bn<128, TA, 0>(p, kb0, kb1, rg, wg, st, t, sub, lane, s_acc); break;
+    default: tile_f32_bn<160, TA, 0>(p, kb0, kb1, rg, wg, st, t, sub, lane, s_acc); break;
   }
 }
 
@@ -426,7 +452,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_kernel(const __grid_co
         et.n0 = n0; et.n_out_total = n_out_total; et.row0 = st.row0; et.grp = st.grp; et.valid_rows = valid_rows; et.m0 = m0;
 #pragma unroll
         for (int h = 0; h < 2; ++h) tile_row(p, mt, q * 32 + half * 16 + (lane >> 2) + 8 * h, et.m[h], et.ok[h]);
-        tile_regs<EPI>(p, kb0, kb1, rg, wg, ps, et, lane, s_acc, s_r1, s_r2);
+        if constexpr (EPI == EPI_F32) {
+          if (p.a_mn) tile_f32<1>(p, kb0, kb1, rg, wg, st, et, half, lane, s_acc);
+          else tile_f32<0>(p, kb0, kb1, rg, wg, st, et, half, lane, s_acc);
+        } else {
+          tile_regs<EPI>(p, kb0, kb1, rg, wg, ps, et, lane, s_acc, s_r1, s_r2);
+        }
       }
     }
     if (lane == 0) bulk_wait<0>();   // staged stores must have left shared memory (and landed) before the CTA exits
@@ -637,6 +668,17 @@ int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p) {
     const bool has_res = d->res1 || d->res2 || d->scales;
     if (p.tma_store && !f32 && n_out % 32 == 0 && vec_ok && !d->a_major_mn && !(d->b_major_mn && has_res) && !p.probe && use != 2)
       p.epi_mode = d->geglu ? EPI_GEGLU : has_res ? EPI_RES : EPI_FAST;
+    // fp32 register epilogue: store or reduce-add, scaled by scales[0] at most, any operand majors, ragged N
+    const bool f32_plain = !d->bias && !d->rowbias && !d->res1 && !d->res2 && !d->geglu && !d->gn_sum && !d->gnb_sum && !d->interleave &&
+                           d->act == SVDX_ACT_NONE;
+    if (p.tma_store && f32 && f32_plain && !p.probe && use != 2) {
+      uint32_t box16[3] = {32, 16, 1};
+      uint64_t dims[3] = {(uint64_t)n_out, R, G};
+      uint64_t strides[2] = {(uint64_t)d->ldo * 4, (uint64_t)d->ldo * 4 * R};
+      rc = svdx_make_tmap_ex(&p.tmo16, d->out, 1, 128, 3, dims, strides, box16);
+      if (rc) return rc;
+      p.epi_mode = EPI_F32;
+    }
   }
   if (p.split_k > 1 && (p.bias || p.rowbias || p.res1 || p.res2 || p.geglu)) return svdx_fail(SVDX_E_BADARG, "tapgemm: split_k with epilogue operands");
   if (p.gnb_sum) {
@@ -681,7 +723,7 @@ int svdx_tapgemm_fill(const SvdxTapGemm* d, TapGemmKParams& p) {
     p.act = d->act;
     p.epi_mode = EPI_FAST_ACT;
   }
-  if (d->b_major_mn && p.epi_mode != EPI_GENERIC && (p.epi_mode != EPI_FAST || p.gn_sum))
+  if (d->b_major_mn && p.epi_mode != EPI_GENERIC && p.epi_mode != EPI_F32 && (p.epi_mode != EPI_FAST || p.gn_sum))
     return svdx_fail(SVDX_E_BADARG, "tapgemm: MN-major B takes the plain epilogue only (no gn_sum / gnb sums / act)");
   if (wide320 && p.epi_mode != EPI_FAST && p.epi_mode != EPI_RES && p.epi_mode != EPI_FAST_GNB && p.epi_mode != EPI_FAST_IL && p.epi_mode != EPI_FAST_ACT)
     return svdx_fail(SVDX_E_BADARG, "tapgemm: block_n 320 needs a bf16 output through the TMA-store epilogues (N % 320 == 0, aligned rows)");
@@ -731,13 +773,15 @@ extern "C" int svdx_tapgemm(const SvdxTapGemm* d, void* stream_v) {
     if (e == cudaSuccess) e = set_smem<EPI_FAST_IL>();
     if (e == cudaSuccess) e = set_smem<EPI_FAST_IL_GN>();
     if (e == cudaSuccess) e = set_smem<EPI_FAST_ACT>();
+    if (e == cudaSuccess) e = set_smem<EPI_F32>();
     if (e != cudaSuccess) return svdx_fail_cuda(e, "tapgemm: set smem attribute");
     attr_done[slot] = true;
   }
   const int total_tiles = p.m_tiles * p.n_tiles * p.split_k;
   int grid = svdx_num_sms();
   if (grid > total_tiles) grid = total_tiles;
-  if (p.epi_mode == EPI_FAST_ACT) launch<EPI_FAST_ACT>(grid, stream, p);
+  if (p.epi_mode == EPI_F32) launch<EPI_F32>(grid, stream, p);
+  else if (p.epi_mode == EPI_FAST_ACT) launch<EPI_FAST_ACT>(grid, stream, p);
   else if (p.epi_mode == EPI_FAST_IL && p.gn_sum) launch<EPI_FAST_IL_GN>(grid, stream, p);
   else if (p.epi_mode == EPI_FAST_IL) launch<EPI_FAST_IL>(grid, stream, p);
   else if (p.epi_mode == EPI_FAST_GNB) launch<EPI_FAST_GNB>(grid, stream, p);

@@ -62,6 +62,7 @@ struct __align__(64) TapGemmKParams {
   bf16* pre;
   long long ldpre;
   CUtensorMap tmo;     // output (bf16: 32x32 box, 64B swizzle; fp32: 32x32 box, 128B swizzle), dims {n_out, rows, groups}
+  CUtensorMap tmo16;   // EPI_F32: the fp32 output map of tmo with 16-row boxes (one per consumer warp)
   CUtensorMap tmpre;   // GEGLU pre-activation [M, N]
   float* gn_sum;       // fused GroupNorm statistics of the output (per slab m / gn_rows, per channel): [slab][2][gn_ld]
   long long gn_ld;
@@ -144,7 +145,7 @@ SVDX_DEVINL void conv_tile_boxes(const TapGemmKParams& p, int t, int lane, ConvB
 // Rows past the end of the group / matrix and columns past n_out are clipped by the tensor map.
 struct EpiStage {
   uint32_t base;   // this warp's 4 KB staging region (1024-aligned)
-  uint32_t off;    // bf16: alternates between the two 2 KB halves
+  uint32_t off;    // bf16 and EPI_F32: alternates between the two 2 KB halves
   int row0, grp;   // tensor-map coordinates of this warp's first row
 };
 
@@ -218,9 +219,10 @@ SVDX_DEVINL void gn_chunk_sums(const TapGemmKParams& p, uint32_t buf, int lane, 
 }
 
 // ---- specialised epilogues (kernel template parameter EPI): the hot shapes have short K, so the per-chunk instruction
-// count of the epilogue decides their speed. Every EPI but EPI_GENERIC assumes a bf16 output written through TMA, whole
-// 32-column chunks (n_out % 32 == 0), 16-byte aligned bias rows and a K-major A operand, and reads the accumulator straight
-// from the wgmma registers (epilogue_regs); everything else parks the tile and takes the generic epilogue_tile below.
+// count of the epilogue decides their speed. Every EPI but EPI_GENERIC and EPI_F32 assumes a bf16 output written through TMA,
+// whole 32-column chunks (n_out % 32 == 0), 16-byte aligned bias rows and a K-major A operand, and reads the accumulator straight
+// from the wgmma registers (epilogue_regs); EPI_F32 is the fp32 counterpart (epilogue_f32); everything else parks the tile
+// and takes the generic epilogue_tile below.
 constexpr int EPI_GENERIC = 0, EPI_FAST = 1, EPI_GEGLU = 2, EPI_RES = 3;
 // + fused GroupNorm statistics of the output (separate instantiations: the plain ones keep their register budget)
 constexpr int EPI_FAST_GN = 4, EPI_RES_GN = 5;
@@ -230,6 +232,9 @@ constexpr int EPI_FAST_GNB = 6;
 constexpr int EPI_FAST_IL = 7, EPI_FAST_IL_GN = 8;
 // plain epilogue + activation (act(acc + bias)): its own instantiation, so the others keep their register budget
 constexpr int EPI_FAST_ACT = 9;
+// fp32 output through TMA (store or reduce-add: weight gradients, split-K partials), optionally scaled by scales[0]; any
+// operand majors, ragged N; no bias / row-bias / residuals (epilogue_f32)
+constexpr int EPI_F32 = 10;
 
 // the activations of EPI_FAST_ACT: GELU (erf) and quick_gelu x * sigmoid(1.702 x)
 template <int N>
@@ -580,6 +585,47 @@ SVDX_DEVINL void epilogue_regs(const TapGemmKParams& p, const float (&acc)[BN / 
     if constexpr (GN) gn_chunk_sums(p, mine, lane, col0, t.n_out_total, mw, max(0, min(16, vr)));
     if constexpr (GNB) gnb_chunk_sums<16>(p, mine, mine + 2048u, lane, col0, t.n_out_total, mw, max(0, min(16, vr)));
     ++ps.round;
+  }
+}
+
+// EPI_F32: each consumer warp stages its own 16 rows x 32 columns of a chunk as fp32 (2 KB, the 128B swizzle of tmo) with
+// st.shared.v2 straight from the fragments, alternating between the two halves of its 4 KB region, and its lane 0 issues
+// the 16-row TMA store or reduce-add (tmo16). No pair barrier: the two warps of a quarter run their chunks independently.
+// Per element the arithmetic is the parked epilogue's: acc, times scales[0] when given.
+template <int BN>
+SVDX_DEVINL void epilogue_f32(const TapGemmKParams& p, const float (&acc)[BN / 2], EpiStage& st, const EpiTile& t, int sub, int lane,
+                              float s_acc) {
+  const bool reduce = p.out_dtype == SVDX_OUT_F32_ATOMIC;
+  // fragment register 4 j + 2 h + e: row lane / 4 + 8 h, columns 8 j + 2 (lane % 4) + e = 16-byte piece 2 j + (lane % 4) / 2,
+  // 8-byte half lane % 2; rows lane / 4 and lane / 4 + 8 swizzle alike (128B swizzle: piece ^= row % 8)
+  const uint32_t row_off = (uint32_t)(lane >> 2) * 128u + 8u * (lane & 1);
+  const int sw = lane >> 2, pc = (lane & 3) >> 1;
+#pragma unroll
+  for (int ch = 0; ch < BN / 32; ++ch) {
+    const int col0 = t.n0 + 32 * ch;
+    if (col0 >= t.n_out_total) break;                     // warp-uniform
+    if (lane == 0) bulk_wait_read<1>();                   // the half written two chunks ago has been read out
+    __syncwarp();
+    const uint32_t buf = st.base + st.off + row_off;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const uint32_t a = buf + ((uint32_t)((2 * j + pc) ^ sw) << 4);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float x = acc[16 * ch + 4 * j + 2 * h], y = acc[16 * ch + 4 * j + 2 * h + 1];
+        if (p.scales) { x *= s_acc; y *= s_acc; }
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a + h * 1024u), "f"(x), "f"(y) : "memory");
+      }
+    }
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+      const uint32_t src = st.base + st.off;
+      if (reduce) tma_reduce_add_3d(&p.tmo16, src, col0, t.row0 + 16 * sub, t.grp);
+      else tma_store_3d(&p.tmo16, src, col0, t.row0 + 16 * sub, t.grp);
+      bulk_commit();
+    }
+    st.off ^= 2048;
   }
 }
 

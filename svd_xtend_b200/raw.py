@@ -2,6 +2,7 @@
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import os
 from typing import Optional, Sequence
 
@@ -157,28 +158,41 @@ def _wide_tile_ok(M, N, k_total, out, ldo, geglu, a_mn, b_mn, b_mode, split_k, o
     return True
 
 
-_WGRAD_L2_BYTES_PER_CLK = 6500.0     # weight-gradient GEMMs are L2 -> SM bound
+# Weight-gradient GEMMs are bound by operand traffic from L2: per SM by the bytes a CTA keeps in flight through its 5-stage ring
+# (~34 B/clk), for the whole GPU by L2 -> SM bandwidth (~4,500 B/clk); plus ~4,000 clk per tile (ring ramp, fp32 reduce-add).
+# Fitted to every (width, split) of the config-2 weight gradients on an H100 80GB HBM3 (700 W, 1980 MHz).
+_WGRAD_SM_BYTES_PER_CLK = 34.0
+_WGRAD_L2_BYTES_PER_CLK = 4500.0
+_WGRAD_TILE_CLK = 4000.0
+_WGRAD_SPLITS = (1, 2, 3, 4, 5, 6, 8, 10, 12, 14, 16, 20, 24, 32)
 
 
 def wgrad_plan(O: int, K: int, M: int):
     """(block_n, split_k) of a weight-gradient GEMM dW[O, K] += dy[M, O]^T x[M, K] (MN-major operands, fp32 reduce-add
     epilogue). Tile width and the split of the token contraction are chosen TOGETHER by a small model: CTAs = tiles * split,
-    time = waves * (k-blocks per CTA * max(tensor pipe, L2 -> SM bytes of the CTAs running concurrently) + tile reduce-add)."""
-    sms = num_sms()
+    time = waves * (k-blocks per CTA * max(tensor pipe, a CTA's L2 -> SM bytes, L2 -> SM bytes of the CTAs running
+    concurrently) + per-tile cost). Splits stop at 4 waves of CTAs and 4 k-blocks per CTA."""
+    return _wgrad_plan(O, K, M, num_sms())
+
+
+@functools.lru_cache(maxsize=None)
+def _wgrad_plan(O: int, K: int, M: int, sms: int):
     kb = (M + 63) // 64
     m_tiles = (O + 127) // 128
     best = None
     for bn in ((128, 64) if K > 64 else (64,)):     # ties go to the earlier width; MN-major tiles are at most 128 wide
         n_tiles = (K + bn - 1) // bn
         tiles = m_tiles * n_tiles
-        splits = {1, max(1, min(kb // 32, sms // max(tiles, 1))), max(1, min(kb // 8, -(-sms // max(tiles, 1))))}
-        for split in sorted(splits):
+        for split in _WGRAD_SPLITS:
+            if split > 1 and (tiles * split > 4 * sms or kb // split < 4 or -(-kb // -(-kb // split)) != split):
+                continue                                   # the last condition: the library would drop empty splits
             ctas = tiles * split
             active = min(ctas, sms)
             bytes_kb = 16384 + 128.0 * K / n_tiles            # out-of-range B columns of the last tile are not fetched
-            per = max(4.0 * max(bn / 2.0, 32.0 + bn / 4.0), bytes_kb * active / _WGRAD_L2_BYTES_PER_CLK)
+            per = max(4.0 * max(bn / 2.0, 32.0 + bn / 4.0), bytes_kb / _WGRAD_SM_BYTES_PER_CLK,
+                      bytes_kb * active / _WGRAD_L2_BYTES_PER_CLK)
             waves = -(-ctas // sms)
-            cost = waves * ((kb / split) * per + bn * 8.0 + 3000.0)
+            cost = waves * ((kb / split) * per + _WGRAD_TILE_CLK)
             if best is None or cost < best[0] * 0.97:
                 best = (cost, bn, split)
     return best[1], best[2]
