@@ -3,7 +3,10 @@
      weights on each rank's clip, bit-identical across ranks;
  (2) sharded path (ShardedAdamW: reduce-scatter + AdamW on 1/N + bf16 all-gather): after one step every rank holds the same
      bf16 operand weights, equal to those of the all-reduce + replicated FusedAdamW step, and gather_masters() restores the
-     fp32 masters everywhere."""
+     fp32 masters everywhere;
+ (3) the same step as ONE kernel over NVLink peer memory (P2PShardedAdamW), eager and replayed from a CUDA graph;
+ (4) checkpoint and resume of ShardedAdamW: train at world N, state_dict() (collective), continue; a fresh optimizer that loads
+     the dict at world N continues bit for bit, and one at world N/2 (a subgroup) ends on masters within the tolerance of (2)."""
 import os
 import sys
 
@@ -27,7 +30,7 @@ dev = torch.device("cuda", local)
 dist.init_process_group("nccl", device_id=dev)
 
 
-def build():
+def build(pad_world=None):
     torch.manual_seed(0)
     unet = UNetSpatioTemporalConditionModel(**TINY).to(dev)
     unet.requires_grad_(False)
@@ -35,7 +38,7 @@ def build():
         if "temporal_transformer_block" in n:
             p.requires_grad_(True)
     unet.train()
-    arena = ParamArena(unet, pad_to=world * 64)
+    arena = ParamArena(unet, pad_to=(pad_world or world) * 64)
     unet.attach_arena(arena)
     return unet, arena
 
@@ -154,6 +157,58 @@ torch.cuda.synchronize()
 rep_equal = torch.equal(shadow_p2p3, arena.shadow) if world == 2 else ((shadow_p2p3.float() - arena.shadow.float()).abs().max().item() < 1e-2 * arena.shadow.float().abs().max().item())
 print(f"[ddp_check] rank {rank}: p2p fused step, 3 CUDA-graph replays vs 3 NCCL sharded steps: operands equal: {rep_equal}, t = {popt.t} / {opt.t}", flush=True)
 assert rep_equal and popt.t == 4 and opt.t == 4
+# ---- (4) checkpoint and resume of the sharded optimizer. Every rank feeds step t the gradient singles[rank] * (1 + t / 4), so
+# the mean gradient is the same at every world size; the weights are "saved" as the gathered masters.
+def train(o, a, ts, grad_of):
+    for t in ts:
+        o.lr = 1e-3 / (1 + 0.1 * t)
+        a.grad.copy_(grad_of(t)[:a.numel])
+        o.step()
+    torch.cuda.synchronize()
+
+
+own = lambda t: singles[rank] * (1.0 + 0.25 * t)
+unet4, arena4 = build()
+opt4 = ShardedAdamW(arena4, lr=1e-3, weight_decay=1e-2)
+train(opt4, arena4, range(3), own)
+sd = opt4.state_dict()                                                  # collective: the same full dict on every rank
+opt4.gather_masters()
+w3 = arena4.data.clone()
+train(opt4, arena4, range(3, 6), own)
+opt4.gather_masters()
+torch.cuda.synchronize()
+w6, m6 = arena4.data.clone(), opt4.m.clone()
+arena4.data.copy_(w3)
+arena4.refresh_shadow()
+opt5 = ShardedAdamW(arena4, lr=7.0, betas=(0.5, 0.5))                   # hyperparameters come from the dict
+opt5.load_state_dict(sd)
+train(opt5, arena4, range(3, 6), own)
+opt5.gather_masters()
+torch.cuda.synchronize()
+resumed_equal = torch.equal(arena4.data, w6) and torch.equal(opt5.m, m6) and opt5.t == 6
+print(f"[ddp_check] rank {rank}: checkpoint at world {world}: resumed run equals the uninterrupted one bit for bit: {resumed_equal}", flush=True)
+assert resumed_equal
+half = world // 2
+sub = dist.new_group(list(range(half))) if half else None
+if half and rank < half:
+    _, arena_h = build(pad_world=half)
+    arena_h.data.copy_(w3[:arena_h.numel])
+    arena_h.refresh_shadow()
+    opt_h = ShardedAdamW(arena_h, lr=7.0, group=sub)
+    assert opt_h.world == half
+    opt_h.load_state_dict(sd)
+    # sub-rank r stands for ranks r, r + half, ...: their gradients summed and scaled so that the mean over the half world is
+    # the mean over the full one
+    fold = lambda t: sum(singles[j] for j in range(rank, world, half)) * (half / world) * (1.0 + 0.25 * t)
+    train(opt_h, arena_h, range(3, 6), fold)
+    opt_h.gather_masters()
+    torch.cuda.synchronize()
+    e_half = ((arena_h.data - w6[:arena_h.numel]).norm() / (w6 - w3).norm()).item()
+    print(f"[ddp_check] rank {rank}: checkpoint of world {world} resumed at world {half}: masters vs the world-{world} continuation, "
+          f"rel-l2 of the update {e_half:.3e}, t = {opt_h.t}", flush=True)
+    assert e_half < 1e-3 and opt_h.t == 6
+elif not half:
+    print(f"[ddp_check] rank {rank}: world 1: no smaller world to resume at", flush=True)
 dist.barrier()
 torch.cuda.synchronize()
 sys.stdout.flush()

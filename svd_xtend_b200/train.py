@@ -10,6 +10,7 @@ clip per rank, §8e); the only exchange is one gradient all-reduce per step over
     unet.attach_arena(arena)            # kernels accumulate parameter gradients straight into arena.grad
     reducer = GradReducer(arena)        # bucketed ncclAllReduce on a side stream, overlapped with backward
     opt = FusedAdamW(arena, lr=...)     # one kernel over the flat buffers (torch.optim.AdamW semantics)
+    sd = opt.state_dict()               # checkpoints in torch.optim.AdamW's layout; opt.load_state_dict(sd) resumes exactly
 """
 from __future__ import annotations
 
@@ -155,6 +156,99 @@ class ParamArena:
             p.grad = self.grad_views[p]
 
 
+# ---- checkpoints of the fp32 optimizers in torch.optim.AdamW's state-dict layout --------------------------------------------
+# One group over arena.params (registration order filtered by requires_grad, the order train_svd.py:761-773 hands AdamW), and
+# state[i] = {"step": 0-dim fp32 tensor, "exp_avg", "exp_avg_sq": fp32 tensors of the parameter's shape} on the CPU. These two
+# functions are the only place that maps that layout to the flat moment buffers.
+_MOMENTS = ("exp_avg", "exp_avg_sq")
+
+
+def _adamw_group(lr, betas, eps, weight_decay) -> dict:
+    """torch.optim.AdamW's group entry (its keys follow the installed torch) without "params\""""
+    g = torch.optim.AdamW([torch.zeros(1)], lr=lr, betas=betas, eps=eps, weight_decay=weight_decay).state_dict()["param_groups"][0]
+    g.pop("params")
+    return g
+
+
+def adamw_state_dict(arena: ParamArena, step: int, hyper: dict, moments: Iterable[torch.Tensor]) -> dict:
+    """torch.optim.AdamW(arena.params, lr, betas, eps, weight_decay).state_dict() for flat arena-length moment buffers.
+
+    hyper: lr, betas, eps, weight_decay, plus keys of the optimizer's param_groups[0] that AdamW does not define (a scheduler's
+    `initial_lr`). moments: m, then v (any device); each is copied to the CPU, parameter by parameter, before the next one is
+    drawn, so a caller may yield the same temporary buffer twice."""
+    hp = {k: hyper[k] for k in ("lr", "betas", "eps", "weight_decay")}
+    group = _adamw_group(**hp)
+    group.update({k: v for k, v in hyper.items() if k not in group})
+    group["params"] = list(range(len(arena.params)))
+    state = {i: {"step": torch.tensor(float(step), dtype=F32)} for i in range(len(arena.params))}
+    for key, flat in zip(_MOMENTS, moments):
+        for i, (p, o) in enumerate(zip(arena.params, arena.offsets)):
+            state[i][key] = flat[o:o + p.numel()].view(p.shape).to("cpu", copy=True)
+    return {"state": state, "param_groups": [group]}
+
+
+def _indices(ix: List[int]) -> str:
+    return str(ix) if len(ix) <= 8 else f"{ix[:8]} and {len(ix) - 8} more"
+
+
+def _step_of(s) -> float:
+    return float(s.item() if isinstance(s, torch.Tensor) else s)
+
+
+@torch.no_grad()
+def load_adamw_state_dict(arena: ParamArena, sd: dict, m: torch.Tensor, v: torch.Tensor, lo: int = 0) -> dict:
+    """Check `sd` (torch.optim.AdamW's layout, as adamw_state_dict writes it) against the arena, then write the moments of the
+    arena range [lo, lo + m.numel()) into m / v; the arena padding is written as zero. Every check runs before anything is
+    written; a failure raises ValueError naming the parameter indices. Returns the group's hyperparameters and the step count
+    (one for all parameters: the fused kernels keep a single device counter)."""
+    who = "load_state_dict"
+    n = len(arena.params)
+    groups, state = sd.get("param_groups"), sd.get("state")
+    if not isinstance(groups, (list, tuple)) or len(groups) != 1 or not isinstance(state, dict):
+        raise ValueError(f"{who}: one parameter group expected, the dict has {len(groups) if isinstance(groups, (list, tuple)) else groups!r}")
+    g = groups[0]
+    ids = list(g.get("params", []))
+    if len(ids) != n:
+        raise ValueError(f"{who}: the group holds {len(ids)} parameters, the arena {n}")
+    absent = [k for k in ("lr", "betas", "eps", "weight_decay") if k not in g]
+    if absent:
+        raise ValueError(f"{who}: the group lacks {absent}")
+    for key, bad, what in (("amsgrad", True, "amsgrad"), ("maximize", True, "maximize"),
+                           ("decoupled_weight_decay", False, "coupled weight decay (torch.optim.Adam)")):
+        if key in g and bool(g[key]) == bad:
+            raise ValueError(f"{who}: the saved optimizer used {what}, which the fused AdamW kernels do not implement")
+    missing = [i for i, k in enumerate(ids) if not isinstance(state.get(k), dict) or any(x not in state[k] for x in ("step",) + _MOMENTS)]
+    if missing:
+        raise ValueError(f"{who}: no state for parameters {_indices(missing)} (they never had a gradient in the saved run); the "
+                         "fused form keeps one step count for all parameters and needs every one")
+    bad = [i for i, (p, k) in enumerate(zip(arena.params, ids))
+           if any(not isinstance(state[k][x], torch.Tensor) or not state[k][x].is_floating_point() or state[k][x].shape != p.shape
+                  for x in _MOMENTS)]
+    if bad:
+        raise ValueError(f"{who}: the moments of parameters {_indices(bad)} are not floating-point tensors of their parameter's shape")
+    by_step: Dict[float, List[int]] = {}
+    for i, k in enumerate(ids):
+        by_step.setdefault(_step_of(state[k]["step"]), []).append(i)
+    if len(by_step) > 1:
+        raise ValueError(f"{who}: parameters at different step counts ("
+                         + ", ".join(f"{s:g}: {_indices(ix)}" for s, ix in sorted(by_step.items())) + "); one device counter here")
+    (step,) = by_step
+    if step < 0 or step != int(step) or step > 2 ** 24:
+        raise ValueError(f"{who}: the step count {step:g} of parameters 0..{n - 1} is not an integer in [0, 2^24]")
+    hi = lo + m.numel()
+    m.zero_()
+    v.zero_()
+    for p, o, k in zip(arena.params, arena.offsets, ids):
+        a, b = max(o, lo), min(o + p.numel(), hi)
+        if a < b:
+            for dst, key in ((m, "exp_avg"), (v, "exp_avg_sq")):
+                dst[a - lo:b - lo].copy_(state[k][key].reshape(-1)[a - o:b - o])
+    b1, b2 = g["betas"]
+    known = _adamw_group(1e-3, (0.9, 0.999), 1e-8, 1e-2)
+    return {"lr": float(g["lr"]), "betas": (float(b1), float(b2)), "eps": float(g["eps"]), "weight_decay": float(g["weight_decay"]),
+            "step": step, "extra": {k: x for k, x in g.items() if k not in known and k != "params"}}
+
+
 class FusedAdamW:
     """torch.optim.AdamW semantics (train_svd.py:767-773) as ONE elementwise kernel over the arena (+ a 1-thread kernel
     that advances the step count). Every quantity that changes from step to step — learning rate, step, bias
@@ -231,6 +325,31 @@ class FusedAdamW:
         if self.arena.shadow is not None:
             ts.append(self.arena.shadow)
         return ts + self._ema_tensors()
+
+    # ---- checkpoints in torch.optim.AdamW's layout (adamw_state_dict): torch.optim.AdamW, ShardedAdamW and P2PShardedAdamW
+    # at any world size load them, and they load here. The masters are the model's weights (save_pretrained / state_dict).
+    def _hyper(self) -> dict:
+        extra = {k: x for k, x in self.param_groups[0].items() if k not in ("lr", "params")}
+        return dict(extra, lr=self._lr, betas=tuple(self.betas), eps=self.eps, weight_decay=self.weight_decay)
+
+    def _set_hyper(self, h: dict):
+        self.betas, self.eps, self.weight_decay = h["betas"], h["eps"], h["weight_decay"]
+        self._lr = h["lr"]
+        self.param_groups[0].update(h["extra"])
+        self.param_groups[0]["lr"] = self._lr
+        # the tick recomputes 1 - beta^t from the step with the device's powf before the next update: bit for bit what an
+        # uninterrupted run has
+        self.state.copy_(torch.tensor([self._lr, *self.betas, self.eps, self.weight_decay, h["step"], 1.0, 1.0], dtype=F32))
+
+    def state_dict(self) -> dict:
+        """torch.optim.AdamW's state dict of this optimizer, moments on the CPU (one synchronisation for the step count)"""
+        return adamw_state_dict(self.arena, self.t, self._hyper(), (self.m, self.v))
+
+    @torch.no_grad()
+    def load_state_dict(self, sd: dict) -> None:
+        """load a state dict of torch.optim.AdamW over the same parameters, of this class or of a sharded one saved at any world
+        size, into the existing buffers (a GraphedStep captured before stays valid); ValueError before any write if it does not fit"""
+        self._set_hyper(load_adamw_state_dict(self.arena, sd, self.m, self.v))
 
 
 class FusedAdamW8bit:
@@ -416,6 +535,7 @@ class ShardedAdamW:
             raise ValueError(f"ShardedAdamW: build the arena with ParamArena(..., pad_to={self.world * 64}) (equal, aligned shards)")
         n = arena.numel // self.world
         self.lo, self.hi = self.rank * n, (self.rank + 1) * n
+        self.betas, self.weight_decay, self.eps = betas, weight_decay, eps
         dev = arena.data.device
         self.m = torch.zeros(n, device=dev, dtype=F32)
         self.v = torch.zeros(n, device=dev, dtype=F32)
@@ -431,6 +551,29 @@ class ShardedAdamW:
     t = FusedAdamW.t
     _ema_args = FusedAdamW._ema_args
     _ema_tensors = FusedAdamW._ema_tensors
+    _hyper = FusedAdamW._hyper
+    _set_hyper = FusedAdamW._set_hyper
+
+    def state_dict(self) -> dict:
+        """COLLECTIVE: every rank calls it and gets the same full torch.optim.AdamW state dict (rank 0 saves it). m, then v, is
+        all-gathered into one temporary arena-length fp32 buffer and copied to the CPU before the next gather, so the peak
+        extra device memory is one arena (1.6 GB for the as-scripted temporal set, 6.1 GB for the whole UNet). Call
+        gather_masters() too before saving the weights."""
+        return adamw_state_dict(self.arena, self.t, self._hyper(), self._gathered_moments())
+
+    def _gathered_moments(self):
+        tmp = torch.empty_like(self.arena.data)
+        for mine in (self.m, self.v):
+            tmp[self.lo:self.hi].copy_(mine)
+            self.all_gather_(tmp)
+            yield tmp
+
+    @torch.no_grad()
+    def load_state_dict(self, sd: dict) -> None:
+        """local, no collective: this rank copies its [lo, hi) slice of the per-parameter moments. A dict saved at any world
+        size, or by FusedAdamW / torch.optim.AdamW over the same parameters, loads at any other. On resume every rank also loads
+        the full weights and calls arena.refresh_shadow()."""
+        self._set_hyper(load_adamw_state_dict(self.arena, sd, self.m, self.v, self.lo))
 
     def attach_ema(self, ema):
         """FusedAdamW.attach_ema for the sharded update: the EMA buffer has the arena's full length and each rank advances its
