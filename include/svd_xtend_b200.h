@@ -362,10 +362,8 @@ int svdx_outer_accum(const void* dy, int64_t lddy, const void* x, int64_t ldx, i
  *   out[12..15] = {a, 0, 1-a, 0}        {s, 0} pairs for svdx_axpby_bf16 (gradients of the residual operands) */
 int svdx_blend_scales(const float* mix_factor, float* out16, void* stream);
 /* fused multi-tensor AdamW on a flat fp32 buffer (torch.optim.AdamW of train_svd.py:767-773); when shadow_bf16 is given
- * the updated parameters are also written as bf16 at the same flat offsets (the forward GEMM operands) */
-int svdx_adamw(float* p, const float* g, float* m, float* v, int64_t n, float lr, float beta1, float beta2,
-               float eps, float weight_decay, int32_t step, float grad_scale, void* shadow_bf16, void* stream);
-/* the same update with every step-varying scalar in DEVICE memory, so that it can be captured in a CUDA graph and replayed:
+ * the updated parameters are also written as bf16 at the same flat offsets (the forward GEMM operands). Every
+ * step-varying scalar is in DEVICE memory, so that the update can be captured in a CUDA graph and replayed:
  * state = float[8] {lr, beta1, beta2, eps, weight_decay, step, 1-beta1^step, 1-beta2^step}. The call first advances
  * step and the bias corrections on the device (a 1-thread kernel), then updates; the host changes the learning rate by
  * writing state[0] (lr scheduler of train_svd.py:790-796). Two launches. */

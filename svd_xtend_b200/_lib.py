@@ -111,8 +111,6 @@ _PROTOS = {
     "svdx_gemv": [c_void_p, c_i64, c_void_p, c_i64, c_int, c_int, c_int, c_void_p, c_void_p, c_i64, c_int, c_float, c_int, c_void_p],
     "svdx_outer_accum": [c_void_p, c_i64, c_void_p, c_i64, c_int, c_int, c_int, c_void_p, c_void_p, c_i64, c_void_p],
     "svdx_blend_scales": [c_void_p, c_void_p, c_void_p],
-    "svdx_adamw": [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_float, c_float, c_float, c_float, c_float,
-                   c_int, c_float, c_void_p, c_void_p],
     "svdx_adamw_graph": [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_float, c_void_p, c_void_p],
     "svdx_adamw_p2p": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_i64, c_i64, c_void_p, c_float, c_int, c_void_p],
     "svdx_adamw_graph_ema": [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p],

@@ -492,23 +492,7 @@ __global__ void blend_scales_kernel(const float* mix, float* out) {
   out[12] = a; out[13] = 0.f; out[14] = 1.f - a; out[15] = 0.f;      // {s, 0} pairs for svdx_axpby_bf16 (scaled copies)
 }
 
-__global__ void adamw_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, long long n,
-                             float lr, float b1, float b2, float eps, float wd, float bc1, float bc2, float gscale, bf16* __restrict__ shadow) {
-  const long long i = gtid();
-  if (i >= n) return;
-  const float gi = g[i] * gscale;
-  float pi = p[i] * (1.f - lr * wd);
-  const float mi = b1 * m[i] + (1.f - b1) * gi;
-  const float vi = b2 * v[i] + (1.f - b2) * gi * gi;
-  m[i] = mi;
-  v[i] = vi;
-  const float denom = sqrtf(vi) / sqrtf(bc2) + eps;
-  pi -= (lr / bc1) * mi / denom;
-  p[i] = pi;
-  if (shadow) shadow[i] = __float2bfloat16(pi);   // bf16 operand copy of the updated weight, same flat offset
-}
-
-// CUDA-graph-safe form: every scalar that changes between steps lives in a small device buffer
+// AdamW is CUDA-graph-safe: every scalar that changes between steps lives in a small device buffer
 //   state[0] lr  [1] beta1  [2] beta2  [3] eps  [4] weight_decay  [5] step (float, exact up to 2^24)  [6] 1-beta1^step  [7] 1-beta2^step
 // adamw_tick advances the step count and the bias corrections on the device, so a captured graph that contains
 // tick + update replays torch.optim.AdamW's step sequence; the learning rate is whatever the host last wrote to state[0].
@@ -546,47 +530,61 @@ __global__ void adamw_ema_tick_kernel(float* state, double* ema_state) {
 // torch's `s.sub_(omd * (s - p))`
 SVDX_DEVINL float ema_update(float e, float p, float omd) { return __fsub_rn(e, __fmul_rn(omd, __fsub_rn(e, p))); }
 
+// e <- ema_update(e, p[k]) over four adjacent elements
+SVDX_DEVINL float4 ema_update4(float4 e, const float* p, float omd) {
+  return make_float4(ema_update(e.x, p[0], omd), ema_update(e.y, p[1], omd), ema_update(e.z, p[2], omd), ema_update(e.w, p[3], omd));
+}
+
+// The fp32 update (torch.optim.AdamW), stated once: adamw_state_kernel's vector body and scalar tail and adamw_p2p_kernel
+// must agree bit for bit (ShardedAdamW and P2PShardedAdamW produce the same weights, at any length), so all three call
+// adamw_update. Of the two products in b * m + (1 - b) * g the compiler contracts one into the FMA, and which one follows
+// the form of the operands it is handed: every caller passes p, m, v as local scalars, which keeps fma(b, m, (1 - b) * g).
+struct AdamCoef {     // per launch, from state[8]
+  float b1, b2, eps, decay, step_size, inv_sqrt_bc2;
+};
+SVDX_DEVINL AdamCoef adamw_coef(const float* __restrict__ state) {
+  const float lr = state[0], b1 = state[1], b2 = state[2], eps = state[3], wd = state[4], bc1 = state[6], bc2 = state[7];
+  return {b1, b2, eps, 1.f - lr * wd, lr / bc1, rsqrtf(bc2)};
+}
+SVDX_DEVINL void adamw_update(const AdamCoef& c, float g, float& p, float& m, float& v) {
+  m = c.b1 * m + (1.f - c.b1) * g;
+  v = c.b2 * v + (1.f - c.b2) * g * g;
+  p = p * c.decay - c.step_size * m / (sqrtf(v) * c.inv_sqrt_bc2 + c.eps);
+}
+// four adjacent elements at 16-byte aligned p / m / v, updated in place from the gradient g4 * gscale; pp receives the new masters
+SVDX_DEVINL void adamw_update4(const AdamCoef& c, float4 g4, float gscale, float* p, float* m, float* v, float (&pp)[4]) {
+  const float4 p4 = *reinterpret_cast<float4*>(p), m4 = *reinterpret_cast<float4*>(m), v4 = *reinterpret_cast<float4*>(v);
+  float mm[4] = {m4.x, m4.y, m4.z, m4.w}, vv[4] = {v4.x, v4.y, v4.z, v4.w};
+  const float gg[4] = {g4.x * gscale, g4.y * gscale, g4.z * gscale, g4.w * gscale};
+  pp[0] = p4.x; pp[1] = p4.y; pp[2] = p4.z; pp[3] = p4.w;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    float pi = pp[k], mi = mm[k], vi = vv[k];
+    adamw_update(c, gg[k], pi, mi, vi);
+    pp[k] = pi; mm[k] = mi; vv[k] = vi;
+  }
+  *reinterpret_cast<float4*>(p) = make_float4(pp[0], pp[1], pp[2], pp[3]);
+  *reinterpret_cast<float4*>(m) = make_float4(mm[0], mm[1], mm[2], mm[3]);
+  *reinterpret_cast<float4*>(v) = make_float4(vv[0], vv[1], vv[2], vv[3]);
+}
+
 template <bool EMA>
 __global__ void adamw_state_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, long long n4,
                                    long long n, const float* __restrict__ state, float gscale, bf16* __restrict__ shadow,
                                    float* __restrict__ ema, const double* __restrict__ ema_state) {
   const long long i4 = gtid();
   if (i4 >= n4) return;
-  const float lr = state[0], b1 = state[1], b2 = state[2], eps = state[3], wd = state[4], bc1 = state[6], bc2 = state[7];
-  const float decay = 1.f - lr * wd, step_size = lr / bc1, inv_sqrt_bc2 = rsqrtf(bc2);
+  const AdamCoef c = adamw_coef(state);
   const long long i = i4 * 4;
   if (i + 3 < n) {
-    const float4 g4 = *reinterpret_cast<const float4*>(g + i);
-    float4 p4 = *reinterpret_cast<float4*>(p + i), m4 = *reinterpret_cast<float4*>(m + i), v4 = *reinterpret_cast<float4*>(v + i);
-    float pp[4] = {p4.x, p4.y, p4.z, p4.w}, mm[4] = {m4.x, m4.y, m4.z, m4.w}, vv[4] = {v4.x, v4.y, v4.z, v4.w};
-    const float gg[4] = {g4.x * gscale, g4.y * gscale, g4.z * gscale, g4.w * gscale};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      mm[k] = b1 * mm[k] + (1.f - b1) * gg[k];
-      vv[k] = b2 * vv[k] + (1.f - b2) * gg[k] * gg[k];
-      pp[k] = pp[k] * decay - step_size * mm[k] / (sqrtf(vv[k]) * inv_sqrt_bc2 + eps);
-    }
-    *reinterpret_cast<float4*>(p + i) = make_float4(pp[0], pp[1], pp[2], pp[3]);
-    *reinterpret_cast<float4*>(m + i) = make_float4(mm[0], mm[1], mm[2], mm[3]);
-    *reinterpret_cast<float4*>(v + i) = make_float4(vv[0], vv[1], vv[2], vv[3]);
-    if (shadow) {
-      uint2 o;
-      o.x = pack_bf16x2(pp[0], pp[1]);
-      o.y = pack_bf16x2(pp[2], pp[3]);
-      *reinterpret_cast<uint2*>(shadow + i) = o;
-    }
-    if constexpr (EMA) {
-      const float omd = (float)ema_state[8];
-      float4 e4 = *reinterpret_cast<float4*>(ema + i);
-      e4.x = ema_update(e4.x, pp[0], omd); e4.y = ema_update(e4.y, pp[1], omd);
-      e4.z = ema_update(e4.z, pp[2], omd); e4.w = ema_update(e4.w, pp[3], omd);
-      *reinterpret_cast<float4*>(ema + i) = e4;
-    }
+    float pp[4];
+    adamw_update4(c, *reinterpret_cast<const float4*>(g + i), gscale, p + i, m + i, v + i, pp);
+    if (shadow) *reinterpret_cast<uint2*>(shadow + i) = make_uint2(pack_bf16x2(pp[0], pp[1]), pack_bf16x2(pp[2], pp[3]));
+    if constexpr (EMA) *reinterpret_cast<float4*>(ema + i) = ema_update4(*reinterpret_cast<float4*>(ema + i), pp, (float)ema_state[8]);
   } else {
     for (long long k = i; k < n; ++k) {
-      const float gi = g[k] * gscale;
-      const float mi = b1 * m[k] + (1.f - b1) * gi, vi = b2 * v[k] + (1.f - b2) * gi * gi;
-      const float pi = p[k] * decay - step_size * mi / (sqrtf(vi) * inv_sqrt_bc2 + eps);
+      float pi = p[k], mi = m[k], vi = v[k];
+      adamw_update(c, g[k] * gscale, pi, mi, vi);
       m[k] = mi; v[k] = vi; p[k] = pi;
       if (shadow) shadow[k] = __float2bfloat16(pi);
       if constexpr (EMA) ema[k] = ema_update(ema[k], pi, (float)ema_state[8]);
@@ -610,8 +608,7 @@ template <bool EMA>
 __global__ void __launch_bounds__(256) adamw_p2p_kernel(float* __restrict__ p, float* __restrict__ m, float* __restrict__ v, const __grid_constant__ AdamP2P ptr,
                                                         int world, long long lo, long long n4, const float* __restrict__ state, float gscale,
                                                         float* __restrict__ ema, const double* __restrict__ ema_state) {
-  const float lr = state[0], b1 = state[1], b2 = state[2], eps = state[3], wd = state[4], bc1 = state[6], bc2 = state[7];
-  const float decay = 1.f - lr * wd, step_size = lr / bc1, inv_sqrt_bc2 = rsqrtf(bc2);
+  const AdamCoef c = adamw_coef(state);
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long i4 = gtid(); i4 < n4; i4 += stride) {
     const long long i = i4 * 4;
@@ -627,29 +624,12 @@ __global__ void __launch_bounds__(256) adamw_p2p_kernel(float* __restrict__ p, f
       for (int k = 0; k < 4; ++k)
         if (r0 + k < world) { g4.x += t[k].x; g4.y += t[k].y; g4.z += t[k].z; g4.w += t[k].w; }
     }
-    float4 p4 = *reinterpret_cast<float4*>(p + i), m4 = *reinterpret_cast<float4*>(m + i), v4 = *reinterpret_cast<float4*>(v + i);
-    float pp[4] = {p4.x, p4.y, p4.z, p4.w}, mm[4] = {m4.x, m4.y, m4.z, m4.w}, vv[4] = {v4.x, v4.y, v4.z, v4.w};
-    const float gg[4] = {g4.x * gscale, g4.y * gscale, g4.z * gscale, g4.w * gscale};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      mm[k] = b1 * mm[k] + (1.f - b1) * gg[k];
-      vv[k] = b2 * vv[k] + (1.f - b2) * gg[k] * gg[k];
-      pp[k] = pp[k] * decay - step_size * mm[k] / (sqrtf(vv[k]) * inv_sqrt_bc2 + eps);
-    }
-    *reinterpret_cast<float4*>(p + i) = make_float4(pp[0], pp[1], pp[2], pp[3]);
-    *reinterpret_cast<float4*>(m + i) = make_float4(mm[0], mm[1], mm[2], mm[3]);
-    *reinterpret_cast<float4*>(v + i) = make_float4(vv[0], vv[1], vv[2], vv[3]);
-    uint2 o;
-    o.x = pack_bf16x2(pp[0], pp[1]);
-    o.y = pack_bf16x2(pp[2], pp[3]);
+    float pp[4];
+    adamw_update4(c, g4, gscale, p + i, m + i, v + i, pp);
+    const uint2 o = make_uint2(pack_bf16x2(pp[0], pp[1]), pack_bf16x2(pp[2], pp[3]));
     for (int r = 0; r < world; ++r) *reinterpret_cast<uint2*>(ptr.shadow[r] + lo + i) = o;
-    if constexpr (EMA) {     // this rank's slice of the EMA only: no peer traffic
-      const float omd = (float)ema_state[8];
-      float4 e4 = *reinterpret_cast<float4*>(ema + i);
-      e4.x = ema_update(e4.x, pp[0], omd); e4.y = ema_update(e4.y, pp[1], omd);
-      e4.z = ema_update(e4.z, pp[2], omd); e4.w = ema_update(e4.w, pp[3], omd);
-      *reinterpret_cast<float4*>(ema + i) = e4;
-    }
+    if constexpr (EMA)     // this rank's slice of the EMA only: no peer traffic
+      *reinterpret_cast<float4*>(ema + i) = ema_update4(*reinterpret_cast<float4*>(ema + i), pp, (float)ema_state[8]);
   }
   __threadfence_system();     // the peer stores are performed system-wide before this kernel counts as complete
 }
@@ -679,11 +659,8 @@ __global__ void __launch_bounds__(256) multi_ema_kernel(const EmaJob* __restrict
 #pragma unroll
     for (int k = 0; k < EMA_CHUNK / 1024; ++k) {
       const long long i = c0 + (k * 256 + threadIdx.x) * 4;
-      float4 e4 = *reinterpret_cast<float4*>(j.shadow + i);
       const float4 p4 = __ldg(reinterpret_cast<const float4*>(j.param + i));
-      e4.x = ema_update(e4.x, p4.x, omd); e4.y = ema_update(e4.y, p4.y, omd);
-      e4.z = ema_update(e4.z, p4.z, omd); e4.w = ema_update(e4.w, p4.w, omd);
-      *reinterpret_cast<float4*>(j.shadow + i) = e4;
+      *reinterpret_cast<float4*>(j.shadow + i) = ema_update4(*reinterpret_cast<float4*>(j.shadow + i), &p4.x, omd);
     }
   } else {
     for (long long i = c0 + threadIdx.x; i < c1; i += 256) j.shadow[i] = ema_update(j.shadow[i], j.param[i], omd);
@@ -845,13 +822,9 @@ __global__ void __launch_bounds__(256) adamw8bit_kernel(const Adam8Job* __restri
         *reinterpret_cast<uint4*>(j.shadow + base) = make_uint4(pack_bf16x2(pp[0], pp[1]), pack_bf16x2(pp[2], pp[3]),
                                                                 pack_bf16x2(pp[4], pp[5]), pack_bf16x2(pp[6], pp[7]));
       if constexpr (EMA) {
-        float4 e0 = *reinterpret_cast<float4*>(j.ema + base), e1 = *reinterpret_cast<float4*>(j.ema + base + 4);
-        e0.x = ema_update(e0.x, pp[0], omd); e0.y = ema_update(e0.y, pp[1], omd);
-        e0.z = ema_update(e0.z, pp[2], omd); e0.w = ema_update(e0.w, pp[3], omd);
-        e1.x = ema_update(e1.x, pp[4], omd); e1.y = ema_update(e1.y, pp[5], omd);
-        e1.z = ema_update(e1.z, pp[6], omd); e1.w = ema_update(e1.w, pp[7], omd);
-        *reinterpret_cast<float4*>(j.ema + base) = e0;
-        *reinterpret_cast<float4*>(j.ema + base + 4) = e1;
+        const float4 e0 = *reinterpret_cast<float4*>(j.ema + base), e1 = *reinterpret_cast<float4*>(j.ema + base + 4);
+        *reinterpret_cast<float4*>(j.ema + base) = ema_update4(e0, pp, omd);
+        *reinterpret_cast<float4*>(j.ema + base + 4) = ema_update4(e1, pp + 4, omd);
       }
     } else {
 #pragma unroll
@@ -1382,16 +1355,6 @@ extern "C" int svdx_blend_scales(const float* mix_factor, float* out3, void* str
   if (!mix_factor || !out3) return svdx_fail(SVDX_E_BADARG, "blend_scales: null");
   blend_scales_kernel<<<1, 1, 0, ST(stream)>>>(mix_factor, out3);
   SVDX_CHECK_LAUNCH("blend_scales");
-  return SVDX_OK;
-}
-
-extern "C" int svdx_adamw(float* p, const float* g, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps,
-                          float weight_decay, int32_t step, float grad_scale, void* shadow_bf16, void* stream) {
-  if (!p || !g || !m || !v || n <= 0 || step < 1) return svdx_fail(SVDX_E_BADARG, "adamw: bad arguments");
-  const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
-  adamw_kernel<<<nblocks(n), 256, 0, ST(stream)>>>(p, g, m, v, n, lr, beta1, beta2, eps, weight_decay, bc1, bc2, grad_scale,
-                                                   reinterpret_cast<bf16*>(shadow_bf16));
-  SVDX_CHECK_LAUNCH("adamw");
   return SVDX_OK;
 }
 

@@ -733,13 +733,6 @@ def blend_scales(mix_factor, out3):  # out3: float[8]
     return out3
 
 
-def adamw(p, g, m, v, lr, beta1, beta2, eps, weight_decay, step, grad_scale=1.0, shadow=None):
-    if _fam("adamw", 0.0, (30.0 if shadow is not None else 28.0) * p.numel()):
-        return
-    check(load().svdx_adamw(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(), lr, beta1, beta2, eps, weight_decay,
-                            step, grad_scale, _ptr(shadow), _stream()), "adamw")
-
-
 def _ema_args(ema, ema_state, n):
     if (ema is None) != (ema_state is None):
         raise ValueError("ema and ema_state go together")

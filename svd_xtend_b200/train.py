@@ -88,21 +88,9 @@ class ParamArena:
         if self.shadow is not None:
             raw.cast_f32_bf16(self.data, self.shadow)
 
-    def shadow_matrix(self, params: List[torch.nn.Parameter]) -> Optional[torch.Tensor]:
-        """bf16 [sum O_i, I] view of adjacent 2-D parameters (or of one), None if they are not contiguous in the arena"""
-        if self.shadow is None or any(p not in self.offset_of for p in params):
-            return None
-        I = params[0][0].numel()
-        o0 = self.offset_of[params[0]]
-        o = o0
-        for p in params:
-            if self.offset_of[p] != o or p[0].numel() != I:
-                return None
-            o += p.numel()
-        return self.shadow[o0:o].view(-1, I)
-
-    def grad_matrix(self, params: List[torch.nn.Parameter]) -> Optional[torch.Tensor]:
-        """fp32 [sum O_i, I] view of the gradient arena over adjacent 2-D parameters, None if they are not contiguous"""
+    def _span(self, params: List[torch.nn.Parameter]) -> Optional[tuple]:
+        """(o0, o1, I): the arena range of adjacent 2-D parameters (or of one) that share the row length I, None if they are
+        not all in the arena or not contiguous in it"""
         if any(p not in self.offset_of for p in params):
             return None
         I = params[0][0].numel()
@@ -112,7 +100,17 @@ class ParamArena:
             if self.offset_of[p] != o or p[0].numel() != I:
                 return None
             o += p.numel()
-        return self.grad[o0:o].view(-1, I)
+        return o0, o, I
+
+    def shadow_matrix(self, params: List[torch.nn.Parameter]) -> Optional[torch.Tensor]:
+        """bf16 [sum O_i, I] view of adjacent 2-D parameters (or of one), None if they are not contiguous in the arena"""
+        span = None if self.shadow is None else self._span(params)
+        return None if span is None else self.shadow[span[0]:span[1]].view(-1, span[2])
+
+    def grad_matrix(self, params: List[torch.nn.Parameter]) -> Optional[torch.Tensor]:
+        """fp32 [sum O_i, I] view of the gradient arena over adjacent 2-D parameters, None if they are not contiguous"""
+        span = self._span(params)
+        return None if span is None else self.grad[span[0]:span[1]].view(-1, span[2])
 
     def transposed_matrix(self, params: List[torch.nn.Parameter]) -> Optional[torch.Tensor]:
         """bf16 [I, sum O_i] transposed operand, refreshed for ALL registered matrices by one svdx_multi_transpose launch"""
@@ -249,18 +247,19 @@ def load_adamw_state_dict(arena: ParamArena, sd: dict, m: torch.Tensor, v: torch
             "step": step, "extra": {k: x for k, x in g.items() if k not in known and k != "params"}}
 
 
-class FusedAdamW:
-    """torch.optim.AdamW semantics (train_svd.py:767-773) as ONE elementwise kernel over the arena (+ a 1-thread kernel
-    that advances the step count). Every quantity that changes from step to step — learning rate, step, bias
-    corrections — lives in the device buffer `state` (float[8]: lr, beta1, beta2, eps, weight_decay, step, 1-b1^t,
+class _ArenaAdamW:
+    """What the fused AdamW forms share: the hyperparameters, and every quantity that changes from step to step — learning
+    rate, step, bias corrections — in the device buffer `state` (float[8]: lr, beta1, beta2, eps, weight_decay, step, 1-b1^t,
     1-b2^t), so a CUDA graph that captured `step()` replays the CORRECT sequence of updates; an lr scheduler writes
-    `opt.lr = value` (a 4-byte H2D copy outside the graph) between replays."""
+    `opt.lr = value` (a 4-byte H2D copy outside the graph) between replays. A subclass allocates its moment buffers, names them
+    in `_moment_buffers` and provides step(), state_dict() and load_state_dict()."""
 
-    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8):
+    _moment_buffers: tuple = ()          # attribute names of the moment buffers, in snapshot_tensors' order
+    _ema_sharded = False          # an attached EMA is advanced slice by slice over the ranks
+
+    def __init__(self, arena: ParamArena, lr, betas, weight_decay, eps):
         self.arena = arena
         self.betas, self.weight_decay, self.eps = betas, weight_decay, eps
-        self.m = torch.zeros_like(arena.data)
-        self.v = torch.zeros_like(arena.data)
         self._lr = float(lr)
         self.state = torch.tensor([float(lr), betas[0], betas[1], eps, weight_decay, 0.0, 1.0, 1.0], device=arena.data.device, dtype=F32)
         self._lr_host = torch.empty(1, dtype=F32).pin_memory() if arena.data.is_cuda else torch.empty(1, dtype=F32)
@@ -276,8 +275,10 @@ class FusedAdamW:
         every step(): its shadows of the arena's parameters are re-homed into one flat fp32 buffer at the arena offsets and
         updated by the AdamW kernel from the new masters (8 more bytes per parameter, no extra launch), so a captured
         GraphedStep replays the EMA with the right decay sequence. The EMA's copies of frozen parameters are dropped: their
-        EMA is the parameter. From then on `ema.step()` raises."""
-        ema._attach(self, sharded=False)
+        EMA is the parameter. From then on `ema.step()` raises. Under the sharded forms the buffer keeps the arena's full
+        length and each rank advances its [lo, hi) slice: call `gather_ema()` before copy_to / state_dict / save_pretrained
+        (they raise on an EMA advanced since the last gather)."""
+        ema._attach(self, sharded=self._ema_sharded)
         self.ema = ema
 
     def _ema_args(self, lo=None, hi=None):
@@ -310,9 +311,7 @@ class FusedAdamW:
         """number of updates applied so far (reads the device counter: synchronises)"""
         return int(self.state[5].item())
 
-    def step(self, grad_scale: float = 1.0):
-        a = self.arena
-        raw.adamw_graph(a.data, a.grad, self.m, self.v, self.state, grad_scale, shadow=a.shadow, **self._ema_args())
+    def _updated(self):
         if self.on_updated is not None:
             self.on_updated()
 
@@ -321,18 +320,17 @@ class FusedAdamW:
 
     def snapshot_tensors(self) -> List[torch.Tensor]:
         """everything a warm-up step mutates (for GraphedStep(restore=...)), the attached EMA included"""
-        ts = [self.arena.data, self.m, self.v, self.state]
+        ts = [self.arena.data, *(getattr(self, name) for name in self._moment_buffers), self.state]
         if self.arena.shadow is not None:
             ts.append(self.arena.shadow)
         return ts + self._ema_tensors()
 
-    # ---- checkpoints in torch.optim.AdamW's layout (adamw_state_dict): torch.optim.AdamW, ShardedAdamW and P2PShardedAdamW
-    # at any world size load them, and they load here. The masters are the model's weights (save_pretrained / state_dict).
     def _hyper(self) -> dict:
         extra = {k: x for k, x in self.param_groups[0].items() if k not in ("lr", "params")}
         return dict(extra, lr=self._lr, betas=tuple(self.betas), eps=self.eps, weight_decay=self.weight_decay)
 
     def _set_hyper(self, h: dict):
+        """hyperparameters and step count of a loaded checkpoint: lr, betas, eps, weight_decay, step, extra (further group keys)"""
         self.betas, self.eps, self.weight_decay = h["betas"], h["eps"], h["weight_decay"]
         self._lr = h["lr"]
         self.param_groups[0].update(h["extra"])
@@ -341,6 +339,25 @@ class FusedAdamW:
         # uninterrupted run has
         self.state.copy_(torch.tensor([self._lr, *self.betas, self.eps, self.weight_decay, h["step"], 1.0, 1.0], dtype=F32))
 
+
+class FusedAdamW(_ArenaAdamW):
+    """torch.optim.AdamW semantics (train_svd.py:767-773) as ONE elementwise kernel over the arena (+ a 1-thread kernel
+    that advances the step count)."""
+
+    _moment_buffers = ("m", "v")
+
+    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8):
+        super().__init__(arena, lr, betas, weight_decay, eps)
+        self.m = torch.zeros_like(arena.data)
+        self.v = torch.zeros_like(arena.data)
+
+    def step(self, grad_scale: float = 1.0):
+        a = self.arena
+        raw.adamw_graph(a.data, a.grad, self.m, self.v, self.state, grad_scale, shadow=a.shadow, **self._ema_args())
+        self._updated()
+
+    # ---- checkpoints in torch.optim.AdamW's layout (adamw_state_dict): torch.optim.AdamW, ShardedAdamW and P2PShardedAdamW
+    # at any world size load them, and they load here. The masters are the model's weights (save_pretrained / state_dict).
     def state_dict(self) -> dict:
         """torch.optim.AdamW's state dict of this optimizer, moments on the CPU (one synchronisation for the step count)"""
         return adamw_state_dict(self.arena, self.t, self._hyper(), (self.m, self.v))
@@ -352,7 +369,7 @@ class FusedAdamW:
         self._set_hyper(load_adamw_state_dict(self.arena, sd, self.m, self.v))
 
 
-class FusedAdamW8bit:
+class FusedAdamW8bit(_ArenaAdamW):
     """FusedAdamW with block-wise 8-bit moments (bitsandbytes' AdamW8bit, train_svd.py --use_8bit_adam; the update is stated in
     oracle/svd_adam8bit_oracle.py): a parameter with at least `min_8bit_size` elements keeps m / v as uint8 codes plus one fp32
     absmax per 256-element block counted from its own arena offset (arena padding belongs to no block); a smaller one keeps
@@ -360,10 +377,12 @@ class FusedAdamW8bit:
     FusedAdamW, so a captured GraphedStep replays the right sequence. About 2.03 bytes of state per parameter instead of 8.
     The update is deterministic, so under GradReducer every rank's replica stays identical."""
 
+    _moment_buffers = ("codes1", "codes2", "absmax1", "absmax2", "m32", "v32")
+
     def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, min_8bit_size: int = 4096):
         from .optim8bit import dynamic_map, num_blocks
-        self.arena = arena
-        self.betas, self.weight_decay, self.eps, self.min_8bit_size = betas, weight_decay, eps, int(min_8bit_size)
+        super().__init__(arena, lr, betas, weight_decay, eps)
+        self.min_8bit_size = int(min_8bit_size)
         dev = arena.data.device
         self.qmap1, self.qmap2 = dynamic_map(True).to(dev), dynamic_map(False).to(dev)
         # per parameter: (param, arena offset, quant, state offset (codes / fp32 elements), absmax offset)
@@ -384,25 +403,12 @@ class FusedAdamW8bit:
         self.absmax2 = torch.zeros(blocks, dtype=F32, device=dev)
         self.m32 = torch.zeros(f32, dtype=F32, device=dev)
         self.v32 = torch.zeros(f32, dtype=F32, device=dev)
-        self._lr = float(lr)
-        self.state = torch.tensor([float(lr), betas[0], betas[1], eps, weight_decay, 0.0, 1.0, 1.0], device=dev, dtype=F32)
-        self._lr_host = torch.empty(1, dtype=F32).pin_memory() if arena.data.is_cuda else torch.empty(1, dtype=F32)
-        self.on_updated = None
-        self.param_groups = [{"lr": float(lr), "params": arena.params}]
-        self.ema = None
         self._table = None
         self._index = {p: i for i, (p, *_r) in enumerate(self.layout)}
 
-    lr = FusedAdamW.lr
-    sync_lr = FusedAdamW.sync_lr
-    t = FusedAdamW.t
-    _ema_tensors = FusedAdamW._ema_tensors
-
     def attach_ema(self, ema):
-        """FusedAdamW.attach_ema for the 8-bit update: the EMA of the new masters is advanced in the same launch"""
-        ema._attach(self, sharded=False)
-        self.ema = ema
-        self._table = None
+        super().attach_ema(ema)
+        self._table = None          # the job table carries the EMA's addresses
 
     def state_views(self, p: torch.nn.Parameter) -> Dict[str, torch.Tensor]:
         """this parameter's optimizer state as views into the flat buffers (bitsandbytes' keys, without step)"""
@@ -443,21 +449,11 @@ class FusedAdamW8bit:
         tb = self._table
         raw.adamw8bit(tb.dev, tb.prefix, tb.njobs, tb.blocks, self.qmap1, self.qmap2, self.state, grad_scale,
                       ema_state=None if self.ema is None else self.ema._state, nbytes=self._nbytes)
-        if self.on_updated is not None:
-            self.on_updated()
-
-    def zero_grad(self, set_to_none: bool = False):
-        self.arena.zero_grad()
-
-    def snapshot_tensors(self) -> List[torch.Tensor]:
-        ts = [self.arena.data, self.codes1, self.codes2, self.absmax1, self.absmax2, self.m32, self.v32, self.state]
-        if self.arena.shadow is not None:
-            ts.append(self.arena.shadow)
-        return ts + self._ema_tensors()
+        self._updated()
 
     # ---- checkpoints in bitsandbytes' per-parameter layout (svd_xtend_b200.optim8bit.AdamW8bit loads them too) ----
     def state_dict(self) -> dict:
-        step = int(self.state[5].item())
+        step = self.t
         st = {}
         for i, (p, *_r) in enumerate(self.layout):
             d = {k: (v if k.startswith("qmap") else v.clone()) for k, v in self.state_views(p).items()}
@@ -506,14 +502,11 @@ class FusedAdamW8bit:
         if len(steps) > 1:
             raise ValueError("FusedAdamW8bit.load_state_dict: parameters at different step counts (one device counter here)")
         b1, b2 = g.get("betas", self.betas)
-        self.betas, self.eps, self.weight_decay = (b1, b2), g.get("eps", self.eps), g.get("weight_decay", self.weight_decay)
-        step = steps.pop() if steps else 0
-        self.state.copy_(torch.tensor([float(g.get("lr", self._lr)), b1, b2, self.eps, self.weight_decay, float(step), 1.0, 1.0], dtype=F32))
-        self._lr = float(g.get("lr", self._lr))
-        self.param_groups[0]["lr"] = self._lr
+        self._set_hyper({"lr": float(g.get("lr", self._lr)), "betas": (b1, b2), "eps": g.get("eps", self.eps),
+                         "weight_decay": g.get("weight_decay", self.weight_decay), "step": float(steps.pop() if steps else 0), "extra": {}})
 
 
-class ShardedAdamW:
+class ShardedAdamW(_ArenaAdamW):
     """Data-parallel update with the optimizer state SHARDED over the ranks (ZeRO-1 on the flat arenas), all in NCCL
     collectives that capture into the step's CUDA graph:
 
@@ -527,32 +520,20 @@ class ShardedAdamW:
     checkpoint or reading `p.data` of arbitrary parameters. Semantics of the update itself = torch.optim.AdamW on the MEAN
     gradient, as DistributedDataParallel + AdamW would give (train_svd.py:767-773, :815-824)."""
 
+    _moment_buffers = ("m", "v")
+    _ema_sharded = True
+
     def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, group=None):
-        self.arena, self.group = arena, group
+        super().__init__(arena, lr, betas, weight_decay, eps)
+        self.group = group
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
         if arena.numel % (self.world * 64):
             raise ValueError(f"ShardedAdamW: build the arena with ParamArena(..., pad_to={self.world * 64}) (equal, aligned shards)")
         n = arena.numel // self.world
         self.lo, self.hi = self.rank * n, (self.rank + 1) * n
-        self.betas, self.weight_decay, self.eps = betas, weight_decay, eps
-        dev = arena.data.device
-        self.m = torch.zeros(n, device=dev, dtype=F32)
-        self.v = torch.zeros(n, device=dev, dtype=F32)
-        self._lr = float(lr)
-        self.state = torch.tensor([float(lr), betas[0], betas[1], eps, weight_decay, 0.0, 1.0, 1.0], device=dev, dtype=F32)
-        self._lr_host = torch.empty(1, dtype=F32).pin_memory() if arena.data.is_cuda else torch.empty(1, dtype=F32)
-        self.on_updated = None
-        self.param_groups = [{"lr": float(lr), "params": arena.params}]
-        self.ema = None
-
-    lr = FusedAdamW.lr
-    sync_lr = FusedAdamW.sync_lr
-    t = FusedAdamW.t
-    _ema_args = FusedAdamW._ema_args
-    _ema_tensors = FusedAdamW._ema_tensors
-    _hyper = FusedAdamW._hyper
-    _set_hyper = FusedAdamW._set_hyper
+        self.m = torch.zeros(n, device=arena.data.device, dtype=F32)
+        self.v = torch.zeros(n, device=arena.data.device, dtype=F32)
 
     def state_dict(self) -> dict:
         """COLLECTIVE: every rank calls it and gets the same full torch.optim.AdamW state dict (rank 0 saves it). m, then v, is
@@ -574,13 +555,6 @@ class ShardedAdamW:
         size, or by FusedAdamW / torch.optim.AdamW over the same parameters, loads at any other. On resume every rank also loads
         the full weights and calls arena.refresh_shadow()."""
         self._set_hyper(load_adamw_state_dict(self.arena, sd, self.m, self.v, self.lo))
-
-    def attach_ema(self, ema):
-        """FusedAdamW.attach_ema for the sharded update: the EMA buffer has the arena's full length and each rank advances its
-        [lo, hi) slice. Call `gather_ema()` before copy_to / state_dict / save_pretrained (they raise on an EMA advanced
-        since the last gather)."""
-        ema._attach(self, sharded=True)
-        self.ema = ema
 
     def gather_ema(self):
         """make every slice of the attached EMA current on this rank (in-place all-gather, like gather_masters)"""
@@ -620,21 +594,11 @@ class ShardedAdamW:
             self.all_gather_(a.shadow)
         else:
             self.all_gather_(a.data)
-        if self.on_updated is not None:
-            self.on_updated()
+        self._updated()
 
     def gather_masters(self):
         """make the fp32 masters of ALL slices current on this rank (before save_pretrained / state_dict)"""
         self.all_gather_(self.arena.data)
-
-    def zero_grad(self, set_to_none: bool = False):
-        self.arena.zero_grad()
-
-    def snapshot_tensors(self) -> List[torch.Tensor]:
-        ts = [self.arena.data, self.m, self.v, self.state]
-        if self.arena.shadow is not None:
-            ts.append(self.arena.shadow)
-        return ts + self._ema_tensors()
 
 
 def map_peer_buffers(t: torch.Tensor, group=None) -> List[int]:
@@ -706,8 +670,7 @@ class P2PShardedAdamW(ShardedAdamW):
                       **self._ema_args(self.lo, self.hi))
         if self.world > 1:
             self._fence()                                   # every shadow is complete, nobody still reads this rank's gradients
-        if self.on_updated is not None:
-            self.on_updated()
+        self._updated()
 
 
 class GradReducer:

@@ -288,19 +288,28 @@ def test_misc_elementwise(raw):
     raw.axpby(x, x, y, s3)
     torch.cuda.synchronize()
     _close(y, x.float() * (s3[0] + s3[1]), tol=1e-2, what="axpby")
-    # AdamW vs torch
-    p = _rand(1000, seed=24)
-    g = _rand(1000, seed=25)
+    # AdamW vs torch, at a length whose last elements take the kernel's scalar tail
+    p0 = _rand(1003, seed=24)
+    g = _rand(1003, seed=25)
+    p = p0.clone()
     pt = p.clone().requires_grad_(True)
     opt = torch.optim.AdamW([pt], lr=1e-2, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2)
     m = torch.zeros_like(p)
     v = torch.zeros_like(p)
+    state = torch.tensor([1e-2, 0.9, 0.999, 1e-8, 1e-2, 0.0, 1.0, 1.0], device=DEV)
     for step in (1, 2, 3):
         pt.grad = g.clone()
         opt.step()
-        raw.adamw(p, g, m, v, 1e-2, 0.9, 0.999, 1e-8, 1e-2, step)
+        raw.adamw_graph(p, g, m, v, state)
     torch.cuda.synchronize()
     assert torch.allclose(p, pt.detach(), atol=1e-5, rtol=1e-5)
+    # the tail's bits are the vector body's: the same three elements updated as part of a 4-element buffer
+    p4, g4 = torch.cat([p0[1000:], p0[:1]]), torch.cat([g[1000:], g[:1]])
+    m4, v4, state4 = torch.zeros_like(p4), torch.zeros_like(p4), torch.tensor([1e-2, 0.9, 0.999, 1e-8, 1e-2, 0.0, 1.0, 1.0], device=DEV)
+    for _ in range(3):
+        raw.adamw_graph(p4, g4, m4, v4, state4)
+    torch.cuda.synchronize()
+    assert torch.equal(p4[:3], p[1000:]) and torch.equal(m4[:3], m[1000:]) and torch.equal(v4[:3], v[1000:])
 
 
 def test_multi_transpose_bit_exact(raw):
