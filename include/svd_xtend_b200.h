@@ -420,6 +420,25 @@ int svdx_adamw8bit(const void* jobs, const int32_t* block_prefix, int32_t njobs,
 int svdx_adamw8bit_ema(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
                        const float* qmap2, float* state, float grad_scale, double* ema_state, void* stream);
 
+/* Batch assembly of a training step from video frames (train_svd.py:942-1017; svd_xtend_b200.video_train). Every operation is
+ * rounded separately (no FMA), in the reference's order.
+ * svdx_vae_frames_in: the VAE encoder's input rows, bf16 [(B*F + B) * H*W][c_pad] (token-major, channels >= 3 zero), as
+ * svdx_nchw_to_nhwc writes them: rows of frame n < B*F are the clip frames x[b][f] (n = b*F + f); rows of frame B*F + b are the
+ * noise-augmented conditioning frame fl(fl(eps[b] * sigma_c[b]) + x[b][0]) (:957-958). x: [B][F][3][H][W] of dtype code
+ * x_dtype (0 fp32, 1 bf16); eps: fp32 [B][3][H][W]; sigma_c: DEVICE fp32 [B]. One launch. */
+int svdx_vae_frames_in(const void* x, int32_t x_dtype, const float* cond_eps, const float* cond_sigma, int32_t B, int32_t F,
+                       int32_t H, int32_t W, int32_t c_pad, void* dst, void* stream);
+/* svdx_edm_prepare: from the fp32 moments [B*(F+1)][2C][h][w] of that encode (mean, then logvar), per latent element
+ *   z = mean + exp(0.5 * clamp(logvar, -30, 20)) * eps,  latent = z * sf,  noisy = latent + noise * sigma[b]
+ * (:948, :287, :951, :967) and the conditioning latents c = (z_c * sf) * (1 / sf) of frame B*F + b (:959-960: torch's division of
+ * a CUDA tensor by a scalar multiplies by the fp32 reciprocal), writes (all fp32)
+ *   sample  [B][F][2C][h][w]: channels < C noisy / sqrt(sigma^2 + 1) (:972), channels >= C image_mask[b] * c (:1008-1017);
+ *   noisy   [B][F][C][h][w];  latents [B][F][C][h][w] (the target).
+ * latent_eps, noise: fp32 [B*F][C][h][w]; cond_latent_eps: fp32 [B][C][h][w]; sigma, image_mask: DEVICE fp32 [B]. One launch. */
+int svdx_edm_prepare(const float* moments, const float* latent_eps, const float* noise, const float* cond_latent_eps,
+                     const float* sigma, const float* image_mask, float scaling_factor, int32_t B, int32_t F, int32_t C,
+                     int32_t h, int32_t w, float* sample, float* noisy, float* latents, void* stream);
+
 /* many bf16 transposes dst[i][o] = src_base[src_off + o*I + i] in one launch (dgrad operands of all trainable linears).
  * jobs: device array of {int64 src_off; void* dst; int32 O; int32 I}; tile_prefix[j] = first 32x32 tile of job j. */
 int svdx_multi_transpose(const void* src_base, const void* jobs, const int32_t* tile_prefix, int32_t njobs, int32_t total_tiles,

@@ -1,0 +1,140 @@
+#!/usr/bin/env python
+"""Training step from video frames (svd_xtend_b200.video_train.VideoTrainStep) on the H100 path, one JSON line.
+
+    python scripts/bench_video_train.py --config 2|4 [--steps K] [--warmup W]
+
+Seeded default-init SVD UNet (the config's trainable set and gradient checkpointing), VAE encoder and CLIP ViT-H image encoder,
+FusedAdamW, B = 1, conditioning dropout 0.1. Three forms of the step, timed in alternating windows of K steps, medians of 3:
+  * graphed: VideoTrainStep (frames -> VAE encode -> CLIP -> batch assembly -> UNet -> loss -> backward -> AdamW, one graph),
+    frames from a device buffer, draws made eagerly each step;
+  * eager: the same VideoTrainStep with cuda_graph=False;
+  * latent_only: the latent-input graphed step bench.py times (workload.synthetic_batch, no VAE / CLIP).
+Reports ms per step and frames/s of each, max_memory_allocated after all three are built, the card's name and power limit, and
+the SM clock sampled during the timed windows. A form that does not fit on the card is reported as failed. Writes nothing to
+the source tree.
+"""
+import argparse
+import json
+import os
+import statistics
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+import torch  # noqa: E402
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--config", type=int, choices=(2, 4), default=2)
+    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=2)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise RuntimeError("bench_video_train.py needs a CUDA device: the step has no CPU fallback")
+
+    from bench import ClockSampler
+    from oracle.svd_clip_oracle import CLIP_CONFIG          # the SVD checkpoint's image_encoder/ and vae/ configurations
+    from oracle.svd_vae_oracle import VAE_CONFIG
+    from scripts.bench_decode import power_limit_w
+    from svd_xtend_b200.clip import CLIPVisionModelWithProjection
+    from svd_xtend_b200.train import FusedAdamW, GraphedStep, ParamArena
+    from svd_xtend_b200.unet import UNetSpatioTemporalConditionModel
+    from svd_xtend_b200.vae import AutoencoderKLTemporalDecoder
+    from svd_xtend_b200.video_train import VideoTrainStep
+    from svd_xtend_b200.workload import BENCH_CONFIGS, SVD_CONFIG, edm_loss, synthetic_batch
+
+    dev = torch.device("cuda", 0)
+    cfg = BENCH_CONFIGS[args.config]
+    F, H, W = cfg["frames"], 8 * cfg["h"], 8 * cfg["w"]
+    steps, warmup = max(args.steps, 1), max(args.warmup, 1)
+    torch.manual_seed(1234)
+    with torch.device(dev):
+        unet = UNetSpatioTemporalConditionModel(**SVD_CONFIG)
+        vae = AutoencoderKLTemporalDecoder(**VAE_CONFIG)
+        clip = CLIPVisionModelWithProjection(**CLIP_CONFIG)
+    for m in (unet, vae, clip):
+        m.to(dev).requires_grad_(False)
+    vae.eval()
+    clip.eval()
+    for n, p in unet.named_parameters():
+        if "temporal_transformer_block" in n:          # train_svd.py:761-766
+            p.requires_grad_(True)
+    unet.train()
+    if cfg["grad_ckpt"]:
+        unet.enable_gradient_checkpointing()
+    arena = ParamArena(unet)
+    unet.attach_arena(arena)
+    opt = FusedAdamW(arena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8)
+    opt.on_updated = lambda: unet.refresh_trainable_operands(shadow_current=True)
+    g = torch.Generator(device="cpu").manual_seed(5)
+    frames = (torch.rand(1, F, 3, H, W, generator=g) * 2 - 1).to(dev)
+
+    forms, failed = {}, {}
+    kw = dict(frames_shape=(1, F, H, W), conditioning_dropout_prob=0.1, generator=torch.Generator(dev).manual_seed(0))
+    try:
+        graphed = VideoTrainStep(unet, vae, clip, opt, **kw)
+        forms["graphed"] = lambda: graphed(frames)
+    except torch.OutOfMemoryError as e:
+        failed["graphed"] = f"OutOfMemoryError: {str(e).splitlines()[0]}"
+        torch.cuda.empty_cache()
+    b = {k: v.to(dev) for k, v in synthetic_batch(1, F, cfg["h"], cfg["w"], seed=1234).items()}
+
+    def latent_step(bb):
+        arena.zero_grad()
+        pred = unet(bb["sample"], bb["timestep"], bb["encoder_hidden_states"], added_time_ids=bb["added_time_ids"]).sample
+        loss = edm_loss(pred.float(), bb["noisy"], bb["latents"], bb["sigmas"])
+        loss.backward()
+        opt.step()
+        return loss
+    try:
+        latent = GraphedStep(latent_step, b, warmup=3, restore=opt.snapshot_tensors(),
+                             on_restored=lambda: unet.refresh_trainable_operands(shadow_current=True))
+        forms["latent_only"] = latent.replay
+    except torch.OutOfMemoryError as e:
+        failed["latent_only"] = f"OutOfMemoryError: {str(e).splitlines()[0]}"
+        torch.cuda.empty_cache()
+    eager = VideoTrainStep(unet, vae, clip, opt, cuda_graph=False, **kw)
+    forms["eager"] = lambda: eager(frames)
+    try:
+        for fn in forms.values():
+            for _ in range(warmup):
+                fn()
+        torch.cuda.synchronize()
+    except torch.OutOfMemoryError as e:
+        failed["eager"] = f"OutOfMemoryError: {str(e).splitlines()[0]}"
+        forms.pop("eager")
+        torch.cuda.empty_cache()
+    mem = torch.cuda.max_memory_allocated()
+
+    clocks = ClockSampler(0)
+    c0 = clocks.count()
+    times = {k: [] for k in forms}
+    loss = None
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    for _ in range(3):
+        for k, fn in forms.items():
+            torch.cuda.synchronize()
+            e0.record()
+            for _ in range(steps):
+                loss = fn()
+            e1.record()
+            torch.cuda.synchronize()
+            times[k].append(e0.elapsed_time(e1) / steps)
+    c1 = clocks.count()
+    clk = clocks.stop(c0, c1)
+    res = {}
+    for k, ts in times.items():
+        ms = statistics.median(ts)
+        res[k] = {"ms_per_step": round(ms, 3), "frames_per_s": round(F * 1e3 / ms, 2), "windows_ms": [round(t, 3) for t in ts]}
+    res.update({k: {"failed": v} for k, v in failed.items()})
+    print(json.dumps({"metric": "video_train_step", "config": args.config, "frames": F, "pixels": [H, W], "batch": 1,
+                      "steps_per_window": steps, "forms": res, "final_loss": None if loss is None else float(loss.float().item()),
+                      "max_memory_allocated_gib": round(mem / 2 ** 30, 2), "device": torch.cuda.get_device_name(dev),
+                      "power_limit_w": power_limit_w(0), "sm_clock": clk}))
+
+
+if __name__ == "__main__":
+    main()

@@ -121,6 +121,9 @@ _PROTOS = {
     "svdx_adamw8bit_ema": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p],
     "svdx_multi_transpose": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p],
     "svdx_lora_merge": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p],
+    "svdx_vae_frames_in": [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
+    "svdx_edm_prepare": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int, c_int, c_int, c_int,
+                         c_void_p, c_void_p, c_void_p, c_void_p],
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOS) + ("svdx_last_error",)

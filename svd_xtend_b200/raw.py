@@ -585,6 +585,41 @@ def nchw_to_nhwc(src, dst, N, Cc, H, W, c_pad):
     return dst
 
 
+def vae_frames_in(x, cond_eps, cond_sigma, dst, c_pad=64):
+    """the VAE encoder's bf16 input rows [(B*F + B) * H*W, c_pad] of the clip frames x [B, F, 3, H, W] (fp32 / bf16), followed by
+    the B noise-augmented conditioning frames fl(fl(cond_eps[b] * cond_sigma[b]) + x[b, 0]); cond_eps fp32 [B, 3, H, W],
+    cond_sigma fp32 [B] on the device"""
+    B, F, Cc, H, W = x.shape
+    if Cc != 3 or not x.is_contiguous() or x.dtype not in (torch.float32, bf16):
+        raise ValueError("vae_frames_in: x must be a contiguous fp32 / bf16 [B, F, 3, H, W] tensor")
+    if cond_eps.dtype != torch.float32 or not cond_eps.is_contiguous() or cond_eps.numel() != B * 3 * H * W:
+        raise ValueError("vae_frames_in: cond_eps must be a contiguous fp32 tensor of B*3*H*W elements")
+    if cond_sigma.dtype != torch.float32 or cond_sigma.numel() != B:
+        raise ValueError("vae_frames_in: cond_sigma must be fp32 [B]")
+    if dst.dtype != bf16 or not dst.is_contiguous() or dst.shape != (B * (F + 1) * H * W, c_pad):
+        raise ValueError(f"vae_frames_in: dst must be a contiguous bf16 [{B * (F + 1) * H * W}, {c_pad}] tensor")
+    check(load().svdx_vae_frames_in(x.data_ptr(), dtype_code(x, "frames"), cond_eps.data_ptr(), cond_sigma.data_ptr(), B, F, H, W,
+                                    c_pad, dst.data_ptr(), _stream()), "vae_frames_in")
+    return dst
+
+
+def edm_prepare(moments, latent_eps, noise, cond_latent_eps, sigma, image_mask, scaling_factor, sample, noisy, latents):
+    """posterior samples, EDM noising and the UNet input from the moments [B*(F+1), 2C, h, w] of one encode of the clip and
+    conditioning frames (svd_xtend_b200.h, svdx_edm_prepare): sample [B, F, 2C, h, w], noisy / latents [B, F, C, h, w], all fp32"""
+    B, F, C2, h, w = sample.shape
+    C = C2 // 2
+    shapes = ((moments, (B * (F + 1), C2, h, w)), (latent_eps, (B * F * C * h * w,)), (noise, (B * F * C * h * w,)),
+              (cond_latent_eps, (B * C * h * w,)), (sigma, (B,)), (image_mask, (B,)), (noisy, (B, F, C, h, w)),
+              (latents, (B, F, C, h, w)), (sample, (B, F, C2, h, w)))
+    for t, shape in shapes:
+        if t.dtype != torch.float32 or not t.is_contiguous() or (t.shape if len(shape) > 1 else (t.numel(),)) != shape:
+            raise ValueError(f"edm_prepare: expected a contiguous fp32 tensor of shape {shape}, got {tuple(t.shape)} {t.dtype}")
+    check(load().svdx_edm_prepare(moments.data_ptr(), latent_eps.data_ptr(), noise.data_ptr(), cond_latent_eps.data_ptr(), sigma.data_ptr(),
+                                  image_mask.data_ptr(), float(scaling_factor), B, F, C, h, w, sample.data_ptr(), noisy.data_ptr(),
+                                  latents.data_ptr(), _stream()), "edm_prepare")
+    return sample, noisy, latents
+
+
 def nhwc_to_nchw(src, dst, N, Cc, H, W):
     check(load().svdx_nhwc_to_nchw(src.data_ptr(), _rowmajor(src, "src"), dst.data_ptr(), dtype_code(dst, "NCHW output"), N, Cc, H, W, _stream()),
           "nhwc_to_nchw")

@@ -295,16 +295,24 @@ class AutoencoderKLTemporalDecoder(nn.Module):
         return _mid_attention(E, a, x, g)
 
     def _run(self, x: torch.Tensor) -> torch.Tensor:
+        N, Cin, H, W = x.shape
+        x0 = torch.empty(N * H * W, self.ROW_PAD, device=x.device, dtype=bf16)
+        xin = x.contiguous()
+        raw.nchw_to_nhwc(xin if xin.dtype in (F32, bf16, torch.float16) else xin.float(), x0, N, Cin, H, W, self.ROW_PAD)
+        out = self._run_rows(x0, N, H, W)
+        return out.to(x.dtype) if x.dtype in (bf16, torch.float16) else out
+
+    ROW_PAD = 64          # columns of the encoder's input rows (conv_in's channels zero padded to one 64-wide k-block)
+
+    def _run_rows(self, x0: torch.Tensor, N: int, H: int, W: int) -> torch.Tensor:
+        """the encoder on its bf16 input rows x0 [N*H*W, ROW_PAD] (token-major, as svdx_nchw_to_nhwc writes them) -> the fp32
+        NCHW moments [N, 2*latent_channels, H/f, W/f]"""
         E = self._engine
         enc = self.encoder
-        N, Cin, H, W = x.shape
-        dev = x.device
+        dev = x0.device
         E.begin(recording=False)
         g = Geom(N, 1, H, W)
-        cpad = 64
-        x0 = torch.empty(N * H * W, cpad, device=dev, dtype=bf16)
-        xin = x.contiguous()
-        raw.nchw_to_nhwc(xin if xin.dtype in (F32, bf16, torch.float16) else xin.float(), x0, N, Cin, H, W, cpad)
+        cpad = self.ROW_PAD
         h = E.conv2d_3x3(Var(x0), g, enc.conv_in, i_pad=cpad, gn_rows=g.HW)
         for blk in enc.down_blocks:
             for r in blk.resnets:
@@ -325,7 +333,7 @@ class AutoencoderKLTemporalDecoder(nn.Module):
         m = E.linear(y, self.quant_conv.weight, self.quant_conv.bias)
         out = torch.empty(N, C2, g.H, g.W, device=dev, dtype=F32)
         raw.nhwc_to_nchw(m.data, out, N, C2, g.H, g.W)
-        return out.to(x.dtype) if x.dtype in (bf16, torch.float16) else out
+        return out
 
     # ------------------------------------------------------------------ the decode path
     def decode(self, z: torch.Tensor, num_frames: int, return_dict: bool = True):

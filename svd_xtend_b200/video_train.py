@@ -1,0 +1,216 @@
+"""A training step from video frames on H100: the body of train_svd.py's training loop (:942-1036) from the clip's pixels to the
+optimizer update, with the package's frozen VAE encoder and CLIP image encoder in front of the UNet.
+
+    step = VideoTrainStep(unet, vae, image_encoder, opt, frames_shape=(1, 14, 320, 512), conditioning_dropout_prob=0.1,
+                          generator=torch.Generator("cuda").manual_seed(0))
+    loss = step(pixel_values)           # [B, F, 3, H, W] in [-1, 1], fp32 or bf16; the 0-dim device loss
+
+Per step: the random draws (`draw_train_noise`) happen eagerly, outside any graph; then `assemble_train_batch` builds the
+UNet batch (the dict `workload.synthetic_batch` returns) and the step runs forward, `workload.edm_loss`, backward and the
+optimizer, all inside one captured `train.GraphedStep`. The batch assembly is two kernels of csrc/edm.cu around one VAE encode:
+`svdx_vae_frames_in` writes the encoder's input rows of the B*F clip frames and the B noise-augmented conditioning frames (one
+encode of B*(F+1) frames replaces the reference's two: the encoder works frame by frame), and `svdx_edm_prepare` turns the
+moments into the posterior samples, the noisy latents, the target and the UNet input. The per-clip scalars (log-normal sigmas,
+timesteps, time ids, dropout masks) are O(B) torch ops. oracle/svd_train_batch_oracle.py states the same in torch.
+"""
+from __future__ import annotations
+
+from typing import Dict, Optional
+
+import torch
+
+from . import raw
+from .clip import CLIP_MEAN, CLIP_STD, encode_image
+from .workload import edm_loss
+
+F32 = torch.float32
+
+# (name, kind) in the reference's draw order: posterior sample of the clip (:948 -> :287), the EDM noise (:951), the uniform of
+# the conditioning sigma (:954 -> :66), the conditioning-frame noise (:957-958), the posterior sample of the conditioning frame
+# (:959), the uniform of the EDM sigma (:964) and the conditioning-dropout uniform (:993, only when dropout is on)
+DRAWS = (("latent_eps", "randn"), ("noise", "randn"), ("cond_u", "rand"), ("cond_pixel_eps", "randn"), ("cond_latent_eps", "randn"),
+         ("sigma_u", "rand"), ("dropout_u", "rand"))
+
+
+def draw_shapes(B: int, F: int, H: int, W: int, conditioning_dropout: bool = True) -> Dict[str, tuple]:
+    """name -> shape of every draw of one step, in draw order (h = H / 8, w = W / 8)"""
+    h, w = H // 8, W // 8
+    shapes = dict(latent_eps=(B * F, 4, h, w), noise=(B, F, 4, h, w), cond_u=(B,), cond_pixel_eps=(B, 3, H, W),
+                  cond_latent_eps=(B, 4, h, w), sigma_u=(B,), dropout_u=(B,))
+    if not conditioning_dropout:
+        del shapes["dropout_u"]
+    return shapes
+
+
+def draw_train_noise(B: int, F: int, H: int, W: int, generator: Optional[torch.Generator] = None, device="cuda",
+                     conditioning_dropout: bool = True) -> Dict[str, torch.Tensor]:
+    """The random draws of one training step from frames [B, F, 3, H, W], as named fp32 tensors on `device`, drawn in this
+    order (h = H / 8, w = W / 8):
+
+        1 latent_eps       [B*F, 4, h, w]   randn   posterior sample of the clip frames
+        2 noise            [B, F, 4, h, w]  randn   EDM noise
+        3 cond_u           [B]              rand    uniform of the conditioning sigma, LogNormal(-3, 0.5)
+        4 cond_pixel_eps   [B, 3, H, W]     randn   noise augmentation of the conditioning frame
+        5 cond_latent_eps  [B, 4, h, w]     randn   posterior sample of the conditioning frame
+        6 sigma_u          [B]              rand    uniform of the EDM sigma, LogNormal(0.7, 1.6)
+        7 dropout_u        [B]              rand    conditioning dropout (only when conditioning_dropout)
+
+    Each is drawn from `generator` on the generator's own device (CPU or CUDA; the default generator of `device` when None) and
+    then moved to `device`, as diffusers' randn_tensor does, so a CPU generator gives the same values on any device."""
+    gdev = torch.device(device) if generator is None else generator.device
+    kinds = dict(DRAWS)
+    return {name: getattr(torch, kinds[name])(shape, generator=generator, device=gdev, dtype=F32).to(device)
+            for name, shape in draw_shapes(B, F, H, W, conditioning_dropout).items()}
+
+
+def log_normal(u: torch.Tensor, loc: float, scale: float) -> torch.Tensor:
+    """rand_log_normal (train_svd.py:64-67) from its uniform draw u, in fp32"""
+    return torch.distributions.Normal(loc, scale).icdf(u * (1 - 2e-7) + 1e-7).exp()
+
+
+def _unet_dims(unet_config):
+    """(in_channels, cross_attention_dim, addition_time_embed_dim, add_embedding in_features) of a UNet or its config"""
+    cfg = getattr(unet_config, "config", unet_config)
+    add = getattr(unet_config, "add_embedding", None)
+    in_features = add.linear_1.in_features if add is not None else cfg.projection_class_embeddings_input_dim
+    return cfg.in_channels, cfg.cross_attention_dim, cfg.addition_time_embed_dim, in_features
+
+
+def check_train_inputs(vae, image_encoder, unet_config, pixel_values, draws, conditioning_dropout_prob=None):
+    """every check of assemble_train_batch, before any launch: ValueError / TypeError for what does not fit, RuntimeError for
+    models or tensors off the GPU (there is no CPU path)"""
+    if pixel_values.dim() != 5 or pixel_values.shape[2] != 3:
+        raise ValueError(f"pixel_values must be [B, F, 3, H, W], got {tuple(pixel_values.shape)}")
+    if pixel_values.dtype not in (F32, torch.bfloat16):
+        raise TypeError(f"pixel_values has dtype {pixel_values.dtype}; supported: float32, bfloat16")
+    B, F, _, H, W = pixel_values.shape
+    if H % 64 or W % 64:
+        raise ValueError(f"frame height and width must be multiples of 64 (the UNet's latents, H/8 x W/8, need sides that are "
+                         f"multiples of 8); got {H}x{W}")
+    in_ch, cross, add_dim, add_in = _unet_dims(unet_config)
+    lc = vae.config.latent_channels
+    if 2 * lc != in_ch:
+        raise ValueError(f"the VAE's latent_channels x 2 = {2 * lc} must equal the UNet's in_channels = {in_ch} (noisy latents "
+                         "concatenated with the conditioning latents)")
+    if lc != 4 or 1 << (len(vae.config.block_out_channels) - 1) != 8:
+        raise ValueError("the VAE must have 4 latent channels and downsample by 8 (the draws are [., 4, H/8, W/8])")
+    if image_encoder.config.projection_dim != cross:
+        raise ValueError(f"the CLIP projection_dim {image_encoder.config.projection_dim} must equal the UNet's cross_attention_dim {cross}")
+    if add_dim * 3 != add_in:
+        raise ValueError(f"Model expects an added time embedding vector of length {add_in}, but a vector of {add_dim * 3} was "
+                         "created (addition_time_embed_dim x 3 time ids). The model has an incorrect config.")
+    shapes = draw_shapes(B, F, H, W, conditioning_dropout_prob is not None)
+    for name, shape in shapes.items():
+        t = draws.get(name)
+        if t is None or t.dtype != F32 or tuple(t.shape) != shape:
+            raise ValueError(f"draws[{name!r}] must be an fp32 tensor of shape {shape} (draw_train_noise), got "
+                             f"{None if t is None else (tuple(t.shape), t.dtype)}")
+    for n, p in list(vae.named_parameters()) + list(image_encoder.named_parameters()):
+        raw.dtype_code(p, f"parameter {n}")
+    on_gpu = [pixel_values.is_cuda, vae.device.type == "cuda", image_encoder.device.type == "cuda"] + [draws[n].is_cuda for n in shapes]
+    if not all(on_gpu):
+        raise RuntimeError("svd_xtend_b200: assemble_train_batch only runs on a CUDA (sm_90a) device (frames, draws, VAE and image "
+                           "encoder); there is no CPU fallback")
+    return B, F, H, W
+
+
+def assemble_train_batch(vae, image_encoder, unet_config, pixel_values: torch.Tensor, draws: Dict[str, torch.Tensor], *,
+                         conditioning_dropout_prob: Optional[float] = None, fps: int = 7, motion_bucket_id: int = 127,
+                         image_mean=CLIP_MEAN, image_std=CLIP_STD) -> Dict[str, torch.Tensor]:
+    """train_svd.py:944-1017 from the frames pixel_values [B, F, 3, H, W] (in [-1, 1]) and the step's draws (draw_train_noise) ->
+    the UNet batch, the dict workload.synthetic_batch returns: sample [B, F, 8, h, w], timestep [B], encoder_hidden_states
+    [B, 1, cross_dim], added_time_ids [B, 3], latents / noisy [B, F, 4, h, w] and sigmas [B, 1, 1, 1, 1], all fp32.
+
+    unet_config: the UNet or its config. The VAE and the image encoder run forward only. Unlike the reference, every clip's
+    added_time_ids carry its own conditioning sigma, and everything before the UNet is fp32 (INTEGRATION.md §3.2)."""
+    B, F, H, W = check_train_inputs(vae, image_encoder, unet_config, pixel_values, draws, conditioning_dropout_prob)
+    dev = pixel_values.device
+    x = pixel_values.contiguous()
+    cond_sigma = log_normal(draws["cond_u"], -3.0, 0.5)          # :954
+    sigma = log_normal(draws["sigma_u"], 0.7, 1.6)               # :964
+    with torch.no_grad():
+        rows = torch.empty(B * (F + 1) * H * W, vae.ROW_PAD, device=dev, dtype=torch.bfloat16)
+        raw.vae_frames_in(x, draws["cond_pixel_eps"], cond_sigma, rows, vae.ROW_PAD)
+        moments = vae._run_rows(rows, B * (F + 1), H, W)
+        emb = encode_image(image_encoder, x[:, 0], image_mean, image_std).float()      # the clean first frame (:975)
+    ehs = emb.unsqueeze(1)
+    if conditioning_dropout_prob is None:
+        image_mask = torch.ones(B, device=dev, dtype=F32)
+    else:
+        p = conditioning_dropout_prob
+        r = draws["dropout_u"]
+        ehs = torch.where((r < 2 * p).reshape(B, 1, 1), torch.zeros_like(ehs), ehs)            # :996-999
+        image_mask = 1 - (r >= p).to(F32) * (r < 3 * p).to(F32)                                # :1003-1008
+    h, w = H // 8, W // 8
+    sample = torch.empty(B, F, 8, h, w, device=dev, dtype=F32)
+    noisy = torch.empty(B, F, 4, h, w, device=dev, dtype=F32)
+    latents = torch.empty(B, F, 4, h, w, device=dev, dtype=F32)
+    raw.edm_prepare(moments, draws["latent_eps"], draws["noise"], draws["cond_latent_eps"], sigma, image_mask,
+                    vae.config.scaling_factor, sample, noisy, latents)
+    added_time_ids = torch.stack([torch.full_like(cond_sigma, float(fps)), torch.full_like(cond_sigma, float(motion_bucket_id)),
+                                  cond_sigma], dim=1)
+    return dict(sample=sample, timestep=0.25 * sigma.log(), encoder_hidden_states=ehs, added_time_ids=added_time_ids,
+                latents=latents, noisy=noisy, sigmas=sigma.reshape(B, 1, 1, 1, 1))
+
+
+class VideoTrainStep:
+    """One training step from frames: `step(pixel_values)` -> the 0-dim device loss.
+
+    Each call copies the frames [B, F, 3, H, W] (frames_shape; fp32 or bf16, pinned host or device memory) into a static device
+    buffer, draws the step's noise eagerly (draw_train_noise, from `generator`) into static buffers, and replays one captured
+    train.GraphedStep: opt.zero_grad -> assemble_train_batch -> UNet forward -> workload.edm_loss -> backward -> opt.step().
+    cuda_graph=False runs the same function eagerly. Any optimizer of the package works (its on_updated hook should refresh the
+    UNet's operands, as for any GraphedStep); `opt.lr = ...` between calls takes effect. Construction leaves the weights, the
+    optimizer's moments and step count, an attached EMA and the generator's state as they were."""
+
+    def __init__(self, unet, vae, image_encoder, opt, *, frames_shape, conditioning_dropout_prob: Optional[float] = None,
+                 generator: Optional[torch.Generator] = None, fps: int = 7, motion_bucket_id: int = 127, image_mean=CLIP_MEAN,
+                 image_std=CLIP_STD, cuda_graph: bool = True):
+        self.unet, self.vae, self.image_encoder, self.opt = unet, vae, image_encoder, opt
+        self.B, self.F, self.H, self.W = (int(v) for v in frames_shape)
+        self.dropout = conditioning_dropout_prob
+        self.kw = dict(conditioning_dropout_prob=conditioning_dropout_prob, fps=fps, motion_bucket_id=motion_bucket_id,
+                       image_mean=image_mean, image_std=image_std)
+        dev = vae.device
+        self.device = dev
+        self.generator = generator if generator is not None else torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
+        self.static = {"pixel_values": torch.zeros(self.B, self.F, 3, self.H, self.W, device=dev, dtype=F32)}
+        gstate = self.generator.get_state()
+        self.static.update(self.draw())
+        check_train_inputs(vae, image_encoder, unet, self.static["pixel_values"], self.static, conditioning_dropout_prob)
+        self.graphed = None
+        if cuda_graph:
+            from .train import GraphedStep
+
+            def restored():
+                self.generator.set_state(gstate)
+                unet.refresh_trainable_operands(shadow_current=opt.arena.shadow is not None)
+
+            self.graphed = GraphedStep(self._step, self.static, warmup=2, restore=opt.snapshot_tensors(), on_restored=restored)
+        else:
+            self.generator.set_state(gstate)
+
+    def draw(self) -> Dict[str, torch.Tensor]:
+        return draw_train_noise(self.B, self.F, self.H, self.W, generator=self.generator, device=self.device,
+                                conditioning_dropout=self.dropout is not None)
+
+    def _step(self, s: Dict[str, torch.Tensor]) -> torch.Tensor:
+        self.opt.zero_grad()
+        b = assemble_train_batch(self.vae, self.image_encoder, self.unet, s["pixel_values"], s, **self.kw)
+        pred = self.unet(b["sample"], b["timestep"], b["encoder_hidden_states"], added_time_ids=b["added_time_ids"]).sample
+        loss = edm_loss(pred.float(), b["noisy"], b["latents"], b["sigmas"])
+        loss.backward()
+        self.opt.step()
+        return loss.detach()
+
+    def __call__(self, pixel_values: torch.Tensor) -> torch.Tensor:
+        if tuple(pixel_values.shape) != (self.B, self.F, 3, self.H, self.W):
+            raise ValueError(f"VideoTrainStep was built for frames {(self.B, self.F, 3, self.H, self.W)}, got {tuple(pixel_values.shape)}")
+        if pixel_values.dtype not in (F32, torch.bfloat16):
+            raise TypeError(f"pixel_values has dtype {pixel_values.dtype}; supported: float32, bfloat16")
+        self.static["pixel_values"].copy_(pixel_values, non_blocking=True)
+        for k, v in self.draw().items():
+            self.static[k].copy_(v)
+        if self.graphed is not None:
+            return self.graphed.replay()
+        return self._step(self.static)
