@@ -428,6 +428,24 @@ int svdx_adamw8bit_ema(const void* jobs, const int32_t* block_prefix, int32_t nj
  * x_dtype (0 fp32, 1 bf16); eps: fp32 [B][3][H][W]; sigma_c: DEVICE fp32 [B]. One launch. */
 int svdx_vae_frames_in(const void* x, int32_t x_dtype, const float* cond_eps, const float* cond_sigma, int32_t B, int32_t F,
                        int32_t H, int32_t W, int32_t c_pad, void* dst, void* stream);
+/* svdx_vae_frames_in_range: the rows of svdx_vae_frames_in for the frames [first, first + count) of its B*(F+1) frame index space
+ * only, into dst [count * H*W][c_pad] (for an encode in frame chunks). Same values, one launch. */
+int svdx_vae_frames_in_range(const void* x, int32_t x_dtype, const float* cond_eps, const float* cond_sigma, int32_t B, int32_t F,
+                             int32_t H, int32_t W, int32_t first, int32_t count, int32_t c_pad, void* dst, void* stream);
+/* Decoded uint8 frames (csrc/frames.cu). Resize = what Pillow's Image.resize((W, H)) returns for an RGB image with its default
+ * BICUBIC filter: 8-bpc two-pass resample, horizontal first into a uint8 intermediate, then vertical, 22-bit fixed-point taps.
+ * svdx_resize_taps_ksize: taps per output pixel along an axis of in_size -> out_size (or < 0 on bad sizes).
+ * svdx_resize_taps (HOST): the taps of that axis, int32 [out_size][2 + ksize]: first source index, tap count, ksize weights.
+ * svdx_frames_u8_in: from uint8 frames src [B][F][H0][W0][3] (HWC, RGB) and DEVICE copies of the taps of H0 -> H (taps_y) and
+ * W0 -> W (taps_x), the rows of svdx_vae_frames_in for the frames [first, first + count) into dst [count * H*W][c_pad] (c_pad a
+ * multiple of 8, dst 16-byte aligned), where x = fl(fl(resize(src) / 127.5f) - 1) (train_svd.py's DummyDataset); for each
+ * conditioning frame B*F + b in the range, also the clean first frame x[b][0] into first_frames fp32 [B][3][H][W] (may be NULL).
+ * One launch. */
+int svdx_resize_taps_ksize(int32_t in_size, int32_t out_size);
+int svdx_resize_taps(int32_t in_size, int32_t out_size, int32_t* taps);
+int svdx_frames_u8_in(const uint8_t* src, int32_t H0, int32_t W0, const int32_t* taps_y, int32_t ksize_y, const int32_t* taps_x,
+                      int32_t ksize_x, const float* cond_eps, const float* cond_sigma, int32_t B, int32_t F, int32_t H, int32_t W,
+                      int32_t first, int32_t count, int32_t c_pad, void* dst, float* first_frames, void* stream);
 /* svdx_edm_prepare: from the fp32 moments [B*(F+1)][2C][h][w] of that encode (mean, then logvar), per latent element
  *   z = mean + exp(0.5 * clamp(logvar, -30, 20)) * eps,  latent = z * sf,  noisy = latent + noise * sigma[b]
  * (:948, :287, :951, :967) and the conditioning latents c = (z_c * sf) * (1 / sf) of frame B*F + b (:959-960: torch's division of

@@ -1,17 +1,22 @@
 #!/usr/bin/env python
 """Training step from video frames (svd_xtend_b200.video_train.VideoTrainStep) on the H100 path, one JSON line.
 
-    python scripts/bench_video_train.py --config 2|4 [--steps K] [--warmup W]
+    python scripts/bench_video_train.py --config 2|4 [--steps K] [--warmup W] [--forms graphed,eager,latent_only]
+                                        [--input float|u8] [--source 1080x1920] [--encode-chunk N] [--frozen-dtype fp32|bf16]
 
 Seeded default-init SVD UNet (the config's trainable set and gradient checkpointing), VAE encoder and CLIP ViT-H image encoder,
-FusedAdamW, B = 1, conditioning dropout 0.1. Three forms of the step, timed in alternating windows of K steps, medians of 3:
+FusedAdamW, B = 1, conditioning dropout 0.1. The forms of the step (--forms, default all three), timed in alternating windows of
+K steps, medians of 3:
   * graphed: VideoTrainStep (frames -> VAE encode -> CLIP -> batch assembly -> UNet -> loss -> backward -> AdamW, one graph),
     frames from a device buffer, draws made eagerly each step;
   * eager: the same VideoTrainStep with cuda_graph=False;
   * latent_only: the latent-input graphed step bench.py times (workload.synthetic_batch, no VAE / CLIP).
-Reports ms per step and frames/s of each, max_memory_allocated after all three are built, the card's name and power limit, and
-the SM clock sampled during the timed windows. A form that does not fit on the card is reported as failed. Writes nothing to
-the source tree.
+--input u8 feeds decoded uint8 frames [1, F, H0, W0, 3] of --source size from pinned host memory (resized on the GPU as Pillow's
+Image.resize does); float feeds fp32 frames [1, F, 3, H, W] from a device buffer. --encode-chunk N encodes N frames at a time.
+--frozen-dtype: the VAE's and CLIP's weights, fp32 (default) or bf16 as train_svd.py holds them under --mixed_precision=bf16.
+Reports ms per step and frames/s of each form, torch.cuda.max_memory_allocated / memory_reserved after each form's
+construction, after the warm-up and after the timed windows, the card's name and power limit, and the SM clock sampled during
+the timed windows. A form that does not fit on the card is reported as failed. Writes nothing to the source tree.
 """
 import argparse
 import json
@@ -26,12 +31,26 @@ if ROOT not in sys.path:
 import torch  # noqa: E402
 
 
+def _mem():
+    return {"max_allocated_gib": round(torch.cuda.max_memory_allocated() / 2 ** 30, 2),
+            "reserved_gib": round(torch.cuda.memory_reserved() / 2 ** 30, 2)}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config", type=int, choices=(2, 4), default=2)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--forms", default="graphed,eager,latent_only")
+    ap.add_argument("--input", choices=("float", "u8"), default="float")
+    ap.add_argument("--source", default="1080x1920", help="H0xW0 of the uint8 frames (--input u8)")
+    ap.add_argument("--encode-chunk", type=int, default=None)
+    ap.add_argument("--frozen-dtype", choices=("fp32", "bf16"), default="fp32")
     args = ap.parse_args()
+    wanted = [f for f in args.forms.split(",") if f]
+    if not wanted or any(f not in ("graphed", "eager", "latent_only") for f in wanted):
+        raise SystemExit(f"--forms: a comma-separated subset of graphed,eager,latent_only, got {args.forms!r}")
+    H0, W0 = (int(v) for v in args.source.lower().split("x"))
     if not torch.cuda.is_available():
         raise RuntimeError("bench_video_train.py needs a CUDA device: the step has no CPU fallback")
 
@@ -57,6 +76,9 @@ def main():
         clip = CLIPVisionModelWithProjection(**CLIP_CONFIG)
     for m in (unet, vae, clip):
         m.to(dev).requires_grad_(False)
+    if args.frozen_dtype == "bf16":             # train_svd.py:665-673
+        vae.to(torch.bfloat16)
+        clip.to(torch.bfloat16)
     vae.eval()
     clip.eval()
     for n, p in unet.named_parameters():
@@ -70,44 +92,56 @@ def main():
     opt = FusedAdamW(arena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8)
     opt.on_updated = lambda: unet.refresh_trainable_operands(shadow_current=True)
     g = torch.Generator(device="cpu").manual_seed(5)
-    frames = (torch.rand(1, F, 3, H, W, generator=g) * 2 - 1).to(dev)
+    if args.input == "u8":
+        frames = torch.randint(0, 256, (1, F, H0, W0, 3), generator=g, dtype=torch.uint8).pin_memory()
+    else:
+        frames = (torch.rand(1, F, 3, H, W, generator=g) * 2 - 1).to(dev)
+    memory = {"models": _mem()}
 
     forms, failed = {}, {}
-    kw = dict(frames_shape=(1, F, H, W), conditioning_dropout_prob=0.1, generator=torch.Generator(dev).manual_seed(0))
-    try:
-        graphed = VideoTrainStep(unet, vae, clip, opt, **kw)
-        forms["graphed"] = lambda: graphed(frames)
-    except torch.OutOfMemoryError as e:
-        failed["graphed"] = f"OutOfMemoryError: {str(e).splitlines()[0]}"
-        torch.cuda.empty_cache()
-    b = {k: v.to(dev) for k, v in synthetic_batch(1, F, cfg["h"], cfg["w"], seed=1234).items()}
+    kw = dict(frames_shape=(1, F, H, W), conditioning_dropout_prob=0.1, generator=torch.Generator(dev).manual_seed(0),
+              source_size=(H0, W0) if args.input == "u8" else None, encode_chunk_size=args.encode_chunk)
 
-    def latent_step(bb):
-        arena.zero_grad()
-        pred = unet(bb["sample"], bb["timestep"], bb["encoder_hidden_states"], added_time_ids=bb["added_time_ids"]).sample
-        loss = edm_loss(pred.float(), bb["noisy"], bb["latents"], bb["sigmas"])
-        loss.backward()
-        opt.step()
-        return loss
-    try:
-        latent = GraphedStep(latent_step, b, warmup=3, restore=opt.snapshot_tensors(),
-                             on_restored=lambda: unet.refresh_trainable_operands(shadow_current=True))
-        forms["latent_only"] = latent.replay
-    except torch.OutOfMemoryError as e:
-        failed["latent_only"] = f"OutOfMemoryError: {str(e).splitlines()[0]}"
+    def oom(name, e):
+        failed[name] = f"OutOfMemoryError: {str(e).splitlines()[0]}"
         torch.cuda.empty_cache()
-    eager = VideoTrainStep(unet, vae, clip, opt, cuda_graph=False, **kw)
-    forms["eager"] = lambda: eager(frames)
-    try:
-        for fn in forms.values():
+
+    if "graphed" in wanted:
+        try:
+            graphed = VideoTrainStep(unet, vae, clip, opt, **kw)
+            forms["graphed"] = lambda: graphed(frames)
+        except torch.OutOfMemoryError as e:
+            oom("graphed", e)
+        memory["graphed_built"] = _mem()
+    if "latent_only" in wanted:
+        b = {k: v.to(dev) for k, v in synthetic_batch(1, F, cfg["h"], cfg["w"], seed=1234).items()}
+
+        def latent_step(bb):
+            arena.zero_grad()
+            pred = unet(bb["sample"], bb["timestep"], bb["encoder_hidden_states"], added_time_ids=bb["added_time_ids"]).sample
+            loss = edm_loss(pred.float(), bb["noisy"], bb["latents"], bb["sigmas"])
+            loss.backward()
+            opt.step()
+            return loss
+        try:
+            latent = GraphedStep(latent_step, b, warmup=3, restore=opt.snapshot_tensors(),
+                                 on_restored=lambda: unet.refresh_trainable_operands(shadow_current=True))
+            forms["latent_only"] = latent.replay
+        except torch.OutOfMemoryError as e:
+            oom("latent_only", e)
+        memory["latent_only_built"] = _mem()
+    if "eager" in wanted:
+        eager = VideoTrainStep(unet, vae, clip, opt, cuda_graph=False, **kw)
+        forms["eager"] = lambda: eager(frames)
+    for k in list(forms):
+        try:
             for _ in range(warmup):
-                fn()
-        torch.cuda.synchronize()
-    except torch.OutOfMemoryError as e:
-        failed["eager"] = f"OutOfMemoryError: {str(e).splitlines()[0]}"
-        forms.pop("eager")
-        torch.cuda.empty_cache()
-    mem = torch.cuda.max_memory_allocated()
+                forms[k]()
+            torch.cuda.synchronize()
+        except torch.OutOfMemoryError as e:
+            forms.pop(k)
+            oom(k, e)
+    memory["warmed_up"] = _mem()
 
     clocks = ClockSampler(0)
     c0 = clocks.count()
@@ -125,15 +159,18 @@ def main():
             times[k].append(e0.elapsed_time(e1) / steps)
     c1 = clocks.count()
     clk = clocks.stop(c0, c1)
+    memory["timed"] = _mem()
     res = {}
     for k, ts in times.items():
         ms = statistics.median(ts)
         res[k] = {"ms_per_step": round(ms, 3), "frames_per_s": round(F * 1e3 / ms, 2), "windows_ms": [round(t, 3) for t in ts]}
     res.update({k: {"failed": v} for k, v in failed.items()})
     print(json.dumps({"metric": "video_train_step", "config": args.config, "frames": F, "pixels": [H, W], "batch": 1,
-                      "steps_per_window": steps, "forms": res, "final_loss": None if loss is None else float(loss.float().item()),
-                      "max_memory_allocated_gib": round(mem / 2 ** 30, 2), "device": torch.cuda.get_device_name(dev),
-                      "power_limit_w": power_limit_w(0), "sm_clock": clk}))
+                      "input": args.input, "source": [H0, W0] if args.input == "u8" else None, "encode_chunk": args.encode_chunk,
+                      "frozen_dtype": args.frozen_dtype, "steps_per_window": steps, "forms": res,
+                      "final_loss": None if loss is None else float(loss.float().item()),
+                      "max_memory_allocated_gib": round(torch.cuda.max_memory_allocated() / 2 ** 30, 2), "memory": memory,
+                      "device": torch.cuda.get_device_name(dev), "power_limit_w": power_limit_w(0), "sm_clock": clk}))
 
 
 if __name__ == "__main__":

@@ -122,6 +122,12 @@ _PROTOS = {
     "svdx_multi_transpose": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p],
     "svdx_lora_merge": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p],
     "svdx_vae_frames_in": [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
+    "svdx_vae_frames_in_range": [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                 c_void_p],
+    "svdx_resize_taps_ksize": [c_int, c_int],
+    "svdx_resize_taps": [c_int, c_int, c_void_p],
+    "svdx_frames_u8_in": [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                          c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "svdx_edm_prepare": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int, c_int, c_int, c_int,
                          c_void_p, c_void_p, c_void_p, c_void_p],
 }

@@ -18,18 +18,19 @@ SVDX_DEVINL float ld_pix(const void* x, int bf, long long i) {
   return bf ? __bfloat162float(reinterpret_cast<const bf16*>(x)[i]) : reinterpret_cast<const float*>(x)[i];
 }
 
-// row n < B*F: clip frame n = b*F + f; row B*F + b: fl(fl(eps[b] * sigma_c[b]) + x[b, 0])
+// row n < B*F: clip frame n = b*F + f; row B*F + b: fl(fl(eps[b] * sigma_c[b]) + x[b, 0]). dst holds the rows of the frames
+// [first, first + count).
 __global__ void vae_frames_in_kernel(const void* __restrict__ x, int x_bf16, const float* __restrict__ eps,
-                                     const float* __restrict__ sigma_c, int B, int F, int H, int W, int c_pad,
+                                     const float* __restrict__ sigma_c, int B, int F, int H, int W, int first, int count, int c_pad,
                                      bf16* __restrict__ dst) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long hw = (long long)H * W;
-  const long long total = (long long)B * (F + 1) * hw * c_pad;
+  const long long total = (long long)count * hw * c_pad;
   if (idx >= total) return;
   const int c = (int)(idx % c_pad);
   const long long pix = idx / c_pad;
   const long long p = pix % hw;
-  const int n = (int)(pix / hw);
+  const int n = first + (int)(pix / hw);
   float v = 0.f;
   if (c < 3) {
     if (n < B * F) {
@@ -88,9 +89,19 @@ extern "C" int svdx_vae_frames_in(const void* x, int32_t x_dtype, const float* c
                                   int32_t F, int32_t H, int32_t W, int32_t c_pad, void* dst, void* stream) {
   if (!x || !cond_eps || !cond_sigma || !dst || B <= 0 || F <= 0 || H <= 0 || W <= 0 || c_pad < 3 || (x_dtype != 0 && x_dtype != 1))
     return svdx_fail(SVDX_E_BADARG, "vae_frames_in: bad arguments (fp32 / bf16 frames [B, F, 3, H, W], c_pad >= 3)");
-  const long long total = (long long)B * (F + 1) * H * W * c_pad;
-  vae_frames_in_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ST(stream)>>>(x, x_dtype, cond_eps, cond_sigma, B, F, H, W, c_pad,
-                                                                                reinterpret_cast<bf16*>(dst));
+  return svdx_vae_frames_in_range(x, x_dtype, cond_eps, cond_sigma, B, F, H, W, 0, B * (F + 1), c_pad, dst, stream);
+}
+
+extern "C" int svdx_vae_frames_in_range(const void* x, int32_t x_dtype, const float* cond_eps, const float* cond_sigma, int32_t B,
+                                        int32_t F, int32_t H, int32_t W, int32_t first, int32_t count, int32_t c_pad, void* dst,
+                                        void* stream) {
+  if (!x || !cond_eps || !cond_sigma || !dst || B <= 0 || F <= 0 || H <= 0 || W <= 0 || c_pad < 3 || (x_dtype != 0 && x_dtype != 1) ||
+      first < 0 || count <= 0 || first + count > B * (F + 1))
+    return svdx_fail(SVDX_E_BADARG, "vae_frames_in_range: bad arguments (fp32 / bf16 frames [B, F, 3, H, W], c_pad >= 3, "
+                                    "0 <= first < first + count <= B*(F+1))");
+  const long long total = (long long)count * H * W * c_pad;
+  vae_frames_in_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ST(stream)>>>(x, x_dtype, cond_eps, cond_sigma, B, F, H, W, first,
+                                                                                count, c_pad, reinterpret_cast<bf16*>(dst));
   SVDX_CHECK_LAUNCH("vae_frames_in");
   return SVDX_OK;
 }

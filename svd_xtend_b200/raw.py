@@ -603,6 +603,72 @@ def vae_frames_in(x, cond_eps, cond_sigma, dst, c_pad=64):
     return dst
 
 
+def vae_frames_in_range(x, cond_eps, cond_sigma, dst, first, count, c_pad=64):
+    """the rows of vae_frames_in for the frames [first, first + count) of its B*(F+1) frame index space (clip frames, then the
+    conditioning frames) only: dst bf16 [count * H*W, c_pad]"""
+    B, F, Cc, H, W = x.shape
+    if Cc != 3 or not x.is_contiguous() or x.dtype not in (torch.float32, bf16):
+        raise ValueError("vae_frames_in_range: x must be a contiguous fp32 / bf16 [B, F, 3, H, W] tensor")
+    if cond_eps.dtype != torch.float32 or not cond_eps.is_contiguous() or cond_eps.numel() != B * 3 * H * W:
+        raise ValueError("vae_frames_in_range: cond_eps must be a contiguous fp32 tensor of B*3*H*W elements")
+    if cond_sigma.dtype != torch.float32 or cond_sigma.numel() != B:
+        raise ValueError("vae_frames_in_range: cond_sigma must be fp32 [B]")
+    if not 0 <= first < first + count <= B * (F + 1):
+        raise ValueError(f"vae_frames_in_range: frames [{first}, {first + count}) are not within [0, {B * (F + 1)})")
+    if dst.dtype != bf16 or not dst.is_contiguous() or dst.shape != (count * H * W, c_pad):
+        raise ValueError(f"vae_frames_in_range: dst must be a contiguous bf16 [{count * H * W}, {c_pad}] tensor")
+    check(load().svdx_vae_frames_in_range(x.data_ptr(), dtype_code(x, "frames"), cond_eps.data_ptr(), cond_sigma.data_ptr(), B, F, H, W,
+                                          first, count, c_pad, dst.data_ptr(), _stream()), "vae_frames_in")
+    return dst
+
+
+def resize_taps(in_size: int, out_size: int) -> torch.Tensor:
+    """the taps of Pillow's 8-bpc BICUBIC resample of one axis in_size -> out_size (svdx_resize_taps, computed on the host):
+    int32 [out_size, 2 + ksize] = first source index, tap count, ksize 22-bit fixed-point weights"""
+    lib = load()
+    ks = lib.svdx_resize_taps_ksize(int(in_size), int(out_size))
+    if ks < 0:
+        _lib.check(ks, "resize_taps")
+    taps = torch.empty(int(out_size), 2 + ks, dtype=torch.int32)
+    rc = lib.svdx_resize_taps(int(in_size), int(out_size), taps.data_ptr())
+    if rc:
+        _lib.check(rc, "resize_taps")
+    return taps
+
+
+def frames_u8_in(src, taps_y, taps_x, cond_eps, cond_sigma, dst, size, first, count, first_frames=None, c_pad=64):
+    """from uint8 HWC frames src [B, F, H0, W0, 3] on the device: Pillow's BICUBIC resize to size = (H, W) (taps_y / taps_x: device
+    copies of resize_taps(H0, H) / resize_taps(W0, W)), fl(fl(u / 127.5f) - 1), and the rows of vae_frames_in for the frames
+    [first, first + count) into dst bf16 [count * H*W, c_pad]; the clean first frames fp32 [B, 3, H, W] into first_frames (if
+    given) for the conditioning frames in the range (svdx_frames_u8_in)"""
+    if src.dtype != torch.uint8:
+        raise TypeError(f"frames_u8_in: src has dtype {src.dtype}; expected uint8")
+    if src.dim() != 5 or src.shape[-1] != 3 or not src.is_contiguous():
+        raise ValueError(f"frames_u8_in: src must be a contiguous uint8 [B, F, H0, W0, 3] tensor, got {tuple(src.shape)}")
+    B, F, H0, W0, _ = src.shape
+    H, W = (int(v) for v in size)
+    for t, n, what in ((taps_y, H, "taps_y"), (taps_x, W, "taps_x")):
+        if t.dtype != torch.int32 or not t.is_contiguous() or t.dim() != 2 or t.shape[0] != n:
+            raise ValueError(f"frames_u8_in: {what} must be a contiguous int32 [{n}, 2 + ksize] tensor (resize_taps)")
+    if cond_eps.dtype != torch.float32 or not cond_eps.is_contiguous() or cond_eps.numel() != B * 3 * H * W:
+        raise ValueError("frames_u8_in: cond_eps must be a contiguous fp32 tensor of B*3*H*W elements")
+    if cond_sigma.dtype != torch.float32 or cond_sigma.numel() != B:
+        raise ValueError("frames_u8_in: cond_sigma must be fp32 [B]")
+    if not 0 <= first < first + count <= B * (F + 1):
+        raise ValueError(f"frames_u8_in: frames [{first}, {first + count}) are not within [0, {B * (F + 1)})")
+    if dst.dtype != bf16 or not dst.is_contiguous() or dst.shape != (count * H * W, c_pad):
+        raise ValueError(f"frames_u8_in: dst must be a contiguous bf16 [{count * H * W}, {c_pad}] tensor")
+    if first_frames is not None and (first_frames.dtype != torch.float32 or not first_frames.is_contiguous()
+                                     or first_frames.shape != (B, 3, H, W)):
+        raise ValueError(f"frames_u8_in: first_frames must be a contiguous fp32 [{B}, 3, {H}, {W}] tensor")
+    if not all(t.is_cuda for t in (src, taps_y, taps_x, cond_eps, cond_sigma, dst)):
+        raise RuntimeError("svd_xtend_b200: frames_u8_in runs on a CUDA (sm_90a) device only; there is no CPU fallback")
+    check(load().svdx_frames_u8_in(src.data_ptr(), H0, W0, taps_y.data_ptr(), taps_y.shape[1] - 2, taps_x.data_ptr(),
+                                   taps_x.shape[1] - 2, cond_eps.data_ptr(), cond_sigma.data_ptr(), B, F, H, W, first, count, c_pad,
+                                   dst.data_ptr(), _ptr(first_frames), _stream()), "frames_u8_in")
+    return dst
+
+
 def edm_prepare(moments, latent_eps, noise, cond_latent_eps, sigma, image_mask, scaling_factor, sample, noisy, latents):
     """posterior samples, EDM noising and the UNet input from the moments [B*(F+1), 2C, h, w] of one encode of the clip and
     conditioning frames (svd_xtend_b200.h, svdx_edm_prepare): sample [B, F, 2C, h, w], noisy / latents [B, F, C, h, w], all fp32"""

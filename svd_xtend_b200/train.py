@@ -753,15 +753,22 @@ class GraphedStep:
     and no reference to a warm-up autograd graph is kept."""
 
     def __init__(self, fn, static_inputs: Dict[str, torch.Tensor], warmup: int = 3, restore: Optional[List[torch.Tensor]] = None,
-                 on_restored=None):
+                 on_restored=None, restore_on_host: bool = False):
         """restore: tensors whose contents the warm-up / capture runs must not change (pass
         `opt.snapshot_tensors()`): they are cloned first and copied back after the capture, so that training starts from
         the caller's weights, optimizer moments and step count, not from `warmup + 2` stray updates on the static batch.
         on_restored: called after the copy-back (e.g. `lambda: unet.refresh_trainable_operands(shadow_current=True)` to
-        re-derive the transposed weight operands from the restored bf16 shadow)."""
+        re-derive the transposed weight operands from the restored bf16 shadow).
+        restore_on_host: keep the `restore` snapshot in pinned host memory instead of device clones, which lowers the peak device
+        memory of the construction by the snapshot's size and does not change what a step computes."""
         self.fn = fn
         self.static = static_inputs
-        saved = [t.clone() for t in restore] if restore else []
+        if restore and restore_on_host:
+            saved = [torch.empty(t.shape, dtype=t.dtype, pin_memory=True) for t in restore]
+            for c, t in zip(saved, restore):
+                c.copy_(t, non_blocking=True)
+        else:
+            saved = [t.clone() for t in restore] if restore else []
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
@@ -774,7 +781,7 @@ class GraphedStep:
             self.out = fn(self.static)
         if restore:
             for t, c in zip(restore, saved):
-                t.copy_(c)
+                t.copy_(c, non_blocking=restore_on_host)
             if on_restored is not None:
                 on_restored()
         else:

@@ -12,10 +12,15 @@ optimizer, all inside one captured `train.GraphedStep`. The batch assembly is tw
 encode of B*(F+1) frames replaces the reference's two: the encoder works frame by frame), and `svdx_edm_prepare` turns the
 moments into the posterior samples, the noisy latents, the target and the UNet input. The per-clip scalars (log-normal sigmas,
 timesteps, time ids, dropout masks) are O(B) torch ops. oracle/svd_train_batch_oracle.py states the same in torch.
+
+Decoded uint8 frames [B, F, H0, W0, 3] (VideoTrainStep(source_size=...), assemble_train_batch(size=...)) take the place of
+`svdx_vae_frames_in` with `svdx_frames_u8_in` (csrc/frames.cu), which resizes them as Pillow's Image.resize does
+(oracle/svd_resize_oracle.py) and normalises them as train_svd.py's DummyDataset does. encode_chunk_size encodes the frames in
+chunks.
 """
 from __future__ import annotations
 
-from typing import Dict, Optional
+from typing import Dict, Optional, Tuple
 
 import torch
 
@@ -76,14 +81,32 @@ def _unet_dims(unet_config):
     return cfg.in_channels, cfg.cross_attention_dim, cfg.addition_time_embed_dim, in_features
 
 
-def check_train_inputs(vae, image_encoder, unet_config, pixel_values, draws, conditioning_dropout_prob=None):
+def _check_u8_frames(frames, size):
+    """(B, F, H, W) of uint8 frames [B, F, H0, W0, 3] to be resized to size = (H, W); ValueError / TypeError otherwise"""
+    if size is None:
+        raise TypeError(f"pixel_values has dtype {frames.dtype}; uint8 frames [B, F, H0, W0, 3] need the training size=(H, W)")
+    if frames.dim() != 5 or frames.shape[-1] != 3:
+        raise ValueError(f"uint8 frames must be [B, F, H0, W0, 3] (HWC, RGB), got {tuple(frames.shape)}")
+    H, W = (int(v) for v in size)
+    return frames.shape[0], frames.shape[1], H, W
+
+
+def check_train_inputs(vae, image_encoder, unet_config, pixel_values, draws, conditioning_dropout_prob=None, size=None,
+                       encode_chunk_size=None):
     """every check of assemble_train_batch, before any launch: ValueError / TypeError for what does not fit, RuntimeError for
     models or tensors off the GPU (there is no CPU path)"""
-    if pixel_values.dim() != 5 or pixel_values.shape[2] != 3:
-        raise ValueError(f"pixel_values must be [B, F, 3, H, W], got {tuple(pixel_values.shape)}")
-    if pixel_values.dtype not in (F32, torch.bfloat16):
-        raise TypeError(f"pixel_values has dtype {pixel_values.dtype}; supported: float32, bfloat16")
-    B, F, _, H, W = pixel_values.shape
+    if encode_chunk_size is not None and (int(encode_chunk_size) != encode_chunk_size or encode_chunk_size < 1):
+        raise ValueError(f"encode_chunk_size must be None or a positive number of frames, got {encode_chunk_size!r}")
+    if pixel_values.dtype == torch.uint8:
+        B, F, H, W = _check_u8_frames(pixel_values, size)
+    else:
+        if pixel_values.dim() != 5 or pixel_values.shape[2] != 3:
+            raise ValueError(f"pixel_values must be [B, F, 3, H, W], got {tuple(pixel_values.shape)}")
+        if pixel_values.dtype not in (F32, torch.bfloat16):
+            raise TypeError(f"pixel_values has dtype {pixel_values.dtype}; supported: float32, bfloat16 (uint8 with size=(H, W))")
+        B, F, _, H, W = pixel_values.shape
+        if size is not None and tuple(int(v) for v in size) != (H, W):
+            raise ValueError(f"size={tuple(size)} given for float frames of {H}x{W}; float frames are used at their own size")
     if H % 64 or W % 64:
         raise ValueError(f"frame height and width must be multiples of 64 (the UNet's latents, H/8 x W/8, need sides that are "
                          f"multiples of 8); got {H}x{W}")
@@ -114,25 +137,75 @@ def check_train_inputs(vae, image_encoder, unet_config, pixel_values, draws, con
     return B, F, H, W
 
 
+_TAPS: Dict[tuple, torch.Tensor] = {}
+
+
+def _device_taps(in_size: int, out_size: int, device) -> torch.Tensor:
+    """the resize taps of one axis on `device`, made once per (sizes, device): a step replayed from a CUDA graph reads the copy
+    its eager warm-up made"""
+    key = (in_size, out_size, str(device))
+    if key not in _TAPS:
+        _TAPS[key] = raw.resize_taps(in_size, out_size).to(device)
+    return _TAPS[key]
+
+
 def assemble_train_batch(vae, image_encoder, unet_config, pixel_values: torch.Tensor, draws: Dict[str, torch.Tensor], *,
                          conditioning_dropout_prob: Optional[float] = None, fps: int = 7, motion_bucket_id: int = 127,
-                         image_mean=CLIP_MEAN, image_std=CLIP_STD) -> Dict[str, torch.Tensor]:
+                         image_mean=CLIP_MEAN, image_std=CLIP_STD, size: Optional[Tuple[int, int]] = None,
+                         encode_chunk_size: Optional[int] = None) -> Dict[str, torch.Tensor]:
     """train_svd.py:944-1017 from the frames pixel_values [B, F, 3, H, W] (in [-1, 1]) and the step's draws (draw_train_noise) ->
     the UNet batch, the dict workload.synthetic_batch returns: sample [B, F, 8, h, w], timestep [B], encoder_hidden_states
     [B, 1, cross_dim], added_time_ids [B, 3], latents / noisy [B, F, 4, h, w] and sigmas [B, 1, 1, 1, 1], all fp32.
 
+    pixel_values may also be decoded uint8 frames [B, F, H0, W0, 3] (HWC, RGB) with the training size=(H, W): each frame is
+    resized as Pillow's Image.resize((W, H)) does (BICUBIC, 8 bits per channel) and normalised as u / 127.5 - 1, as train_svd.py's
+    DummyDataset does on the CPU, in the kernel that writes the encoder's input rows (svdx_frames_u8_in).
+
+    encode_chunk_size: None encodes the B*(F+1) frames at once; a number encodes that many frames at a time (as decode_chunk_size
+    in sampling.decode_latents), which bounds the encoder's activations. The encoder works frame by frame, so only the order of
+    its fp32 GroupNorm-statistics atomics differs.
+
     unet_config: the UNet or its config. The VAE and the image encoder run forward only. Unlike the reference, every clip's
     added_time_ids carry its own conditioning sigma, and everything before the UNet is fp32 (INTEGRATION.md §3.2)."""
-    B, F, H, W = check_train_inputs(vae, image_encoder, unet_config, pixel_values, draws, conditioning_dropout_prob)
+    B, F, H, W = check_train_inputs(vae, image_encoder, unet_config, pixel_values, draws, conditioning_dropout_prob, size,
+                                    encode_chunk_size)
     dev = pixel_values.device
     x = pixel_values.contiguous()
     cond_sigma = log_normal(draws["cond_u"], -3.0, 0.5)          # :954
     sigma = log_normal(draws["sigma_u"], 0.7, 1.6)               # :964
+    N, pad = B * (F + 1), vae.ROW_PAD
     with torch.no_grad():
-        rows = torch.empty(B * (F + 1) * H * W, vae.ROW_PAD, device=dev, dtype=torch.bfloat16)
-        raw.vae_frames_in(x, draws["cond_pixel_eps"], cond_sigma, rows, vae.ROW_PAD)
-        moments = vae._run_rows(rows, B * (F + 1), H, W)
-        emb = encode_image(image_encoder, x[:, 0], image_mean, image_std).float()      # the clean first frame (:975)
+        if x.dtype == torch.uint8:
+            taps_y, taps_x = _device_taps(x.shape[2], H, dev), _device_taps(x.shape[3], W, dev)
+            first_frames = torch.empty(B, 3, H, W, device=dev, dtype=F32)
+
+            def fill(rows, first, count):
+                raw.frames_u8_in(x, taps_y, taps_x, draws["cond_pixel_eps"], cond_sigma, rows, (H, W), first, count, first_frames, pad)
+        else:
+            first_frames = x[:, 0]
+
+            def fill(rows, first, count):
+                raw.vae_frames_in_range(x, draws["cond_pixel_eps"], cond_sigma, rows, first, count, pad)
+        if encode_chunk_size is None:
+            rows = torch.empty(N * H * W, pad, device=dev, dtype=torch.bfloat16)
+            if x.dtype == torch.uint8:
+                fill(rows, 0, N)
+            else:
+                raw.vae_frames_in(x, draws["cond_pixel_eps"], cond_sigma, rows, pad)
+            moments = vae._run_rows(rows, N, H, W)
+            del rows
+        else:
+            moments = None
+            for first in range(0, N, int(encode_chunk_size)):
+                count = min(int(encode_chunk_size), N - first)
+                rows = torch.empty(count * H * W, pad, device=dev, dtype=torch.bfloat16)
+                fill(rows, first, count)
+                m = vae._run_rows(rows, count, H, W)
+                if moments is None:
+                    moments = torch.empty((N,) + tuple(m.shape[1:]), device=dev, dtype=m.dtype)
+                moments[first:first + count].copy_(m)
+                del rows, m
+        emb = encode_image(image_encoder, first_frames, image_mean, image_std).float()      # the clean first frame (:975)
     ehs = emb.unsqueeze(1)
     if conditioning_dropout_prob is None:
         image_mask = torch.ones(B, device=dev, dtype=F32)
@@ -161,23 +234,43 @@ class VideoTrainStep:
     train.GraphedStep: opt.zero_grad -> assemble_train_batch -> UNet forward -> workload.edm_loss -> backward -> opt.step().
     cuda_graph=False runs the same function eagerly. Any optimizer of the package works (its on_updated hook should refresh the
     UNet's operands, as for any GraphedStep); `opt.lr = ...` between calls takes effect. Construction leaves the weights, the
-    optimizer's moments and step count, an attached EMA and the generator's state as they were."""
+    optimizer's moments and step count, an attached EMA and the generator's state as they were.
+
+    source_size=(H0, W0): the step takes decoded uint8 frames [B, F, H0, W0, 3] (HWC, RGB; pinned host or device memory) instead,
+    copied 1 byte per channel into a uint8 static buffer and resized on the GPU to frames_shape's H x W as Pillow's
+    Image.resize((W, H)) does (assemble_train_batch). encode_chunk_size: encode that many frames at a time (assemble_train_batch).
+
+    The graphed form keeps the snapshot it restores after the capture in pinned host memory (train.GraphedStep), which with
+    encode_chunk_size is what lets the default size of train_svd.py (25 x 576 x 1024) fit on one 80 GB card."""
 
     def __init__(self, unet, vae, image_encoder, opt, *, frames_shape, conditioning_dropout_prob: Optional[float] = None,
                  generator: Optional[torch.Generator] = None, fps: int = 7, motion_bucket_id: int = 127, image_mean=CLIP_MEAN,
-                 image_std=CLIP_STD, cuda_graph: bool = True):
+                 image_std=CLIP_STD, cuda_graph: bool = True, source_size: Optional[Tuple[int, int]] = None,
+                 encode_chunk_size: Optional[int] = None):
+        if vae.device.type != "cuda":
+            raise RuntimeError("svd_xtend_b200: VideoTrainStep only runs on a CUDA (sm_90a) device; there is no CPU fallback")
         self.unet, self.vae, self.image_encoder, self.opt = unet, vae, image_encoder, opt
         self.B, self.F, self.H, self.W = (int(v) for v in frames_shape)
         self.dropout = conditioning_dropout_prob
+        self.source_size = None if source_size is None else tuple(int(v) for v in source_size)
         self.kw = dict(conditioning_dropout_prob=conditioning_dropout_prob, fps=fps, motion_bucket_id=motion_bucket_id,
-                       image_mean=image_mean, image_std=image_std)
+                       image_mean=image_mean, image_std=image_std, encode_chunk_size=encode_chunk_size)
         dev = vae.device
         self.device = dev
+        if self.source_size is not None:
+            H0, W0 = self.source_size
+            if H0 <= 0 or W0 <= 0:
+                raise ValueError(f"source_size must be two positive sides (H0, W0), got {source_size}")
+            self.kw["size"] = (self.H, self.W)
+            frames = torch.zeros(self.B, self.F, H0, W0, 3, device=dev, dtype=torch.uint8)
+        else:
+            frames = torch.zeros(self.B, self.F, 3, self.H, self.W, device=dev, dtype=F32)
         self.generator = generator if generator is not None else torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
-        self.static = {"pixel_values": torch.zeros(self.B, self.F, 3, self.H, self.W, device=dev, dtype=F32)}
+        self.static = {"pixel_values": frames}
         gstate = self.generator.get_state()
         self.static.update(self.draw())
-        check_train_inputs(vae, image_encoder, unet, self.static["pixel_values"], self.static, conditioning_dropout_prob)
+        check_train_inputs(vae, image_encoder, unet, self.static["pixel_values"], self.static, conditioning_dropout_prob,
+                           self.kw.get("size"), encode_chunk_size)
         self.graphed = None
         if cuda_graph:
             from .train import GraphedStep
@@ -186,7 +279,8 @@ class VideoTrainStep:
                 self.generator.set_state(gstate)
                 unet.refresh_trainable_operands(shadow_current=opt.arena.shadow is not None)
 
-            self.graphed = GraphedStep(self._step, self.static, warmup=2, restore=opt.snapshot_tensors(), on_restored=restored)
+            self.graphed = GraphedStep(self._step, self.static, warmup=2, restore=opt.snapshot_tensors(), on_restored=restored,
+                                       restore_on_host=True)
         else:
             self.generator.set_state(gstate)
 
@@ -203,11 +297,24 @@ class VideoTrainStep:
         self.opt.step()
         return loss.detach()
 
-    def __call__(self, pixel_values: torch.Tensor) -> torch.Tensor:
+    def check_frames(self, pixel_values: torch.Tensor) -> None:
+        """ValueError / TypeError unless pixel_values is what this step was built for"""
+        if self.source_size is not None:
+            want = (self.B, self.F) + self.source_size + (3,)
+            if pixel_values.dtype != torch.uint8:
+                raise TypeError(f"VideoTrainStep was built for uint8 frames (source_size), got dtype {pixel_values.dtype}")
+            if pixel_values.dim() == 5 and pixel_values.shape[-1] != 3:
+                raise ValueError(f"uint8 frames must have 3 (RGB) channels, last dimension of {tuple(pixel_values.shape)}")
+            if tuple(pixel_values.shape) != want:
+                raise ValueError(f"VideoTrainStep was built for uint8 frames {want}, got {tuple(pixel_values.shape)}")
+            return
         if tuple(pixel_values.shape) != (self.B, self.F, 3, self.H, self.W):
             raise ValueError(f"VideoTrainStep was built for frames {(self.B, self.F, 3, self.H, self.W)}, got {tuple(pixel_values.shape)}")
         if pixel_values.dtype not in (F32, torch.bfloat16):
             raise TypeError(f"pixel_values has dtype {pixel_values.dtype}; supported: float32, bfloat16")
+
+    def __call__(self, pixel_values: torch.Tensor) -> torch.Tensor:
+        self.check_frames(pixel_values)
         self.static["pixel_values"].copy_(pixel_values, non_blocking=True)
         for k, v in self.draw().items():
             self.static[k].copy_(v)
