@@ -380,6 +380,24 @@ int svdx_adamw_graph(float* p, const float* g, float* m, float* v, int64_t n, fl
 int svdx_adamw_p2p(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world,
                    int64_t lo, int64_t n, float* state, float grad_scale, int32_t tick, void* stream);
 
+/* Global gradient norm for clipping (torch.nn.utils.clip_grad_norm_ with norm type 2: train_svd.py's --max_grad_norm,
+ * :468-470, :1044-1049), computed and applied on the device so that a captured step clips without a host sync.
+ * sumsq: DEVICE double[1 + 1024]; sumsq[0] receives the result, sumsq[1 ..] is the per-block scratch of the first stage.
+ * svdx_grad_sumsq: sumsq[0] = sum over i < n of (double)g[i]^2 (g 16-byte aligned: the gradient arena or a slice of it). The
+ * partition over blocks depends on n only, the partials are fp64 and a second one-block kernel sums them in index order:
+ * identical bits for the same input, launch after launch and replay after replay. Two launches, no host access.
+ * svdx_grad_sumsq_p2p: the same over the slice [lo, lo + n) of the rank-order sum of grads[0 .. world) (svdx_adamw_p2p's
+ * peer-mapped arenas, summed exactly as that kernel sums them, up to four ranks' loads in flight), so the norm is that of the
+ * gradient svdx_adamw_p2p applies. lo and n multiples of 4. Two launches.
+ * svdx_clip_coef: one thread. From sumsq[0], a DEVICE max_norm and the host scale (1 / world under the sharded optimizers, so
+ * the norm is that of the mean gradient), writes the DEVICE pair out = {total_norm, coef}:
+ *   total_norm = fl(fl(sqrt(sumsq[0])) * scale),  coef = min(max_norm / (total_norm + 1e-6f), 1)
+ * in fp32 with torch's roundings (the division is reciprocal, then multiply). The clamp propagates NaN as torch.clamp does; an
+ * infinite norm gives coef = 0. Pass out + 1 as grad_mul of the update. */
+int svdx_grad_sumsq(const float* g, int64_t n, double* sumsq, void* stream);
+int svdx_grad_sumsq_p2p(const void* const* grads, int32_t world, int64_t lo, int64_t n, double* sumsq, void* stream);
+int svdx_clip_coef(const double* sumsq, const float* max_norm, float scale, float* out, void* stream);
+
 /* Exponential moving average of the weights (train_svd.py:676-679 EMAModel, :1053-1054 ema_unet.step(unet.parameters())
  * -> [D] diffusers.training_utils.EMAModel.step: get_decay on the host, then per parameter tensor
  * s.sub_((1 - d) * (s - p)) if p.requires_grad else s.copy_(p)).
@@ -419,6 +437,25 @@ int svdx_adamw8bit(const void* jobs, const int32_t* block_prefix, int32_t njobs,
  * (svdx_adamw_graph_ema's rule; the tick also advances ema_state). Two launches. */
 int svdx_adamw8bit_ema(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
                        const float* qmap2, float* state, float grad_scale, double* ema_state, void* stream);
+
+/* The six update entry points above with one more, trailing argument grad_mul (before the stream): a DEVICE float the
+ * gradient is also scaled by, read by the update kernel, so the applied gradient is g * (grad_scale * grad_mul[0]); at
+ * grad_scale = 1 that is g * grad_mul[0], the product torch's in-place g.mul_(coef) gives. grad_mul NULL is the entry point
+ * without the suffix, bit for bit. Gradient clipping passes out + 1 of svdx_clip_coef, so the clip is decided on the device and
+ * a captured step needs no host sync. Every other argument and the launches are those of the form without the suffix. */
+int svdx_adamw_graph_mul(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
+                         void* shadow_bf16, const float* grad_mul, void* stream);
+int svdx_adamw_graph_ema_mul(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
+                             void* shadow_bf16, float* ema, double* ema_state, const float* grad_mul, void* stream);
+int svdx_adamw_p2p_mul(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world,
+                       int64_t lo, int64_t n, float* state, float grad_scale, int32_t tick, const float* grad_mul, void* stream);
+int svdx_adamw_p2p_ema_mul(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world,
+                           int64_t lo, int64_t n, float* state, float grad_scale, int32_t tick, float* ema, double* ema_state,
+                           const float* grad_mul, void* stream);
+int svdx_adamw8bit_mul(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
+                       const float* qmap2, float* state, float grad_scale, const float* grad_mul, void* stream);
+int svdx_adamw8bit_ema_mul(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
+                           const float* qmap2, float* state, float grad_scale, double* ema_state, const float* grad_mul, void* stream);
 
 /* Batch assembly of a training step from video frames (train_svd.py:942-1017; svd_xtend_b200.video_train). Every operation is
  * rounded separately (no FMA), in the reference's order.

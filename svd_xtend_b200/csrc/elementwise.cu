@@ -571,10 +571,11 @@ SVDX_DEVINL void adamw_update4(const AdamCoef& c, float4 g4, float gscale, float
 template <bool EMA>
 __global__ void adamw_state_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, long long n4,
                                    long long n, const float* __restrict__ state, float gscale, bf16* __restrict__ shadow,
-                                   float* __restrict__ ema, const double* __restrict__ ema_state) {
+                                   float* __restrict__ ema, const double* __restrict__ ema_state, const float* __restrict__ gmul) {
   const long long i4 = gtid();
   if (i4 >= n4) return;
   const AdamCoef c = adamw_coef(state);
+  if (gmul) gscale *= *gmul;
   const long long i = i4 * 4;
   if (i + 3 < n) {
     float pp[4];
@@ -607,8 +608,10 @@ struct AdamP2P {
 template <bool EMA>
 __global__ void __launch_bounds__(256) adamw_p2p_kernel(float* __restrict__ p, float* __restrict__ m, float* __restrict__ v, const __grid_constant__ AdamP2P ptr,
                                                         int world, long long lo, long long n4, const float* __restrict__ state, float gscale,
-                                                        float* __restrict__ ema, const double* __restrict__ ema_state) {
+                                                        float* __restrict__ ema, const double* __restrict__ ema_state,
+                                                        const float* __restrict__ gmul) {
   const AdamCoef c = adamw_coef(state);
+  if (gmul) gscale *= *gmul;
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long i4 = gtid(); i4 < n4; i4 += stride) {
     const long long i = i4 * 4;
@@ -632,6 +635,110 @@ __global__ void __launch_bounds__(256) adamw_p2p_kernel(float* __restrict__ p, f
       *reinterpret_cast<float4*>(ema + i) = ema_update4(*reinterpret_cast<float4*>(ema + i), pp, (float)ema_state[8]);
   }
   __threadfence_system();     // the peer stores are performed system-wide before this kernel counts as complete
+}
+
+// Global gradient norm for clipping (torch.nn.utils.clip_grad_norm_, the --max_grad_norm of train_svd.py:468-470, :1044-1049).
+// The sum of squares is deterministic: the partition of the float4 index space over SUMSQ_THREADS-thread blocks depends on n
+// only, every thread sums its squares in fp64 in a fixed order, each block reduces in a fixed tree into partials[block], and a
+// second one-block kernel sums the partials in index order. The same input gives the same bits, launch after launch.
+constexpr int SUMSQ_THREADS = 256;
+constexpr int SUMSQ_PARTIALS = 1024;     // at most this many blocks; sumsq = double[1 + SUMSQ_PARTIALS] (svd_xtend_b200.h)
+constexpr int SUMSQ_UNROLL = 4;          // independent 16-byte loads in flight per thread
+
+static inline unsigned sumsq_blocks(long long n4) {
+  const long long b = (n4 + SUMSQ_THREADS * 8 - 1) / (SUMSQ_THREADS * 8);
+  return (unsigned)(b < 1 ? 1 : (b > SUMSQ_PARTIALS ? SUMSQ_PARTIALS : b));
+}
+
+SVDX_DEVINL double sq4(float4 g) {
+  return (double)g.x * g.x + (double)g.y * g.y + (double)g.z * g.z + (double)g.w * g.w;
+}
+
+// fixed-order sum over the block; thread 0 holds the result
+SVDX_DEVINL double block_sum_f64(double v) {
+  __shared__ double part[SUMSQ_THREADS / 32];
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    v = part[0];
+#pragma unroll
+    for (int w = 1; w < SUMSQ_THREADS / 32; ++w) v += part[w];
+  }
+  return v;
+}
+
+// float4 number i4 of the gradient: one arena, or (P2P) the rank-order sum of every rank's slice [lo, lo + 4 n4), summed as
+// adamw_p2p_kernel sums it, so the norm is that of the gradient the update applies
+struct GradSrc {
+  const float* grad[16];
+  int world;
+  long long lo;
+};
+template <bool P2P>
+SVDX_DEVINL float4 grad_load4(const GradSrc& s, long long i4) {
+  if constexpr (!P2P) {
+    return __ldcs(reinterpret_cast<const float4*>(s.grad[0]) + i4);
+  } else {
+    const long long i = s.lo + i4 * 4;
+    float4 g4 = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 1
+    for (int r0 = 0; r0 < s.world; r0 += 4) {
+      float4 t[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        if (r0 + k < s.world) t[k] = __ldcg(reinterpret_cast<const float4*>(s.grad[r0 + k] + i));
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        if (r0 + k < s.world) { g4.x += t[k].x; g4.y += t[k].y; g4.z += t[k].z; g4.w += t[k].w; }
+    }
+    return g4;
+  }
+}
+
+// partials[blockIdx.x] = the block's sum of squares over float4 indices [0, n4) and (non-P2P, thread 0) the n % 4 tail
+template <bool P2P>
+__global__ void __launch_bounds__(SUMSQ_THREADS) grad_sumsq_kernel(const __grid_constant__ GradSrc src, long long n4, int tail,
+                                                                   double* __restrict__ partials) {
+  const long long stride = (long long)gridDim.x * SUMSQ_THREADS;
+  long long i4 = gtid();
+  double acc = 0.0;
+  for (; i4 + (SUMSQ_UNROLL - 1) * stride < n4; i4 += SUMSQ_UNROLL * stride) {
+    float4 g[SUMSQ_UNROLL];
+#pragma unroll
+    for (int k = 0; k < SUMSQ_UNROLL; ++k) g[k] = grad_load4<P2P>(src, i4 + k * stride);
+#pragma unroll
+    for (int k = 0; k < SUMSQ_UNROLL; ++k) acc += sq4(g[k]);
+  }
+  for (; i4 < n4; i4 += stride) acc += sq4(grad_load4<P2P>(src, i4));
+  if (!P2P && tail && gtid() == 0)
+    for (int k = 0; k < tail; ++k) {
+      const double x = src.grad[0][n4 * 4 + k];
+      acc += x * x;
+    }
+  acc = block_sum_f64(acc);
+  if (threadIdx.x == 0) partials[blockIdx.x] = acc;
+}
+
+// sumsq[0] = sum of partials[0 .. nparts) in a fixed order (thread t: parts t, t + 256, ..., then the block tree)
+__global__ void __launch_bounds__(SUMSQ_THREADS) sumsq_finish_kernel(const double* __restrict__ partials, int nparts,
+                                                                     double* __restrict__ sumsq) {
+  double acc = 0.0;
+  for (int k = threadIdx.x; k < nparts; k += SUMSQ_THREADS) acc += partials[k];
+  acc = block_sum_f64(acc);
+  if (threadIdx.x == 0) sumsq[0] = acc;
+}
+
+// out = {total_norm, coef}: total_norm = fl(fl(sqrt(sumsq)) * scale), coef = min(max_norm / (total_norm + 1e-6), 1) with
+// torch's roundings (a Python scalar over a tensor is reciprocal() * scalar in torch). The clamp keeps a NaN coefficient, as
+// torch.clamp does (fminf would return 1 and silently skip the clip of a NaN gradient); an infinite norm gives 0.
+__global__ void clip_coef_kernel(const double* __restrict__ sumsq, const float* __restrict__ max_norm, float scale,
+                                 float* __restrict__ out) {
+  const float total = __fmul_rn((float)sqrt(sumsq[0]), scale);
+  const float coef = __fmul_rn(__frcp_rn(__fadd_rn(total, 1e-6f)), max_norm[0]);
+  out[0] = total;
+  out[1] = coef > 1.f ? 1.f : coef;
 }
 
 // EMAModel.step over many (shadow, parameter) pairs in ONE launch: block -> (job, chunk) through a block prefix table (the
@@ -700,8 +807,10 @@ SVDX_DEVINL int a8_code(const float* mid, float x) {
 template <bool EMA>
 __global__ void __launch_bounds__(256) adamw8bit_kernel(const Adam8Job* __restrict__ jobs, const int* __restrict__ block_prefix, int njobs,
                                                         int total_blocks, const float* __restrict__ qmap1, const float* __restrict__ qmap2,
-                                                        const float* __restrict__ state, float gscale, const double* __restrict__ ema_state) {
+                                                        const float* __restrict__ state, float gscale, const double* __restrict__ ema_state,
+                                                        const float* __restrict__ gmul) {
   __shared__ float q1[256], q2[256], mid1[256], mid2[256];
+  if (gmul) gscale = __fmul_rn(gscale, *gmul);
   for (int k = threadIdx.x; k < 256; k += blockDim.x) {
     q1[k] = qmap1[k];
     q2[k] = qmap2[k];
@@ -1358,21 +1467,26 @@ extern "C" int svdx_blend_scales(const float* mix_factor, float* out3, void* str
   return SVDX_OK;
 }
 
-extern "C" int svdx_adamw_graph(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
-                                void* shadow_bf16, void* stream) {
+extern "C" int svdx_adamw_graph_mul(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
+                                    void* shadow_bf16, const float* grad_mul, void* stream) {
   if (!p || !g || !m || !v || !state || n <= 0 || (reinterpret_cast<uintptr_t>(p) & 15) || (reinterpret_cast<uintptr_t>(g) & 15) ||
       (reinterpret_cast<uintptr_t>(m) & 15) || (reinterpret_cast<uintptr_t>(v) & 15) || (reinterpret_cast<uintptr_t>(shadow_bf16) & 7))
     return svdx_fail(SVDX_E_BADARG, "adamw_graph: bad arguments (16-byte aligned flat buffers, device state[8])");
   adamw_tick_kernel<<<1, 1, 0, ST(stream)>>>(state);
   const long long n4 = (n + 3) / 4;
   adamw_state_kernel<false><<<nblocks(n4), 256, 0, ST(stream)>>>(p, g, m, v, n4, n, state, grad_scale, reinterpret_cast<bf16*>(shadow_bf16),
-                                                                 nullptr, nullptr);
+                                                                 nullptr, nullptr, grad_mul);
   SVDX_CHECK_LAUNCH("adamw_graph");
   return SVDX_OK;
 }
 
-extern "C" int svdx_adamw_graph_ema(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
-                                    void* shadow_bf16, float* ema, double* ema_state, void* stream) {
+extern "C" int svdx_adamw_graph(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
+                                void* shadow_bf16, void* stream) {
+  return svdx_adamw_graph_mul(p, g, m, v, n, state, grad_scale, shadow_bf16, nullptr, stream);
+}
+
+extern "C" int svdx_adamw_graph_ema_mul(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
+                                        void* shadow_bf16, float* ema, double* ema_state, const float* grad_mul, void* stream) {
   if (!p || !g || !m || !v || !state || !ema || !ema_state || n <= 0 || (reinterpret_cast<uintptr_t>(p) & 15) ||
       (reinterpret_cast<uintptr_t>(g) & 15) || (reinterpret_cast<uintptr_t>(m) & 15) || (reinterpret_cast<uintptr_t>(v) & 15) ||
       (reinterpret_cast<uintptr_t>(ema) & 15) || (reinterpret_cast<uintptr_t>(ema_state) & 7) || (reinterpret_cast<uintptr_t>(shadow_bf16) & 7))
@@ -1380,9 +1494,14 @@ extern "C" int svdx_adamw_graph_ema(float* p, const float* g, float* m, float* v
   adamw_ema_tick_kernel<<<1, 1, 0, ST(stream)>>>(state, ema_state);
   const long long n4 = (n + 3) / 4;
   adamw_state_kernel<true><<<nblocks(n4), 256, 0, ST(stream)>>>(p, g, m, v, n4, n, state, grad_scale, reinterpret_cast<bf16*>(shadow_bf16),
-                                                                ema, ema_state);
+                                                                ema, ema_state, grad_mul);
   SVDX_CHECK_LAUNCH("adamw_graph_ema");
   return SVDX_OK;
+}
+
+extern "C" int svdx_adamw_graph_ema(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
+                                    void* shadow_bf16, float* ema, double* ema_state, void* stream) {
+  return svdx_adamw_graph_ema_mul(p, g, m, v, n, state, grad_scale, shadow_bf16, ema, ema_state, nullptr, stream);
 }
 
 extern "C" int svdx_ema_multi(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, double* ema_state,
@@ -1396,7 +1515,8 @@ extern "C" int svdx_ema_multi(const void* jobs, const int32_t* block_prefix, int
 }
 
 static int adamw8bit_launch(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
-                            const float* qmap2, float* state, float grad_scale, double* ema_state, bool ema, void* stream) {
+                            const float* qmap2, float* state, float grad_scale, double* ema_state, bool ema, const float* grad_mul,
+                            void* stream) {
   if (!jobs || !block_prefix || !qmap1 || !qmap2 || !state || njobs <= 0 || total_blocks <= 0 || (reinterpret_cast<uintptr_t>(jobs) & 7) ||
       (reinterpret_cast<uintptr_t>(block_prefix) & 3) || (reinterpret_cast<uintptr_t>(qmap1) & 3) ||
       (reinterpret_cast<uintptr_t>(qmap2) & 3) || (reinterpret_cast<uintptr_t>(state) & 3) ||
@@ -1409,10 +1529,12 @@ static int adamw8bit_launch(const void* jobs, const int32_t* block_prefix, int32
   const Adam8Job* j = reinterpret_cast<const Adam8Job*>(jobs);
   if (ema) {
     adamw_ema_tick_kernel<<<1, 1, 0, ST(stream)>>>(state, ema_state);
-    adamw8bit_kernel<true><<<(unsigned)blocks, 256, 0, ST(stream)>>>(j, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, ema_state);
+    adamw8bit_kernel<true><<<(unsigned)blocks, 256, 0, ST(stream)>>>(j, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, ema_state,
+                                                                      grad_mul);
   } else {
     adamw_tick_kernel<<<1, 1, 0, ST(stream)>>>(state);
-    adamw8bit_kernel<false><<<(unsigned)blocks, 256, 0, ST(stream)>>>(j, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, nullptr);
+    adamw8bit_kernel<false><<<(unsigned)blocks, 256, 0, ST(stream)>>>(j, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, nullptr,
+                                                                       grad_mul);
   }
   SVDX_CHECK_LAUNCH(ema ? "adamw8bit_ema" : "adamw8bit");
   return SVDX_OK;
@@ -1420,16 +1542,28 @@ static int adamw8bit_launch(const void* jobs, const int32_t* block_prefix, int32
 
 extern "C" int svdx_adamw8bit(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
                               const float* qmap2, float* state, float grad_scale, void* stream) {
-  return adamw8bit_launch(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, nullptr, false, stream);
+  return adamw8bit_launch(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, nullptr, false, nullptr, stream);
+}
+
+extern "C" int svdx_adamw8bit_mul(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
+                                  const float* qmap2, float* state, float grad_scale, const float* grad_mul, void* stream) {
+  return adamw8bit_launch(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, nullptr, false, grad_mul, stream);
 }
 
 extern "C" int svdx_adamw8bit_ema(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
                                   const float* qmap2, float* state, float grad_scale, double* ema_state, void* stream) {
-  return adamw8bit_launch(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, ema_state, true, stream);
+  return adamw8bit_launch(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, ema_state, true, nullptr, stream);
+}
+
+extern "C" int svdx_adamw8bit_ema_mul(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks,
+                                      const float* qmap1, const float* qmap2, float* state, float grad_scale, double* ema_state,
+                                      const float* grad_mul, void* stream) {
+  return adamw8bit_launch(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, ema_state, true, grad_mul, stream);
 }
 
 static int adamw_p2p_launch(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo, int64_t n,
-                            float* state, float grad_scale, int32_t tick, float* ema, double* ema_state, void* stream) {
+                            float* state, float grad_scale, int32_t tick, float* ema, double* ema_state, const float* grad_mul,
+                            void* stream) {
   if (!p || !m || !v || !grads || !shadows || !state || world < 1 || world > 16 || n <= 0 || n % 4 || lo % 4 ||
       (reinterpret_cast<uintptr_t>(p) & 15) || (reinterpret_cast<uintptr_t>(m) & 15) || (reinterpret_cast<uintptr_t>(v) & 15))
     return svdx_fail(SVDX_E_BADARG, "adamw_p2p: bad arguments (world <= 16, slice offset / length multiples of 4, 16-byte aligned buffers)");
@@ -1450,22 +1584,75 @@ static int adamw_p2p_launch(float* p, float* m, float* v, const void* const* gra
   long long blocks = (n4 + 255) / 256;
   const long long cap = (long long)svdx_num_sms() * 8;
   if (blocks > cap) blocks = cap;
-  if (ema) adamw_p2p_kernel<true><<<(unsigned)blocks, 256, 0, ST(stream)>>>(p, m, v, ptr, world, lo, n4, state, grad_scale, ema, ema_state);
-  else adamw_p2p_kernel<false><<<(unsigned)blocks, 256, 0, ST(stream)>>>(p, m, v, ptr, world, lo, n4, state, grad_scale, nullptr, nullptr);
+  if (ema) adamw_p2p_kernel<true><<<(unsigned)blocks, 256, 0, ST(stream)>>>(p, m, v, ptr, world, lo, n4, state, grad_scale, ema, ema_state,
+                                                                                  grad_mul);
+  else adamw_p2p_kernel<false><<<(unsigned)blocks, 256, 0, ST(stream)>>>(p, m, v, ptr, world, lo, n4, state, grad_scale, nullptr,
+                                                                                   nullptr, grad_mul);
   SVDX_CHECK_LAUNCH("adamw_p2p");
   return SVDX_OK;
 }
 
 extern "C" int svdx_adamw_p2p(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo, int64_t n,
                               float* state, float grad_scale, int32_t tick, void* stream) {
-  return adamw_p2p_launch(p, m, v, grads, shadows, world, lo, n, state, grad_scale, tick, nullptr, nullptr, stream);
+  return adamw_p2p_launch(p, m, v, grads, shadows, world, lo, n, state, grad_scale, tick, nullptr, nullptr, nullptr, stream);
+}
+
+extern "C" int svdx_adamw_p2p_mul(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo,
+                                  int64_t n, float* state, float grad_scale, int32_t tick, const float* grad_mul, void* stream) {
+  return adamw_p2p_launch(p, m, v, grads, shadows, world, lo, n, state, grad_scale, tick, nullptr, nullptr, grad_mul, stream);
+}
+
+extern "C" int svdx_adamw_p2p_ema_mul(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world,
+                                      int64_t lo, int64_t n, float* state, float grad_scale, int32_t tick, float* ema, double* ema_state,
+                                      const float* grad_mul, void* stream) {
+  if (!ema || !ema_state || (reinterpret_cast<uintptr_t>(ema) & 15) || (reinterpret_cast<uintptr_t>(ema_state) & 7))
+    return svdx_fail(SVDX_E_BADARG, "adamw_p2p_ema: null / misaligned EMA slice or ema_state[9]");
+  return adamw_p2p_launch(p, m, v, grads, shadows, world, lo, n, state, grad_scale, tick, ema, ema_state, grad_mul, stream);
 }
 
 extern "C" int svdx_adamw_p2p_ema(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo,
                                   int64_t n, float* state, float grad_scale, int32_t tick, float* ema, double* ema_state, void* stream) {
-  if (!ema || !ema_state || (reinterpret_cast<uintptr_t>(ema) & 15) || (reinterpret_cast<uintptr_t>(ema_state) & 7))
-    return svdx_fail(SVDX_E_BADARG, "adamw_p2p_ema: null / misaligned EMA slice or ema_state[9]");
-  return adamw_p2p_launch(p, m, v, grads, shadows, world, lo, n, state, grad_scale, tick, ema, ema_state, stream);
+  return svdx_adamw_p2p_ema_mul(p, m, v, grads, shadows, world, lo, n, state, grad_scale, tick, ema, ema_state, nullptr, stream);
+}
+
+static int grad_sumsq_launch(const GradSrc& src, bool p2p, long long n4, int tail, double* sumsq, void* stream) {
+  const unsigned blocks = sumsq_blocks(n4);
+  if (p2p) grad_sumsq_kernel<true><<<blocks, SUMSQ_THREADS, 0, ST(stream)>>>(src, n4, tail, sumsq + 1);
+  else grad_sumsq_kernel<false><<<blocks, SUMSQ_THREADS, 0, ST(stream)>>>(src, n4, tail, sumsq + 1);
+  sumsq_finish_kernel<<<1, SUMSQ_THREADS, 0, ST(stream)>>>(sumsq + 1, (int)blocks, sumsq);
+  SVDX_CHECK_LAUNCH(p2p ? "grad_sumsq_p2p" : "grad_sumsq");
+  return SVDX_OK;
+}
+
+extern "C" int svdx_grad_sumsq(const float* g, int64_t n, double* sumsq, void* stream) {
+  if (!g || !sumsq || n <= 0 || (reinterpret_cast<uintptr_t>(g) & 15) || (reinterpret_cast<uintptr_t>(sumsq) & 7))
+    return svdx_fail(SVDX_E_BADARG, "grad_sumsq: bad arguments (16-byte aligned fp32 gradient, n > 0, device double[1025])");
+  GradSrc src{};
+  src.grad[0] = g;
+  src.world = 1;
+  return grad_sumsq_launch(src, false, n / 4, (int)(n % 4), sumsq, stream);
+}
+
+extern "C" int svdx_grad_sumsq_p2p(const void* const* grads, int32_t world, int64_t lo, int64_t n, double* sumsq, void* stream) {
+  if (!grads || !sumsq || world < 1 || world > 16 || n <= 0 || n % 4 || lo < 0 || lo % 4 || (reinterpret_cast<uintptr_t>(sumsq) & 7))
+    return svdx_fail(SVDX_E_BADARG, "grad_sumsq_p2p: bad arguments (world <= 16, slice offset / length multiples of 4, double[1025])");
+  GradSrc src{};
+  for (int r = 0; r < world; ++r) {
+    if (!grads[r] || (reinterpret_cast<uintptr_t>(grads[r]) & 15)) return svdx_fail(SVDX_E_BADARG, "grad_sumsq_p2p: null / misaligned peer arena");
+    src.grad[r] = reinterpret_cast<const float*>(grads[r]);
+  }
+  src.world = world;
+  src.lo = lo;
+  return grad_sumsq_launch(src, true, n / 4, 0, sumsq, stream);
+}
+
+extern "C" int svdx_clip_coef(const double* sumsq, const float* max_norm, float scale, float* out, void* stream) {
+  if (!sumsq || !max_norm || !out || (reinterpret_cast<uintptr_t>(sumsq) & 7) || (reinterpret_cast<uintptr_t>(max_norm) & 3) ||
+      (reinterpret_cast<uintptr_t>(out) & 3))
+    return svdx_fail(SVDX_E_BADARG, "clip_coef: bad arguments (device double sumsq, float max_norm, float[2] out)");
+  clip_coef_kernel<<<1, 1, 0, ST(stream)>>>(sumsq, max_norm, scale, out);
+  SVDX_CHECK_LAUNCH("clip_coef");
+  return SVDX_OK;
 }
 
 extern "C" int svdx_multi_transpose(const void* src_base, const void* jobs, const int32_t* tile_prefix, int32_t njobs, int32_t total_tiles,

@@ -84,6 +84,13 @@ def _neg_taps(taps):
     return tuple((-a, -b, -c) for a, b, c in taps)
 
 
+def _copy_taps(dst: torch.Tensor, src: torch.Tensor, sel: Sequence[int]) -> None:
+    """dst[:, j, :] = src[:, sel[j], :] by plain slices: an index list would be copied to the device as a pageable tensor, which
+    a captured refresh of the trainable operands (enable_cuda_graphs) cannot do"""
+    for j, t in enumerate(sel):
+        dst[:, j, :].copy_(src[:, t, :])
+
+
 class WeightCache:
     """bf16 operand layouts of the (fp32 or bf16) master parameters.
 
@@ -670,7 +677,7 @@ class Engine:
                         for pl in range(4):
                             sel = [t for t in range(9) if taps[t][2] == pl * nimg]
                             wsub = self.wc.get(("convT_plane", id(w), pl), [w], (I, len(sel) * O),
-                                               lambda buf, sel=sel: buf.view(I, len(sel), O).copy_(wt3[:, sel, :]))
+                                               lambda buf, sel=sel: _copy_taps(buf.view(I, len(sel), O), wt3, sel))
                             tp = tuple((-taps[t][0], -taps[t][1], 0) for t in sel)
                             raw.tapgemm(dy, wsub, dx[pl * M:(pl + 1) * M], M=M, N=I, K=O, mode=A_CONV2D, taps=tp,
                                         conv_whn=(g.W, g.H, nimg), scales=sc)

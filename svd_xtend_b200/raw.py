@@ -29,7 +29,9 @@ def dtype_code(t: torch.Tensor, what: str) -> int:
 LAUNCHES = [0]
 _KERNELS_PER_CALL = {"svdx_groupnorm_apply_fused": 1, "svdx_attention_bwd": 3, "svdx_adamw_graph": 2, "svdx_adamw_p2p": 2,
                      "svdx_adamw_graph_ema": 2, "svdx_adamw_p2p_ema": 2, "svdx_ema_multi": 2, "svdx_adamw8bit": 2,
-                     "svdx_adamw8bit_ema": 2}
+                     "svdx_adamw8bit_ema": 2, "svdx_adamw_graph_mul": 2, "svdx_adamw_graph_ema_mul": 2, "svdx_adamw8bit_mul": 2,
+                     "svdx_adamw8bit_ema_mul": 2, "svdx_adamw_p2p_mul": 2, "svdx_adamw_p2p_ema_mul": 2, "svdx_grad_sumsq": 2,
+                     "svdx_grad_sumsq_p2p": 2}
 
 
 def check(rc: int, what: str = "") -> None:
@@ -841,39 +843,87 @@ def _ema_args(ema, ema_state, n):
         raise ValueError("ema: fp32 buffer of the updated slice's length; ema_state: float64[9] (svd_xtend_b200.h)")
 
 
-def adamw_p2p(p, m, v, peer_grads, peer_shadows, lo, state, grad_scale, tick=True, ema=None, ema_state=None):
+def _grad_mul(grad_mul) -> Optional[int]:
+    """device address of the update's gradient multiplier (svd_xtend_b200.h, the *_mul entry points), None without one"""
+    if grad_mul is None:
+        return None
+    if grad_mul.dtype != torch.float32 or grad_mul.numel() < 1 or not grad_mul.is_cuda:
+        raise ValueError("grad_mul: a device float32 tensor (the first element multiplies the gradient)")
+    return grad_mul.data_ptr()
+
+
+def adamw_p2p(p, m, v, peer_grads, peer_shadows, lo, state, grad_scale, tick=True, ema=None, ema_state=None, grad_mul=None):
     """reduce-scatter + AdamW + all-gather in one kernel over NVLink peer memory (svdx_adamw_p2p): p / m / v are this rank's
     slices, peer_grads / peer_shadows the FULL arenas of every rank (this rank's own included) as tensors mapped into this
     process (train.map_peer_buffers). With `ema` (this rank's fp32 EMA slice) and `ema_state` the same launch also advances
-    the EMA of the updated masters (svdx_adamw_p2p_ema)."""
+    the EMA of the updated masters (svdx_adamw_p2p_ema). grad_mul: a device fp32 scalar the gradient is also multiplied by
+    (the clip coefficient; svdx_adamw_p2p_mul / svdx_adamw_p2p_ema_mul)."""
     world = len(peer_grads)
     n = p.numel()
     _ema_args(ema, ema_state, n)
+    gm = _grad_mul(grad_mul)
     if _fam("adamw", 0.0, (4.0 * world + 28.0 + 2.0 * world + (8.0 if ema is not None else 0.0)) * n):
         return
     ga = (C.c_void_p * world)(*[t if isinstance(t, int) else t.data_ptr() for t in peer_grads])       # tensors or mapped addresses
     sa = (C.c_void_p * world)(*[t if isinstance(t, int) else t.data_ptr() for t in peer_shadows])
+    args = (p.data_ptr(), m.data_ptr(), v.data_ptr(), ga, sa, world, lo, n, state.data_ptr(), float(grad_scale), int(tick))
     if ema is not None:
-        check(load().svdx_adamw_p2p_ema(p.data_ptr(), m.data_ptr(), v.data_ptr(), ga, sa, world, lo, n, state.data_ptr(), float(grad_scale),
-                                        int(tick), ema.data_ptr(), ema_state.data_ptr(), _stream()), "svdx_adamw_p2p_ema")
-        return
-    check(load().svdx_adamw_p2p(p.data_ptr(), m.data_ptr(), v.data_ptr(), ga, sa, world, lo, n, state.data_ptr(), float(grad_scale),
-                                int(tick), _stream()), "svdx_adamw_p2p")
+        args += (ema.data_ptr(), ema_state.data_ptr())
+    name = "svdx_adamw_p2p" + ("_ema" if ema is not None else "") + ("_mul" if gm is not None else "")
+    check(getattr(load(), name)(*args, *(() if gm is None else (gm,)), _stream()), name)
 
 
-def adamw_graph(p, g, m, v, state, grad_scale=1.0, shadow=None, ema=None, ema_state=None):
+def adamw_graph(p, g, m, v, state, grad_scale=1.0, shadow=None, ema=None, ema_state=None, grad_mul=None):
     """CUDA-graph-safe AdamW: lr / betas / eps / weight decay / step / bias corrections live in the device float[8] `state`.
     With `ema` (fp32, same length as p) and `ema_state` (device float64[9]) the update also advances the EMA of the new
-    masters at the same offsets (svdx_adamw_graph_ema)."""
+    masters at the same offsets (svdx_adamw_graph_ema). grad_mul: a device fp32 scalar the gradient is also multiplied by
+    (the clip coefficient; svdx_adamw_graph_mul / svdx_adamw_graph_ema_mul)."""
     _ema_args(ema, ema_state, p.numel())
+    gm = _grad_mul(grad_mul)
     if _fam("adamw", 0.0, ((30.0 if shadow is not None else 28.0) + (8.0 if ema is not None else 0.0)) * p.numel()):
         return
+    args = (p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(), state.data_ptr(), grad_scale, _ptr(shadow))
     if ema is not None:
-        check(load().svdx_adamw_graph_ema(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(), state.data_ptr(), grad_scale,
-                                          _ptr(shadow), ema.data_ptr(), ema_state.data_ptr(), _stream()), "svdx_adamw_graph_ema")
+        args += (ema.data_ptr(), ema_state.data_ptr())
+    name = "svdx_adamw_graph" + ("_ema" if ema is not None else "") + ("_mul" if gm is not None else "")
+    check(getattr(load(), name)(*args, *(() if gm is None else (gm,)), _stream()), name)
+
+
+SUMSQ_PARTIALS = 1024   # per-block partials of svdx_grad_sumsq: its sumsq buffer is float64[1 + SUMSQ_PARTIALS]
+
+
+def _sumsq_buf(sumsq):
+    if sumsq.dtype != torch.float64 or sumsq.numel() < 1 + SUMSQ_PARTIALS or not sumsq.is_contiguous():
+        raise ValueError(f"sumsq: a contiguous device float64[{1 + SUMSQ_PARTIALS}] (result in [0], block partials after it)")
+
+
+def grad_sumsq(g, sumsq):
+    """sumsq[0] = sum of g[i]^2 in fp64 over the flat fp32 gradient g (svdx_grad_sumsq: deterministic, graph-safe)"""
+    _sumsq_buf(sumsq)
+    if g.dtype != torch.float32 or not g.is_contiguous():
+        raise ValueError("grad_sumsq: a contiguous fp32 gradient")
+    if _fam("adamw", 0.0, 4.0 * g.numel()):
         return
-    check(load().svdx_adamw_graph(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(), state.data_ptr(), grad_scale,
-                                  _ptr(shadow), _stream()), "svdx_adamw_graph")
+    check(load().svdx_grad_sumsq(g.data_ptr(), g.numel(), sumsq.data_ptr(), _stream()), "svdx_grad_sumsq")
+
+
+def grad_sumsq_p2p(peer_grads, lo, n, sumsq):
+    """sumsq[0] = sum of squares over [lo, lo + n) of the rank-order sum of every rank's gradient arena (svdx_grad_sumsq_p2p;
+    peer_grads as for adamw_p2p)"""
+    _sumsq_buf(sumsq)
+    world = len(peer_grads)
+    if _fam("adamw", 0.0, 4.0 * world * n):
+        return
+    ga = (C.c_void_p * world)(*[t if isinstance(t, int) else t.data_ptr() for t in peer_grads])
+    check(load().svdx_grad_sumsq_p2p(ga, world, lo, n, sumsq.data_ptr(), _stream()), "svdx_grad_sumsq_p2p")
+
+
+def clip_coef(sumsq, max_norm, scale, out):
+    """out[0] = total norm fl(sqrt(sumsq[0])) * scale, out[1] = the clip coefficient min(max_norm / (norm + 1e-6), 1), NaN kept
+    (svdx_clip_coef, one thread; max_norm a device fp32 scalar, out device fp32[2])"""
+    if max_norm.dtype != torch.float32 or out.dtype != torch.float32 or out.numel() < 2 or sumsq.dtype != torch.float64:
+        raise ValueError("clip_coef: sumsq float64, max_norm float32, out float32[2] (device)")
+    check(load().svdx_clip_coef(sumsq.data_ptr(), max_norm.data_ptr(), float(scale), out.data_ptr(), _stream()), "svdx_clip_coef")
 
 
 EMA_CHUNK = 4096     # elements per block of multi_ema_kernel
@@ -891,22 +941,24 @@ def ema_multi(jobs, block_prefix, njobs, total_blocks, ema_state, nelem):
 A8_BLOCK = 256       # elements per quantisation block of adamw8bit_kernel (one warp)
 
 
-def adamw8bit(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale=1.0, ema_state=None, nbytes=0.0):
+def adamw8bit(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale=1.0, ema_state=None, nbytes=0.0, grad_mul=None):
     """tick + block-wise 8-bit AdamW over many parameters in one launch (svdx_adamw8bit, svdx_adamw8bit_ema with `ema_state`).
     jobs: device bytes of the job table (svd_xtend_b200.h); qmap1 / qmap2: device float[256]; state: device float[8];
-    nbytes (the HBM bytes the update moves) is for the byte accounting only."""
+    nbytes (the HBM bytes the update moves) is for the byte accounting only. grad_mul: a device fp32 scalar the gradient is
+    also multiplied by (the clip coefficient; the *_mul entry points)."""
     if qmap1.dtype != torch.float32 or qmap2.dtype != torch.float32 or qmap1.numel() != 256 or qmap2.numel() != 256:
         raise ValueError("adamw8bit: qmap1 / qmap2 are float32[256]")
+    gm = _grad_mul(grad_mul)
+    if ema_state is not None and (ema_state.dtype != torch.float64 or ema_state.numel() < 9):
+        raise ValueError("adamw8bit: ema_state is float64[9] (svd_xtend_b200.h)")
     if _fam("adamw", 0.0, nbytes):
         return
+    args = (jobs.data_ptr(), block_prefix.data_ptr(), njobs, total_blocks, qmap1.data_ptr(), qmap2.data_ptr(), state.data_ptr(),
+            float(grad_scale))
     if ema_state is not None:
-        if ema_state.dtype != torch.float64 or ema_state.numel() < 9:
-            raise ValueError("adamw8bit: ema_state is float64[9] (svd_xtend_b200.h)")
-        check(load().svdx_adamw8bit_ema(jobs.data_ptr(), block_prefix.data_ptr(), njobs, total_blocks, qmap1.data_ptr(), qmap2.data_ptr(),
-                                        state.data_ptr(), float(grad_scale), ema_state.data_ptr(), _stream()), "svdx_adamw8bit_ema")
-        return
-    check(load().svdx_adamw8bit(jobs.data_ptr(), block_prefix.data_ptr(), njobs, total_blocks, qmap1.data_ptr(), qmap2.data_ptr(),
-                                state.data_ptr(), float(grad_scale), _stream()), "svdx_adamw8bit")
+        args += (ema_state.data_ptr(),)
+    name = "svdx_adamw8bit" + ("_ema" if ema_state is not None else "") + ("_mul" if gm is not None else "")
+    check(getattr(load(), name)(*args, *(() if gm is None else (gm,)), _stream()), name)
 
 
 def multi_transpose(src_base, jobs, tile_prefix, njobs, total_tiles):

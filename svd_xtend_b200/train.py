@@ -126,13 +126,16 @@ class ParamArena:
             self._tjob_index[key] = len(self._tjobs)
             self._tjobs.append((self.offset_of[params[0]], dst, O, I))
             self._tjob_dev = None
+            if not torch.cuda.is_current_stream_capturing():
+                # upload the table now: a later refresh may run inside a capture (a captured forward, or the micro-step of
+                # gradient accumulation before any update), where a pageable host-to-device copy is not allowed
+                self.prepare_transposes()
             return dst
         return self._tjobs[j][1]
 
-    def refresh_transposes(self):
-        if not self._tjobs:
-            return
-        if self._tjob_dev is None:
+    def prepare_transposes(self):
+        """upload the job table of the registered transposes (no launch)"""
+        if self._tjobs and self._tjob_dev is None:
             import struct
             blob = bytearray()
             prefix, tiles = [], 0
@@ -143,6 +146,11 @@ class ParamArena:
             jobs = torch.frombuffer(bytes(blob), dtype=torch.uint8).clone().to(self.data.device)
             pre = torch.tensor(prefix, dtype=torch.int32, device=self.data.device)
             self._tjob_dev = (jobs, pre, len(self._tjobs), tiles)
+
+    def refresh_transposes(self):
+        if not self._tjobs:
+            return
+        self.prepare_transposes()
         jobs, pre, n, tiles = self._tjob_dev
         raw.multi_transpose(self.shadow, jobs, pre, n, tiles)
 
@@ -183,6 +191,25 @@ def adamw_state_dict(arena: ParamArena, step: int, hyper: dict, moments: Iterabl
         for i, (p, o) in enumerate(zip(arena.params, arena.offsets)):
             state[i][key] = flat[o:o + p.numel()].view(p.shape).to("cpu", copy=True)
     return {"state": state, "param_groups": [group]}
+
+
+def check_max_grad_norm(value) -> float:
+    """max_grad_norm as a float; ValueError unless it is a positive, finite number"""
+    try:
+        x = float(value)
+    except (TypeError, ValueError):
+        raise ValueError(f"max_grad_norm must be a positive finite number, got {value!r}") from None
+    if not (0.0 < x < float("inf")) or isinstance(value, bool):
+        raise ValueError(f"max_grad_norm must be a positive finite number, got {value!r}")
+    return x
+
+
+def all_reduce_sumsq(sumsq: torch.Tensor, world: int, group=None) -> None:
+    """The sharded optimizers' global gradient norm, step 1 of 2: sum every rank's fp64 sum of squares over its owned slice
+    (sumsq: a 1-element float64 tensor, in place; captured with a graphed step). Step 2 is svdx_clip_coef with scale = 1 / world,
+    so the norm is that of the mean gradient the update applies."""
+    if world > 1:
+        dist.all_reduce(sumsq, op=dist.ReduceOp.SUM, group=group)
 
 
 def _indices(ix: List[int]) -> str:
@@ -257,7 +284,8 @@ class _ArenaAdamW:
     _moment_buffers: tuple = ()          # attribute names of the moment buffers, in snapshot_tensors' order
     _ema_sharded = False          # an attached EMA is advanced slice by slice over the ranks
 
-    def __init__(self, arena: ParamArena, lr, betas, weight_decay, eps):
+    def __init__(self, arena: ParamArena, lr, betas, weight_decay, eps, max_grad_norm: Optional[float] = None):
+        self._max_norm = None if max_grad_norm is None else check_max_grad_norm(max_grad_norm)
         self.arena = arena
         self.betas, self.weight_decay, self.eps = betas, weight_decay, eps
         self._lr = float(lr)
@@ -269,6 +297,17 @@ class _ArenaAdamW:
         # torch.optim-style view for lr schedulers: `for g in opt.param_groups: g["lr"] = ...` then `opt.sync_lr()`
         self.param_groups = [{"lr": float(lr), "params": arena.params}]
         self.ema = None
+        # global gradient-norm clipping (torch.nn.utils.clip_grad_norm_, train_svd.py --max_grad_norm): every step computes the
+        # norm on the device (svdx_grad_sumsq, svdx_clip_coef) and the update kernel multiplies the gradient by the coefficient,
+        # so a captured step clips without a host sync. The gradient arena itself is not rescaled.
+        self._clip = None
+        if self._max_norm is not None:
+            dev = arena.data.device
+            self._max_norm_dev = torch.tensor([self._max_norm], device=dev, dtype=F32)
+            self._max_norm_host = torch.empty(1, dtype=F32).pin_memory() if arena.data.is_cuda else torch.empty(1, dtype=F32)
+            self._sumsq = torch.zeros(1 + raw.SUMSQ_PARTIALS, device=dev, dtype=torch.float64)
+            self._clip = torch.zeros(2, device=dev, dtype=F32)          # {total_norm, coef} (svdx_clip_coef)
+            self._grad_norm = self._clip[0]
 
     def attach_ema(self, ema):
         """Advance `ema` (an svd_xtend_b200.ema.EMAModel built over the model's parameters, frozen ones included or not) inside
@@ -301,6 +340,36 @@ class _ArenaAdamW:
         self._lr_host[0] = self._lr
         self.state[0:1].copy_(self._lr_host, non_blocking=True)
 
+    @property
+    def max_grad_norm(self) -> Optional[float]:
+        return self._max_norm
+
+    @max_grad_norm.setter
+    def max_grad_norm(self, value: float):
+        """a new threshold for the next updates (a 4-byte H2D copy, like `opt.lr`; a captured step picks it up)"""
+        if self._clip is None:
+            raise ValueError("max_grad_norm: this optimizer was built without clipping (max_grad_norm=None), and a captured step's "
+                             "launches are fixed; build it with max_grad_norm=... to clip")
+        self._max_norm = check_max_grad_norm(value)
+        self._max_norm_host[0] = self._max_norm
+        self._max_norm_dev.copy_(self._max_norm_host, non_blocking=True)
+
+    @property
+    def grad_norm(self) -> torch.Tensor:
+        """0-dim fp32 device tensor at a fixed address: the total (pre-clip) norm of the gradient the last update applied (the
+        mean gradient under the sharded forms), what accelerator.clip_grad_norm_ returns. A graph replay refreshes it; reading
+        its value synchronises."""
+        if self._clip is None:
+            raise ValueError("grad_norm: this optimizer was built without clipping (max_grad_norm=None) and computes no norm")
+        return self._grad_norm
+
+    def _clip_coef(self, scale: float) -> Optional[torch.Tensor]:
+        """after self._sumsq[0] holds the sum of squares of the gradient g the kernel reads: the norm of the applied gradient
+        g * scale (the update's grad_scale) into grad_norm, and the clip coefficient the update also multiplies by (device
+        fp32[1])"""
+        raw.clip_coef(self._sumsq, self._max_norm_dev, scale, self._clip)
+        return self._clip[1:]
+
     def sync_lr(self):
         """push param_groups[0]['lr'] (written by a torch lr scheduler) to the device state"""
         if self.param_groups[0]["lr"] != self._lr:
@@ -319,11 +388,12 @@ class _ArenaAdamW:
         self.arena.zero_grad()
 
     def snapshot_tensors(self) -> List[torch.Tensor]:
-        """everything a warm-up step mutates (for GraphedStep(restore=...)), the attached EMA included"""
+        """everything a warm-up step mutates (for GraphedStep(restore=...)), the attached EMA and the clip's {norm, coef}
+        included (so grad_norm is that of the last real update, not of a warm-up)"""
         ts = [self.arena.data, *(getattr(self, name) for name in self._moment_buffers), self.state]
         if self.arena.shadow is not None:
             ts.append(self.arena.shadow)
-        return ts + self._ema_tensors()
+        return ts + self._ema_tensors() + ([] if self._clip is None else [self._clip])
 
     def _hyper(self) -> dict:
         extra = {k: x for k, x in self.param_groups[0].items() if k not in ("lr", "params")}
@@ -346,14 +416,19 @@ class FusedAdamW(_ArenaAdamW):
 
     _moment_buffers = ("m", "v")
 
-    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8):
-        super().__init__(arena, lr, betas, weight_decay, eps)
+    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8,
+                 max_grad_norm: Optional[float] = None):
+        super().__init__(arena, lr, betas, weight_decay, eps, max_grad_norm)
         self.m = torch.zeros_like(arena.data)
         self.v = torch.zeros_like(arena.data)
 
     def step(self, grad_scale: float = 1.0):
         a = self.arena
-        raw.adamw_graph(a.data, a.grad, self.m, self.v, self.state, grad_scale, shadow=a.shadow, **self._ema_args())
+        coef = None
+        if self._clip is not None:
+            raw.grad_sumsq(a.grad, self._sumsq)
+            coef = self._clip_coef(grad_scale)
+        raw.adamw_graph(a.data, a.grad, self.m, self.v, self.state, grad_scale, shadow=a.shadow, **self._ema_args(), grad_mul=coef)
         self._updated()
 
     # ---- checkpoints in torch.optim.AdamW's layout (adamw_state_dict): torch.optim.AdamW, ShardedAdamW and P2PShardedAdamW
@@ -379,9 +454,10 @@ class FusedAdamW8bit(_ArenaAdamW):
 
     _moment_buffers = ("codes1", "codes2", "absmax1", "absmax2", "m32", "v32")
 
-    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, min_8bit_size: int = 4096):
+    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, min_8bit_size: int = 4096,
+                 max_grad_norm: Optional[float] = None):
         from .optim8bit import dynamic_map, num_blocks
-        super().__init__(arena, lr, betas, weight_decay, eps)
+        super().__init__(arena, lr, betas, weight_decay, eps, max_grad_norm)
         self.min_8bit_size = int(min_8bit_size)
         dev = arena.data.device
         self.qmap1, self.qmap2 = dynamic_map(True).to(dev), dynamic_map(False).to(dev)
@@ -447,8 +523,12 @@ class FusedAdamW8bit(_ArenaAdamW):
             n8 = sum(p.numel() for p, _, q, _, _ in self.layout if q)
             self._nbytes = update_bytes(n8, sum(p.numel() for p in self.arena.params) - n8, self.arena.shadow is not None, self.ema is not None)
         tb = self._table
+        coef = None
+        if self._clip is not None:
+            raw.grad_sumsq(self.arena.grad, self._sumsq)
+            coef = self._clip_coef(grad_scale)
         raw.adamw8bit(tb.dev, tb.prefix, tb.njobs, tb.blocks, self.qmap1, self.qmap2, self.state, grad_scale,
-                      ema_state=None if self.ema is None else self.ema._state, nbytes=self._nbytes)
+                      ema_state=None if self.ema is None else self.ema._state, nbytes=self._nbytes, grad_mul=coef)
         self._updated()
 
     # ---- checkpoints in bitsandbytes' per-parameter layout (svd_xtend_b200.optim8bit.AdamW8bit loads them too) ----
@@ -523,8 +603,9 @@ class ShardedAdamW(_ArenaAdamW):
     _moment_buffers = ("m", "v")
     _ema_sharded = True
 
-    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, group=None):
-        super().__init__(arena, lr, betas, weight_decay, eps)
+    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, group=None,
+                 max_grad_norm: Optional[float] = None):
+        super().__init__(arena, lr, betas, weight_decay, eps, max_grad_norm)
         self.group = group
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
@@ -588,8 +669,13 @@ class ShardedAdamW(_ArenaAdamW):
     def step(self):
         a = self.arena
         g = self.reduce_scatter_grads()
+        coef = None
+        if self._clip is not None:         # the norm of the summed gradient's owned slice, summed over the ranks, of the mean
+            raw.grad_sumsq(g, self._sumsq)
+            all_reduce_sumsq(self._sumsq[:1], self.world, self.group)
+            coef = self._clip_coef(1.0 / self.world)
         raw.adamw_graph(a.data[self.lo:self.hi], g, self.m, self.v, self.state, 1.0 / self.world,
-                        shadow=None if a.shadow is None else a.shadow[self.lo:self.hi], **self._ema_args(self.lo, self.hi))
+                        shadow=None if a.shadow is None else a.shadow[self.lo:self.hi], **self._ema_args(self.lo, self.hi), grad_mul=coef)
         if a.shadow is not None:
             self.all_gather_(a.shadow)
         else:
@@ -646,8 +732,9 @@ class P2PShardedAdamW(ShardedAdamW):
     intermediate HBM passes, one launch; two tiny all-reduces (captured with the step) order the ranks around it. Results are
     those of ShardedAdamW (bit-identical at world 2; at larger worlds the gradient sum runs in rank order on the owner)."""
 
-    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, group=None):
-        super().__init__(arena, lr=lr, betas=betas, weight_decay=weight_decay, eps=eps, group=group)
+    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, group=None,
+                 max_grad_norm: Optional[float] = None):
+        super().__init__(arena, lr=lr, betas=betas, weight_decay=weight_decay, eps=eps, group=group, max_grad_norm=max_grad_norm)
         if arena.shadow is None:
             raise ValueError("P2PShardedAdamW needs the arena's bf16 shadow (CUDA arena)")
         if self.world > 16:
@@ -666,8 +753,15 @@ class P2PShardedAdamW(ShardedAdamW):
         a = self.arena
         if self.world > 1:
             self._fence()                                   # every rank's gradients are final
+        coef = None
+        if self._clip is not None:
+            # a pre-pass over the same peer slices (the gradient crosses NVLink twice when clipping), then the rank sum of the
+            # partials: the norm of the mean gradient the update below applies
+            raw.grad_sumsq_p2p(self.peer_grad, self.lo, self.hi - self.lo, self._sumsq)
+            all_reduce_sumsq(self._sumsq[:1], self.world, self.group)
+            coef = self._clip_coef(1.0 / self.world)
         raw.adamw_p2p(a.data[self.lo:self.hi], self.m, self.v, self.peer_grad, self.peer_shadow, self.lo, self.state, 1.0 / self.world,
-                      **self._ema_args(self.lo, self.hi))
+                      **self._ema_args(self.lo, self.hi), grad_mul=coef)
         if self.world > 1:
             self._fence()                                   # every shadow is complete, nobody still reads this rank's gradients
         self._updated()

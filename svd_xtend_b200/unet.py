@@ -1120,7 +1120,8 @@ class _UNetFn(torch.autograd.Function):
             # optimizer.zero_grad(set_to_none=True) (train_svd.py:1049) dropped the .grad views: the flat gradient arena the
             # kernels accumulate into must start this backward at zero, or gradients would pile up across steps
             model._arena.zero_grad()
-        if ctx.entry is not None:
+        captured = ctx.entry is not None
+        if captured:
             entry, ctx.entry = ctx.entry, None
             if not entry.pending_backward:
                 raise RuntimeError("svd_xtend_b200: backward called twice on the same forward (retain_graph is not supported)")
@@ -1143,8 +1144,13 @@ class _UNetFn(torch.autograd.Function):
             gp = E.pgrads.get(p)
             if gp is None:
                 gp = torch.zeros(p.shape, device=p.device, dtype=F32)   # e.g. attn2.to_q/to_k/norm2: exactly zero
-            gp = gp if p.dtype == F32 else gp.to(p.dtype)
-            if p.grad is None or p.grad is gp:      # (a captured backward re-fills the same static buffer every step)
+            if p.dtype != F32:
+                gp = gp.to(p.dtype)
+            elif captured:
+                # a captured backward re-fills the same static buffer on every replay: .grad is a copy of it, so that a
+                # second backward without zero_grad (gradient accumulation) adds to the first instead of replacing it
+                gp = gp.clone()
+            if p.grad is None:
                 p.grad = gp
             else:
                 p.grad.add_(gp)

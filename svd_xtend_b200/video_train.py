@@ -241,12 +241,25 @@ class VideoTrainStep:
     Image.resize((W, H)) does (assemble_train_batch). encode_chunk_size: encode that many frames at a time (assemble_train_batch).
 
     The graphed form keeps the snapshot it restores after the capture in pinned host memory (train.GraphedStep), which with
-    encode_chunk_size is what lets the default size of train_svd.py (25 x 576 x 1024) fit on one 80 GB card."""
+    encode_chunk_size is what lets the default size of train_svd.py (25 x 576 x 1024) fit on one 80 GB card.
+
+    gradient_accumulation_steps=k > 1 (train_svd.py --gradient_accumulation_steps, accelerate's `accumulate`): every call runs one
+    micro-step (frames and draws -> batch -> UNet -> edm_loss -> (loss / k).backward(), adding into the gradient arena) and
+    returns that micro-batch's unscaled loss; calls k, 2k, ... also run the update (opt.step(), clipping included when the
+    optimizer has max_grad_norm, then opt.zero_grad()). `step.sync_gradients` is True after a call that updated, as accelerate's
+    flag: step a scheduler, log or save there. The micro-step and the update are two captured train.GraphedSteps; construction
+    leaves the gradient arena zeroed, so the first window starts clean. k = 1 is the single captured step above."""
 
     def __init__(self, unet, vae, image_encoder, opt, *, frames_shape, conditioning_dropout_prob: Optional[float] = None,
                  generator: Optional[torch.Generator] = None, fps: int = 7, motion_bucket_id: int = 127, image_mean=CLIP_MEAN,
                  image_std=CLIP_STD, cuda_graph: bool = True, source_size: Optional[Tuple[int, int]] = None,
-                 encode_chunk_size: Optional[int] = None):
+                 encode_chunk_size: Optional[int] = None, gradient_accumulation_steps: int = 1):
+        k = gradient_accumulation_steps
+        if not isinstance(k, int) or isinstance(k, bool) or k < 1:
+            raise ValueError(f"gradient_accumulation_steps must be an int >= 1, got {k!r}")
+        self.accumulation_steps = k
+        self.sync_gradients = False          # True after a call that applied an optimizer update
+        self._calls = 0
         if vae.device.type != "cuda":
             raise RuntimeError("svd_xtend_b200: VideoTrainStep only runs on a CUDA (sm_90a) device; there is no CPU fallback")
         self.unet, self.vae, self.image_encoder, self.opt = unet, vae, image_encoder, opt
@@ -272,6 +285,7 @@ class VideoTrainStep:
         check_train_inputs(vae, image_encoder, unet, self.static["pixel_values"], self.static, conditioning_dropout_prob,
                            self.kw.get("size"), encode_chunk_size)
         self.graphed = None
+        self.graphed_update = None
         if cuda_graph:
             from .train import GraphedStep
 
@@ -279,10 +293,18 @@ class VideoTrainStep:
                 self.generator.set_state(gstate)
                 unet.refresh_trainable_operands(shadow_current=opt.arena.shadow is not None)
 
-            self.graphed = GraphedStep(self._step, self.static, warmup=2, restore=opt.snapshot_tensors(), on_restored=restored,
-                                       restore_on_host=True)
+            if k == 1:
+                self.graphed = GraphedStep(self._step, self.static, warmup=2, restore=opt.snapshot_tensors(), on_restored=restored,
+                                           restore_on_host=True)
+            else:
+                # the micro-step changes nothing but the gradient arena, which is zeroed below
+                self.graphed = GraphedStep(self._micro, self.static, warmup=2, restore=None)
+                self.graphed_update = GraphedStep(lambda _s: self._update(), {}, warmup=2, restore=opt.snapshot_tensors(),
+                                                  on_restored=restored, restore_on_host=True)
         else:
             self.generator.set_state(gstate)
+        if k > 1:
+            opt.arena.zero_grad()
 
     def draw(self) -> Dict[str, torch.Tensor]:
         return draw_train_noise(self.B, self.F, self.H, self.W, generator=self.generator, device=self.device,
@@ -290,12 +312,21 @@ class VideoTrainStep:
 
     def _step(self, s: Dict[str, torch.Tensor]) -> torch.Tensor:
         self.opt.zero_grad()
+        loss = self._micro(s)
+        self.opt.step()
+        return loss
+
+    def _micro(self, s: Dict[str, torch.Tensor]) -> torch.Tensor:
+        """batch -> UNet -> loss -> backward of (loss / k), adding into the gradient arena; the unscaled loss"""
         b = assemble_train_batch(self.vae, self.image_encoder, self.unet, s["pixel_values"], s, **self.kw)
         pred = self.unet(b["sample"], b["timestep"], b["encoder_hidden_states"], added_time_ids=b["added_time_ids"]).sample
         loss = edm_loss(pred.float(), b["noisy"], b["latents"], b["sigmas"])
-        loss.backward()
-        self.opt.step()
+        (loss if self.accumulation_steps == 1 else loss / self.accumulation_steps).backward()
         return loss.detach()
+
+    def _update(self) -> None:
+        self.opt.step()
+        self.opt.zero_grad()
 
     def check_frames(self, pixel_values: torch.Tensor) -> None:
         """ValueError / TypeError unless pixel_values is what this step was built for"""
@@ -318,6 +349,14 @@ class VideoTrainStep:
         self.static["pixel_values"].copy_(pixel_values, non_blocking=True)
         for k, v in self.draw().items():
             self.static[k].copy_(v)
-        if self.graphed is not None:
-            return self.graphed.replay()
-        return self._step(self.static)
+        self._calls += 1
+        self.sync_gradients = self._calls % self.accumulation_steps == 0
+        if self.accumulation_steps == 1:
+            return self.graphed.replay() if self.graphed is not None else self._step(self.static)
+        loss = self.graphed.replay() if self.graphed is not None else self._micro(self.static)
+        if self.sync_gradients:
+            if self.graphed_update is not None:
+                self.graphed_update.replay()
+            else:
+                self._update()
+        return loss
