@@ -477,12 +477,35 @@ int svdx_vae_frames_in_range(const void* x, int32_t x_dtype, const float* cond_e
  * W0 -> W (taps_x), the rows of svdx_vae_frames_in for the frames [first, first + count) into dst [count * H*W][c_pad] (c_pad a
  * multiple of 8, dst 16-byte aligned), where x = fl(fl(resize(src) / 127.5f) - 1) (train_svd.py's DummyDataset); for each
  * conditioning frame B*F + b in the range, also the clean first frame x[b][0] into first_frames fp32 [B][3][H][W] (may be NULL).
- * One launch. */
+ * One launch.
+ * svdx_resize_taps_box_ksize / svdx_resize_taps_box (HOST): the same for Image.resize(size, box=...) along one axis: the source
+ * interval [in0, in1) (Pillow's float box bounds) -> out_size. SVDX_E_BADARG unless 0 <= in0 <= in1 <= in_size (Pillow's box
+ * rules; a box of zero extent is valid) and both are finite. svdx_resize_taps is the box [0, in_size), bit for bit. Pillow copies
+ * an axis with out_size == in_size and the box [0, in_size); those taps are the identity, so the resize stays bit exact.
+ * svdx_frames_u8_in_clips: svdx_frames_u8_in for clips of different source sizes and boxes. Clip b (frames F*b .. F*b + F-1 and
+ * conditioning frame B*F + b) is described by the DEVICE descriptor descs[b]: its frame f is the uint8 [H0][W0][3] image at byte
+ * start + f*H0*W0*3 of src, and its output row y / column x uses tap row ty_off + y of taps_y / tx_off + x of taps_x. The tap
+ * tables are int32 [ty_rows][2 + ksize_y] and [tx_rows][2 + ksize_x]: one fixed row stride, the largest ksize of any clip, each
+ * row as svdx_resize_taps(_box) writes it, zero padded. A descriptor whose frames do not fit in src_bytes, or whose tap rows do
+ * not fit in the tables, reads nothing (those frames come out as u = 0), and tap rows are clamped to the clip's source size.
+ * Same rows, rounding and frame range as svdx_frames_u8_in; svdx_frames_u8_in is the case where every clip shares one descriptor
+ * and runs the same kernel. One launch. */
+typedef struct svdx_clip_desc {
+  int64_t start;               /* byte offset of the clip's frame 0 in src */
+  int32_t H0, W0;              /* its source size */
+  int32_t ty_off, tx_off;      /* its first tap rows in taps_y / taps_x */
+} svdx_clip_desc;
 int svdx_resize_taps_ksize(int32_t in_size, int32_t out_size);
 int svdx_resize_taps(int32_t in_size, int32_t out_size, int32_t* taps);
+int svdx_resize_taps_box_ksize(int32_t in_size, int32_t out_size, float in0, float in1);
+int svdx_resize_taps_box(int32_t in_size, int32_t out_size, float in0, float in1, int32_t* taps);
 int svdx_frames_u8_in(const uint8_t* src, int32_t H0, int32_t W0, const int32_t* taps_y, int32_t ksize_y, const int32_t* taps_x,
                       int32_t ksize_x, const float* cond_eps, const float* cond_sigma, int32_t B, int32_t F, int32_t H, int32_t W,
                       int32_t first, int32_t count, int32_t c_pad, void* dst, float* first_frames, void* stream);
+int svdx_frames_u8_in_clips(const uint8_t* src, int64_t src_bytes, const svdx_clip_desc* descs, const int32_t* taps_y,
+                            int32_t ty_rows, int32_t ksize_y, const int32_t* taps_x, int32_t tx_rows, int32_t ksize_x,
+                            const float* cond_eps, const float* cond_sigma, int32_t B, int32_t F, int32_t H, int32_t W, int32_t first,
+                            int32_t count, int32_t c_pad, void* dst, float* first_frames, void* stream);
 /* svdx_edm_prepare: from the fp32 moments [B*(F+1)][2C][h][w] of that encode (mean, then logvar), per latent element
  *   z = mean + exp(0.5 * clamp(logvar, -30, 20)) * eps,  latent = z * sf,  noisy = latent + noise * sigma[b]
  * (:948, :287, :951, :967) and the conditioning latents c = (z_c * sf) * (1 / sf) of frame B*F + b (:959-960: torch's division of

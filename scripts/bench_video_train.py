@@ -2,7 +2,8 @@
 """Training step from video frames (svd_xtend_b200.video_train.VideoTrainStep) on the H100 path, one JSON line.
 
     python scripts/bench_video_train.py --config 2|4 [--steps K] [--warmup W] [--forms graphed,eager,latent_only]
-                                        [--input float|u8] [--source 1080x1920] [--encode-chunk N] [--frozen-dtype fp32|bf16]
+                                        [--input float|u8|mixed] [--source 1080x1920] [--sources 1080x1920,360x640,...]
+                                        [--encode-chunk N] [--frozen-dtype fp32|bf16]
 
 Seeded default-init SVD UNet (the config's trainable set and gradient checkpointing), VAE encoder and CLIP ViT-H image encoder,
 FusedAdamW, B = 1, conditioning dropout 0.1. The forms of the step (--forms, default all three), timed in alternating windows of
@@ -13,6 +14,12 @@ K steps, medians of 3:
   * latent_only: the latent-input graphed step bench.py times (workload.synthetic_batch, no VAE / CLIP).
 --input u8 feeds decoded uint8 frames [1, F, H0, W0, 3] of --source size from pinned host memory (resized on the GPU as Pillow's
 Image.resize does); float feeds fp32 frames [1, F, 3, H, W] from a device buffer. --encode-chunk N encodes N frames at a time.
+--input mixed feeds a list of uint8 clips [F, H0_b, W0_b, 3] from pinned host memory to a VideoTrainStep(max_source_size=...)
+whose capacity is the largest of --sources; each call takes the next size of --sources (clips of one call cycle through it too),
+so the sizes change from call to call. The forms graphed_u8 (source_size = the first of --sources) and graphed_float (fp32 frames)
+may be added to --forms to time the single-size and float steps in the same session. With --input mixed the report also has the
+resize kernel alone (svdx_frames_u8_in_clips over all B*(F+1) frames, CUDA events, median of 20) and the bytes it reads (each
+source pixel once) and writes (the bf16 rows and the fp32 first frames), computed from the shapes.
 --frozen-dtype: the VAE's and CLIP's weights, fp32 (default) or bf16 as train_svd.py holds them under --mixed_precision=bf16.
 Reports ms per step and frames/s of each form, torch.cuda.max_memory_allocated / memory_reserved after each form's
 construction, after the warm-up and after the timed windows, the card's name and power limit, and the SM clock sampled during
@@ -36,21 +43,56 @@ def _mem():
             "reserved_gib": round(torch.cuda.memory_reserved() / 2 ** 30, 2)}
 
 
+def _kernel_alone(clips, capacity, F, H, W, dev):
+    """svdx_frames_u8_in_clips over the B*(F+1) frames of each call's clips, CUDA events, median of 20 per size; the bytes it
+    must move, from the shapes: every source pixel of the clip read once, the bf16 rows (64 channels) and the fp32 first frame
+    written"""
+    from svd_xtend_b200.video_train import ClipSlots, log_normal
+    out = []
+    for cs in clips:
+        slots = ClipSlots(len(cs), F, (H, W), capacity, dev)
+        slots.load(cs)
+        B = len(cs)
+        eps, sig = torch.zeros(B, 3, H, W, device=dev), log_normal(torch.full((B,), 0.5, device=dev), -3.0, 0.5)
+        rows = torch.empty(B * (F + 1) * H * W, 64, device=dev, dtype=torch.bfloat16)
+        x0 = torch.empty(B, 3, H, W, device=dev)
+        for _ in range(3):
+            slots.fill(rows, 0, B * (F + 1), eps, sig, x0, 64)
+        ts = []
+        for _ in range(20):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            slots.fill(rows, 0, B * (F + 1), eps, sig, x0, 64)
+            e1.record()
+            torch.cuda.synchronize()
+            ts.append(e0.elapsed_time(e1))
+        ms = statistics.median(ts)
+        read = sum(c.numel() for c in cs) + eps.numel() * 4
+        written = rows.numel() * 2 + x0.numel() * 4
+        out.append({"source": list(cs[0].shape[1:3]), "ms": round(ms, 4), "bytes_read": read, "bytes_written": written,
+                    "gb_per_s": round((read + written) / ms / 1e6, 1)})
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config", type=int, choices=(2, 4), default=2)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--forms", default="graphed,eager,latent_only")
-    ap.add_argument("--input", choices=("float", "u8"), default="float")
+    ap.add_argument("--input", choices=("float", "u8", "mixed"), default="float")
     ap.add_argument("--source", default="1080x1920", help="H0xW0 of the uint8 frames (--input u8)")
+    ap.add_argument("--sources", default="1080x1920,720x1280,360x640,1080x1440", help="H0xW0 sizes of the clips (--input mixed)")
     ap.add_argument("--encode-chunk", type=int, default=None)
     ap.add_argument("--frozen-dtype", choices=("fp32", "bf16"), default="fp32")
     args = ap.parse_args()
     wanted = [f for f in args.forms.split(",") if f]
-    if not wanted or any(f not in ("graphed", "eager", "latent_only") for f in wanted):
-        raise SystemExit(f"--forms: a comma-separated subset of graphed,eager,latent_only, got {args.forms!r}")
+    if not wanted or any(f not in ("graphed", "eager", "latent_only", "graphed_u8", "graphed_float") for f in wanted):
+        raise SystemExit(f"--forms: a comma-separated subset of graphed,eager,latent_only,graphed_u8,graphed_float, got {args.forms!r}")
     H0, W0 = (int(v) for v in args.source.lower().split("x"))
+    sources = [tuple(int(v) for v in s.lower().split("x")) for s in args.sources.split(",") if s]
+    if args.input == "mixed":
+        H0, W0 = sources[0]
     if not torch.cuda.is_available():
         raise RuntimeError("bench_video_train.py needs a CUDA device: the step has no CPU fallback")
 
@@ -96,11 +138,23 @@ def main():
         frames = torch.randint(0, 256, (1, F, H0, W0, 3), generator=g, dtype=torch.uint8).pin_memory()
     else:
         frames = (torch.rand(1, F, 3, H, W, generator=g) * 2 - 1).to(dev)
+    if args.input == "mixed":
+        clips = [[torch.randint(0, 256, (F, h0, w0, 3), generator=g, dtype=torch.uint8).pin_memory()] for h0, w0 in sources]
+        u8_frames = clips[0][0][None]
+        float_frames = frames
+        frames = clips
+        calls = [0]
+
+        def next_clips():
+            calls[0] += 1
+            return clips[calls[0] % len(clips)]
     memory = {"models": _mem()}
 
     forms, failed = {}, {}
     kw = dict(frames_shape=(1, F, H, W), conditioning_dropout_prob=0.1, generator=torch.Generator(dev).manual_seed(0),
               source_size=(H0, W0) if args.input == "u8" else None, encode_chunk_size=args.encode_chunk)
+    if args.input == "mixed":
+        kw["max_source_size"] = (max(s[0] for s in sources), max(s[1] for s in sources))
 
     def oom(name, e):
         failed[name] = f"OutOfMemoryError: {str(e).splitlines()[0]}"
@@ -109,10 +163,22 @@ def main():
     if "graphed" in wanted:
         try:
             graphed = VideoTrainStep(unet, vae, clip, opt, **kw)
-            forms["graphed"] = lambda: graphed(frames)
+            forms["graphed"] = (lambda: graphed(next_clips())) if args.input == "mixed" else (lambda: graphed(frames))
         except torch.OutOfMemoryError as e:
             oom("graphed", e)
         memory["graphed_built"] = _mem()
+    for name in ("graphed_u8", "graphed_float"):
+        if name in wanted:
+            if args.input != "mixed":
+                raise SystemExit(f"--forms {name} is a comparison of --input mixed")
+            try:
+                other = dict(kw, max_source_size=None, source_size=(H0, W0) if name == "graphed_u8" else None)
+                st = VideoTrainStep(unet, vae, clip, opt, **other)
+                x = u8_frames if name == "graphed_u8" else float_frames
+                forms[name] = (lambda st=st, x=x: st(x))
+            except torch.OutOfMemoryError as e:
+                oom(name, e)
+            memory[name + "_built"] = _mem()
     if "latent_only" in wanted:
         b = {k: v.to(dev) for k, v in synthetic_batch(1, F, cfg["h"], cfg["w"], seed=1234).items()}
 
@@ -132,7 +198,7 @@ def main():
         memory["latent_only_built"] = _mem()
     if "eager" in wanted:
         eager = VideoTrainStep(unet, vae, clip, opt, cuda_graph=False, **kw)
-        forms["eager"] = lambda: eager(frames)
+        forms["eager"] = (lambda: eager(next_clips())) if args.input == "mixed" else (lambda: eager(frames))
     for k in list(forms):
         try:
             for _ in range(warmup):
@@ -165,8 +231,10 @@ def main():
         ms = statistics.median(ts)
         res[k] = {"ms_per_step": round(ms, 3), "frames_per_s": round(F * 1e3 / ms, 2), "windows_ms": [round(t, 3) for t in ts]}
     res.update({k: {"failed": v} for k, v in failed.items()})
+    kernel = _kernel_alone(clips, kw["max_source_size"], F, H, W, dev) if args.input == "mixed" else None
     print(json.dumps({"metric": "video_train_step", "config": args.config, "frames": F, "pixels": [H, W], "batch": 1,
-                      "input": args.input, "source": [H0, W0] if args.input == "u8" else None, "encode_chunk": args.encode_chunk,
+                      "input": args.input, "source": [H0, W0] if args.input == "u8" else None,
+                      "sources": sources if args.input == "mixed" else None, "resize_kernel": kernel, "encode_chunk": args.encode_chunk,
                       "frozen_dtype": args.frozen_dtype, "steps_per_window": steps, "forms": res,
                       "final_loss": None if loss is None else float(loss.float().item()),
                       "max_memory_allocated_gib": round(torch.cuda.max_memory_allocated() / 2 ** 30, 2), "memory": memory,

@@ -138,8 +138,12 @@ _PROTOS = {
                                  c_void_p],
     "svdx_resize_taps_ksize": [c_int, c_int],
     "svdx_resize_taps": [c_int, c_int, c_void_p],
+    "svdx_resize_taps_box_ksize": [c_int, c_int, c_float, c_float],
+    "svdx_resize_taps_box": [c_int, c_int, c_float, c_float, c_void_p],
     "svdx_frames_u8_in": [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                           c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
+    "svdx_frames_u8_in_clips": [c_void_p, c_i64, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int,
+                                c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "svdx_edm_prepare": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int, c_int, c_int, c_int,
                          c_void_p, c_void_p, c_void_p, c_void_p],
 }

@@ -3,9 +3,11 @@ from __future__ import annotations
 
 import ctypes as C
 import functools
+import math
 import os
 from typing import Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -624,18 +626,82 @@ def vae_frames_in_range(x, cond_eps, cond_sigma, dst, first, count, c_pad=64):
     return dst
 
 
-def resize_taps(in_size: int, out_size: int) -> torch.Tensor:
+def resize_taps(in_size: int, out_size: int, box=None) -> torch.Tensor:
     """the taps of Pillow's 8-bpc BICUBIC resample of one axis in_size -> out_size (svdx_resize_taps, computed on the host):
-    int32 [out_size, 2 + ksize] = first source index, tap count, ksize 22-bit fixed-point weights"""
+    int32 [out_size, 2 + ksize] = first source index, tap count, ksize 22-bit fixed-point weights.
+    box=(lo, hi): the taps of the source interval [lo, hi) of that axis, as Image.resize(size, box=...) resamples it (Pillow
+    stores the bounds as fp32); ValueError unless 0 <= lo <= hi <= in_size. None is the box (0, in_size), bit for bit."""
     lib = load()
-    ks = lib.svdx_resize_taps_ksize(int(in_size), int(out_size))
+    if box is None:
+        ks = lib.svdx_resize_taps_ksize(int(in_size), int(out_size))
+    else:
+        lo, hi = (float(np.float32(v)) for v in box)
+        if not (math.isfinite(lo) and math.isfinite(hi) and 0 <= lo <= hi <= int(in_size)):
+            raise ValueError(f"resize_taps: box {tuple(box)} is not within [0, {in_size}] with lo <= hi")
+        ks = lib.svdx_resize_taps_box_ksize(int(in_size), int(out_size), lo, hi)
     if ks < 0:
         _lib.check(ks, "resize_taps")
     taps = torch.empty(int(out_size), 2 + ks, dtype=torch.int32)
-    rc = lib.svdx_resize_taps(int(in_size), int(out_size), taps.data_ptr())
+    if box is None:
+        rc = lib.svdx_resize_taps(int(in_size), int(out_size), taps.data_ptr())
+    else:
+        rc = lib.svdx_resize_taps_box(int(in_size), int(out_size), lo, hi, taps.data_ptr())
     if rc:
         _lib.check(rc, "resize_taps")
     return taps
+
+
+# svdx_clip_desc: int64 start, int32 H0, W0, ty_off, tx_off (24 bytes)
+CLIP_DESC = np.dtype([("start", "<i8"), ("H0", "<i4"), ("W0", "<i4"), ("ty_off", "<i4"), ("tx_off", "<i4")])
+
+
+def clip_descs(starts, sizes, ty_offs, tx_offs) -> torch.Tensor:
+    """the svdx_clip_desc table of frames_u8_in_clips on the host: int64 [B, 3] holding B descriptors (byte offset of each clip in
+    src, its source size (H0, W0), its first tap rows in taps_y / taps_x)"""
+    d = np.zeros(len(starts), CLIP_DESC)
+    d["start"] = starts
+    d["H0"], d["W0"] = [s[0] for s in sizes], [s[1] for s in sizes]
+    d["ty_off"], d["tx_off"] = ty_offs, tx_offs
+    return torch.from_numpy(d.view(np.int64).reshape(len(starts), 3).copy())
+
+
+def frames_u8_in_clips(src, descs, taps_y, taps_x, cond_eps, cond_sigma, dst, size, F, first, count, first_frames=None, c_pad=64):
+    """frames_u8_in for B clips of different source sizes and boxes (svdx_frames_u8_in_clips): src is a contiguous uint8 buffer on
+    the device holding every clip's frames [F, H0_b, W0_b, 3]; descs the DEVICE table of clip_descs (int64 [B, 3]); taps_y /
+    taps_x int32 [rows, 2 + ksize] tables of resize_taps rows (zero padded to one ksize) that the descriptors index. Writes the
+    rows of the frames [first, first + count) of the B*(F+1) frame space into dst bf16 [count * H*W, c_pad] and the clean first
+    frames into first_frames fp32 [B, 3, H, W] (if given). The kernel reads nothing of a descriptor that does not fit in src or in
+    the tap tables."""
+    if src.dtype != torch.uint8:
+        raise TypeError(f"frames_u8_in_clips: src has dtype {src.dtype}; expected uint8")
+    if not src.is_contiguous() or src.numel() == 0:
+        raise ValueError("frames_u8_in_clips: src must be a non-empty contiguous uint8 tensor")
+    if descs.dtype != torch.int64 or not descs.is_contiguous() or descs.dim() != 2 or descs.shape[1] != 3:
+        raise ValueError("frames_u8_in_clips: descs must be a contiguous int64 [B, 3] tensor (clip_descs)")
+    B = descs.shape[0]
+    H, W = (int(v) for v in size)
+    F = int(F)
+    for t, n, what in ((taps_y, H, "taps_y"), (taps_x, W, "taps_x")):
+        if t.dtype != torch.int32 or not t.is_contiguous() or t.dim() != 2 or t.shape[0] < n or t.shape[1] < 3:
+            raise ValueError(f"frames_u8_in_clips: {what} must be a contiguous int32 [>= {n}, 2 + ksize] tensor (resize_taps rows)")
+    if cond_eps.dtype != torch.float32 or not cond_eps.is_contiguous() or cond_eps.numel() != B * 3 * H * W:
+        raise ValueError("frames_u8_in_clips: cond_eps must be a contiguous fp32 tensor of B*3*H*W elements")
+    if cond_sigma.dtype != torch.float32 or cond_sigma.numel() != B:
+        raise ValueError("frames_u8_in_clips: cond_sigma must be fp32 [B]")
+    if F < 1 or not 0 <= first < first + count <= B * (F + 1):
+        raise ValueError(f"frames_u8_in_clips: frames [{first}, {first + count}) are not within [0, {B * (F + 1)})")
+    if dst.dtype != bf16 or not dst.is_contiguous() or dst.shape != (count * H * W, c_pad):
+        raise ValueError(f"frames_u8_in_clips: dst must be a contiguous bf16 [{count * H * W}, {c_pad}] tensor")
+    if first_frames is not None and (first_frames.dtype != torch.float32 or not first_frames.is_contiguous()
+                                     or first_frames.shape != (B, 3, H, W)):
+        raise ValueError(f"frames_u8_in_clips: first_frames must be a contiguous fp32 [{B}, 3, {H}, {W}] tensor")
+    if not all(t.is_cuda for t in (src, descs, taps_y, taps_x, cond_eps, cond_sigma, dst)):
+        raise RuntimeError("svd_xtend_b200: frames_u8_in_clips runs on a CUDA (sm_90a) device only; there is no CPU fallback")
+    check(load().svdx_frames_u8_in_clips(src.data_ptr(), src.numel(), descs.data_ptr(), taps_y.data_ptr(), taps_y.shape[0],
+                                         taps_y.shape[1] - 2, taps_x.data_ptr(), taps_x.shape[0], taps_x.shape[1] - 2,
+                                         cond_eps.data_ptr(), cond_sigma.data_ptr(), B, F, H, W, first, count, c_pad, dst.data_ptr(),
+                                         _ptr(first_frames), _stream()), "frames_u8_in_clips")
+    return dst
 
 
 def frames_u8_in(src, taps_y, taps_x, cond_eps, cond_sigma, dst, size, first, count, first_frames=None, c_pad=64):
