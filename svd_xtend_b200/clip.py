@@ -185,6 +185,21 @@ class CLIPVisionModelWithProjection(nn.Module):
             model.to(torch_dtype)
         return model
 
+    def save_pretrained(self, save_directory: str, safe_serialization: bool = True, **kwargs):
+        """transformers' layout: config.json (a `clip_vision_model` config) and model.safetensors (or pytorch_model.bin) with
+        the keys `from_pretrained` reads"""
+        os.makedirs(save_directory, exist_ok=True)
+        cfg = dict(vars(self.config), architectures=["CLIPVisionModelWithProjection"], model_type="clip_vision_model",
+                   torch_dtype=str(self.dtype).replace("torch.", ""))
+        with open(os.path.join(save_directory, self.config_name), "w") as f:
+            json.dump(cfg, f, indent=2)
+        sd = {k: v.detach().cpu().contiguous() for k, v in self.state_dict().items()}
+        if safe_serialization:
+            from safetensors.torch import save_file
+            save_file(sd, os.path.join(save_directory, "model.safetensors"), metadata={"format": "pt"})
+        else:
+            torch.save(sd, os.path.join(save_directory, "pytorch_model.bin"))
+
     # ------------------------------------------------------------------ entry points
     def _guard(self, x: torch.Tensor, what: str):
         if not x.is_cuda:

@@ -60,7 +60,7 @@ class VideoLatentSampler:
     def __call__(self, image_latents: torch.Tensor, image_embeddings: torch.Tensor, *, num_frames: int, fps: int = 7,
                  motion_bucket_id: int = 127, noise_aug_strength: float = 0.02, num_inference_steps: int = 25,
                  min_guidance_scale: float = 1.0, max_guidance_scale: float = 3.0, noise: Optional[torch.Tensor] = None,
-                 generator: Optional[torch.Generator] = None) -> torch.Tensor:
+                 generator: Optional[torch.Generator] = None, sigma_min: float = 0.002, sigma_max: float = 700.0) -> torch.Tensor:
         B, _, h, w = image_latents.shape
         dev = image_latents.device
         cfg = max_guidance_scale > 1.0
@@ -73,7 +73,7 @@ class VideoLatentSampler:
         ids = torch.tensor([[float(fps - 1), float(motion_bucket_id), float(noise_aug_strength)]], device=dev, dtype=F32).repeat(B, 1)
         if cfg:
             ids = torch.cat([ids, ids])
-        sigmas = karras_sigmas(num_inference_steps)
+        sigmas = karras_sigmas(num_inference_steps, sigma_min, sigma_max)
         if noise is None:
             noise = torch.randn(B, num_frames, 4, h, w, generator=generator, device=dev, dtype=F32)
         key = (B, num_frames, h, w, cfg, str(dev))
@@ -107,17 +107,24 @@ class VideoLatentSampler:
                     self._step(st)
                     continue
                 if self._graph is None:
-                    saved = st["latents"].clone()
-                    side = torch.cuda.Stream()
-                    side.wait_stream(torch.cuda.current_stream())
-                    with torch.cuda.stream(side):
-                        self._step(st)                     # warm-up: fills the weight-operand cache outside the capture
-                    torch.cuda.current_stream().wait_stream(side)
-                    st["latents"].copy_(saved)
-                    g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g):
-                        self._step(st)
-                    st["latents"].copy_(saved)
+                    # this graph replaces the module's own shape-keyed graphs (unet.enable_cuda_graphs) for the step: warm-up
+                    # and capture run the eager tape, so no graph of the sampling signature is left behind in the module
+                    module_graphs = getattr(self.unet, "_graphs", None)
+                    self.unet._graphs = None
+                    try:
+                        saved = st["latents"].clone()
+                        side = torch.cuda.Stream()
+                        side.wait_stream(torch.cuda.current_stream())
+                        with torch.cuda.stream(side):
+                            self._step(st)                 # warm-up: fills the weight-operand cache outside the capture
+                        torch.cuda.current_stream().wait_stream(side)
+                        st["latents"].copy_(saved)
+                        g = torch.cuda.CUDAGraph()
+                        with torch.cuda.graph(g):
+                            self._step(st)
+                        st["latents"].copy_(saved)
+                    finally:
+                        self.unet._graphs = module_graphs
                     self._graph, self._wstamp = g, wstamp
                 self._graph.replay()
         finally:

@@ -3,12 +3,16 @@
     python -m svd_xtend_b200.shim train_svd.py --pretrained_model_name_or_path=... [script args]
     accelerate launch -m svd_xtend_b200.shim train_svd.py ...
 
-Before the script body runs, the replacement class is installed under the two names the reference
-imports the UNet from: `diffusers.UNetSpatioTemporalConditionModel` (train_svd.py:49) and
-`src.unet_spatio_temporal_condition.UNetSpatioTemporalConditionModel` (train_svd_lora.py:60), and the EMA as
-`diffusers.training_utils.EMAModel` (train_svd.py:52, used with --use_ema), and, for a run with --use_8bit_adam, the 8-bit
-AdamW as `bitsandbytes.optim.AdamW8bit` (train_svd.py:746-773). Where transformers is
-importable, the image encoder is also installed as `transformers.CLIPVisionModelWithProjection` (train_svd.py:646-647).
+Before the script body runs, this package's classes are installed under the names the reference imports them from:
+  * the UNet as `diffusers.UNetSpatioTemporalConditionModel` (train_svd.py:49) and
+    `src.unet_spatio_temporal_condition.UNetSpatioTemporalConditionModel` (train_svd_lora.py:60);
+  * the VAE as `diffusers.AutoencoderKLTemporalDecoder` (train_svd.py:47-50; the per-step encode of :283-291 and the decode of
+    every validation video), in a subclass whose `from_pretrained` loads the temporal decoder, as diffusers' class has one;
+  * the pipeline as `diffusers.StableVideoDiffusionPipeline` (the validation loop, :1093-1157, and the final
+    `save_pretrained`, :1166-1180), built from the passed training modules;
+  * the EMA as `diffusers.training_utils.EMAModel` (train_svd.py:52, used with --use_ema);
+  * for a run with --use_8bit_adam, the 8-bit AdamW as `bitsandbytes.optim.AdamW8bit` (train_svd.py:746-773);
+  * where transformers is importable, the image encoder as `transformers.CLIPVisionModelWithProjection` (train_svd.py:646-647).
 diffusers / accelerate are NOT part of this image (no network), so this shim is exercised only where a
 user's environment provides them; it fails loudly when they are missing.
 """
@@ -35,13 +39,23 @@ def install(use_8bit_adam: bool | None = None) -> None:
         diffusers = importlib.import_module("diffusers")
     except ModuleNotFoundError as e:
         raise RuntimeError("svd_xtend_b200.shim: the reference scripts need `diffusers`, which is not installed here") from e
-    diffusers.UNetSpatioTemporalConditionModel = UNetSpatioTemporalConditionModel
-    for modname in ("diffusers.models", "diffusers.models.unets", "diffusers.models.unets.unet_spatio_temporal_condition"):
-        try:
-            m = importlib.import_module(modname)
-            setattr(m, "UNetSpatioTemporalConditionModel", UNetSpatioTemporalConditionModel)
-        except Exception:
-            pass
+    from .pipeline import StableVideoDiffusionPipeline
+    from .vae import AutoencoderKLTemporalDecoderWithDecoder
+    for name, cls, modnames in (
+            ("UNetSpatioTemporalConditionModel", UNetSpatioTemporalConditionModel,
+             ("diffusers.models", "diffusers.models.unets", "diffusers.models.unets.unet_spatio_temporal_condition")),
+            ("AutoencoderKLTemporalDecoder", AutoencoderKLTemporalDecoderWithDecoder,
+             ("diffusers.models", "diffusers.models.autoencoders", "diffusers.models.autoencoders.autoencoder_kl_temporal_decoder")),
+            ("StableVideoDiffusionPipeline", StableVideoDiffusionPipeline,
+             ("diffusers.pipelines", "diffusers.pipelines.stable_video_diffusion",
+              "diffusers.pipelines.stable_video_diffusion.pipeline_stable_video_diffusion"))):
+        setattr(diffusers, name, cls)
+        for modname in modnames:
+            try:
+                m = importlib.import_module(modname)
+                setattr(m, name, cls)
+            except Exception:
+                pass
     # train_svd_lora.py imports `from src.unet_spatio_temporal_condition import UNetSpatioTemporalConditionModel`
     pkg = sys.modules.get("src") or types.ModuleType("src")
     pkg.__path__ = getattr(pkg, "__path__", [])

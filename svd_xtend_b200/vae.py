@@ -31,6 +31,7 @@ import torch.nn as nn
 
 from . import raw
 from .engine import Engine, F32, Geom, Var, bf16
+from .unet import _Config
 
 
 class _Resnet(nn.Module):
@@ -215,10 +216,13 @@ class AutoencoderKLTemporalDecoder(nn.Module):
     config_name = "config.json"
 
     def __init__(self, in_channels=3, latent_channels=4, block_out_channels=(128, 256, 512, 512), layers_per_block=2,
-                 scaling_factor=0.18215, with_decoder=False, **ignored):
+                 scaling_factor=0.18215, with_decoder=False, force_upcast=True, **config):
+        """keyword arguments this model does not use (config.json's `out_channels`, `sample_size`, `down_block_types`, ...) are
+        kept on `self.config` and written back by `save_pretrained`"""
         super().__init__()
-        self.config = SimpleNamespace(in_channels=in_channels, latent_channels=latent_channels, block_out_channels=tuple(block_out_channels),
-                                      layers_per_block=layers_per_block, scaling_factor=scaling_factor)
+        self.config = _Config(**config)
+        self.config.__dict__.update(in_channels=in_channels, latent_channels=latent_channels, block_out_channels=tuple(block_out_channels),
+                                    layers_per_block=layers_per_block, scaling_factor=scaling_factor, force_upcast=force_upcast)
         if any(c % 32 for c in block_out_channels):
             raise ValueError("block_out_channels must be multiples of 32 (GroupNorm(32) and 32-column epilogue chunks)")
         self.encoder = _Encoder(in_channels, latent_channels, tuple(block_out_channels), layers_per_block)
@@ -236,13 +240,18 @@ class AutoencoderKLTemporalDecoder(nn.Module):
 
     @classmethod
     def from_pretrained(cls, path: str, subfolder: Optional[str] = None, torch_dtype=None, variant: Optional[str] = None,
-                        with_decoder: bool = False, **kw):
-        """with_decoder=False (the training path) drops the decoder.* tensors; True loads them too, strictly"""
+                        with_decoder: bool = False, revision: Optional[str] = None, low_cpu_mem_usage: bool = True, **kw):
+        """with_decoder=False (the training path) drops the decoder.* tensors; True loads them too, strictly. Local directories
+        only: a `revision` or a path that is not a directory raises ValueError. Every key of config.json is kept on `config`."""
+        if revision is not None:
+            raise ValueError(f"AutoencoderKLTemporalDecoder.from_pretrained: revision={revision!r} is not supported (local directories only)")
+        if not os.path.isdir(path):
+            raise ValueError(f"AutoencoderKLTemporalDecoder.from_pretrained: {path!r} is not a local directory (hub downloads are not supported)")
         d = path if subfolder is None else os.path.join(path, subfolder)
         with open(os.path.join(d, cls.config_name)) as f:
             cfg = json.load(f)
-        model = cls(**{k: v for k, v in cfg.items() if k in ("in_channels", "latent_channels", "block_out_channels", "layers_per_block", "scaling_factor")},
-                    with_decoder=with_decoder)
+        cfg.pop("with_decoder", None)
+        model = cls(**cfg, with_decoder=with_decoder)
         stems = ["diffusion_pytorch_model"] if variant is None else [f"diffusion_pytorch_model.{variant}", "diffusion_pytorch_model"]
         for stem in stems:
             p = os.path.join(d, stem + ".safetensors")
@@ -262,6 +271,30 @@ class AutoencoderKLTemporalDecoder(nn.Module):
         if torch_dtype is not None:
             model.to(torch_dtype)
         return model
+
+    def save_pretrained(self, save_directory: str, safe_serialization: bool = True, variant: Optional[str] = None, **kwargs):
+        """diffusers' layout: config.json (every config key, `_class_name` AutoencoderKLTemporalDecoder) and
+        diffusion_pytorch_model[.variant].safetensors (or .bin) with diffusers' keys, decoder.* included when built with it"""
+        os.makedirs(save_directory, exist_ok=True)
+        cfg = self.config.to_dict()
+        cfg["_class_name"] = "AutoencoderKLTemporalDecoder"
+        with open(os.path.join(save_directory, self.config_name), "w") as f:
+            json.dump(cfg, f, indent=2)
+        stem = "diffusion_pytorch_model" + ("" if variant is None else f".{variant}")
+        sd = {k: v.detach().cpu().contiguous() for k, v in self.state_dict().items()}
+        if safe_serialization:
+            from safetensors.torch import save_file
+            save_file(sd, os.path.join(save_directory, stem + ".safetensors"))
+        else:
+            torch.save(sd, os.path.join(save_directory, stem + ".bin"))
+
+    def forward(self, sample: torch.Tensor, sample_posterior: bool = False, return_dict: bool = True,
+                generator: Optional[torch.Generator] = None, num_frames: int = 1):
+        """[D] AutoencoderKLTemporalDecoder.forward: encode, the posterior's mode (or a sample), decode in clips of num_frames"""
+        posterior = self.encode(sample).latent_dist
+        z = posterior.sample(generator=generator) if sample_posterior else posterior.mode()
+        dec = self.decode(z, num_frames=num_frames).sample
+        return SimpleNamespace(sample=dec) if return_dict else (dec,)
 
     # ------------------------------------------------------------------ the encode path
     def encode(self, x: torch.Tensor, return_dict: bool = True):
@@ -445,6 +478,16 @@ class AutoencoderKLTemporalDecoder(nn.Module):
                     conv_whn=(g.W, g.H, N), bias=E.vec_f32(dec.conv_out.bias), block_n=32)
         out = torch.empty(N, Cout, g.H, g.W, device=dev, dtype=z.dtype if z.dtype in (bf16, torch.float16) else F32)
         return raw.time_conv_out(y, E.vec_f32(dec.time_conv_out.weight), E.vec_f32(dec.time_conv_out.bias), out, T)
+
+
+class AutoencoderKLTemporalDecoderWithDecoder(AutoencoderKLTemporalDecoder):
+    """the class svd_xtend_b200.shim installs as `diffusers.AutoencoderKLTemporalDecoder`: diffusers' class always has the
+    temporal decoder, so `from_pretrained` loads it unless told otherwise (the package's own default stays encoder-only)"""
+
+    @classmethod
+    def from_pretrained(cls, path: str, subfolder: Optional[str] = None, torch_dtype=None, variant: Optional[str] = None,
+                        with_decoder: bool = True, **kw):
+        return super().from_pretrained(path, subfolder=subfolder, torch_dtype=torch_dtype, variant=variant, with_decoder=with_decoder, **kw)
 
 
 def tensor_to_vae_latent(t: torch.Tensor, vae: AutoencoderKLTemporalDecoder, noise: Optional[torch.Tensor] = None, generator=None) -> torch.Tensor:
