@@ -1319,6 +1319,9 @@ extern "C" int svdx_nhwc_to_nchw(const void* src, int64_t lds, void* dst, int32_
 static int vec_ok(const void* a, const void* b, int C) {
   return a && b && C > 0 && C % 8 == 0 && !(reinterpret_cast<uintptr_t>(a) & 15) && !(reinterpret_cast<uintptr_t>(b) & 15);
 }
+static bool misaligned16(const void* p) { return reinterpret_cast<uintptr_t>(p) & 15; }
+// a row stride shorter than the row overlaps the next row; one row has no stride to check (torch gives a size-1 dim any stride)
+static bool short_ld(long long ld, long long width, long long nrows) { return nrows > 1 && ld < width; }
 
 extern "C" int svdx_upsample2x(const void* src, void* dst, int32_t N, int32_t H, int32_t W, int32_t C, void* stream) {
   if (!vec_ok(src, dst, C) || N <= 0 || H <= 0 || W <= 0) return svdx_fail(SVDX_E_BADARG, "upsample2x: bad arguments");
@@ -1388,6 +1391,7 @@ extern "C" int svdx_silu_f32(const float* x, float* y, int64_t n, void* stream) 
 extern "C" int svdx_colsum(const void* x, int64_t ldx, int64_t rows, int32_t cols, float* out, int32_t accumulate, void* stream) {
   if (!x || !out || rows <= 0 || cols <= 0 || cols % 8 || ldx % 8 || (reinterpret_cast<uintptr_t>(x) & 15))
     return svdx_fail(SVDX_E_BADARG, "colsum: bad arguments (cols, ldx multiples of 8; 16 B aligned)");
+  if (short_ld(ldx, cols, rows)) return svdx_fail(SVDX_E_BADARG, "colsum: ldx < cols");
   if (!accumulate) cudaMemsetAsync(out, 0, sizeof(float) * cols, ST(stream));
   const int col_blocks = (cols + 255) / 256;
   long long chunks = (4LL * svdx_num_sms() + col_blocks - 1) / col_blocks;
@@ -1404,6 +1408,11 @@ extern "C" int svdx_geglu_bwd(const void* pre, int64_t ldpre, const void* dout, 
                               int32_t h, float* bias_grad, void* stream) {
   if (!pre || !dout || !dpre || rows <= 0 || h <= 0 || h % 8 || ldpre % 8 || lddo % 8 || lddpre % 8)
     return svdx_fail(SVDX_E_BADARG, "geglu_bwd: bad arguments");
+  if (misaligned16(pre) || misaligned16(dout) || misaligned16(dpre))
+    return svdx_fail(SVDX_E_BADARG, "geglu_bwd: pre, dout and dpre must be 16-byte aligned");
+  if (short_ld(ldpre, 2LL * h, rows)) return svdx_fail(SVDX_E_BADARG, "geglu_bwd: ldpre < 2h");
+  if (short_ld(lddo, h, rows)) return svdx_fail(SVDX_E_BADARG, "geglu_bwd: lddo < h");
+  if (short_ld(lddpre, 2LL * h, rows)) return svdx_fail(SVDX_E_BADARG, "geglu_bwd: lddpre < 2h");
   if (!bias_grad) {
     geglu_bwd_plain_kernel<<<nblocks(rows * (h / 8)), 256, 0, ST(stream)>>>(reinterpret_cast<const bf16*>(pre), ldpre, reinterpret_cast<const bf16*>(dout), lddo,
                                                                       reinterpret_cast<bf16*>(dpre), lddpre, rows, h);
@@ -1427,6 +1436,8 @@ extern "C" int svdx_softmax_rows(const void* x, int64_t ldx, int64_t rows, int32
   if (!x || !y || rows <= 0 || cols <= 0 || cols % 8 || ldx % 8 || ldy % 8 || (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(y) & 15) ||
       rows > 0x7fffffffLL)
     return svdx_fail(SVDX_E_BADARG, "softmax_rows: bad arguments (cols, ldx, ldy multiples of 8; 16 B aligned)");
+  if (short_ld(ldx, cols, rows)) return svdx_fail(SVDX_E_BADARG, "softmax_rows: ldx < cols");
+  if (short_ld(ldy, cols, rows)) return svdx_fail(SVDX_E_BADARG, "softmax_rows: ldy < cols");
   softmax_rows_kernel<<<(unsigned)rows, 256, 0, ST(stream)>>>(reinterpret_cast<const bf16*>(x), ldx, cols, scale, reinterpret_cast<bf16*>(y), ldy);
   SVDX_CHECK_LAUNCH("softmax_rows");
   return SVDX_OK;
@@ -1437,6 +1448,9 @@ extern "C" int svdx_gemv(const void* a, int64_t lda, const void* w, int64_t ldw,
   if (!a || !w || !out || M <= 0 || M > 8 || N <= 0 || K <= 0 || K % 8 || lda % 8 || ldw % 8 || (reinterpret_cast<uintptr_t>(a) & 15) ||
       (reinterpret_cast<uintptr_t>(w) & 15) || (out_dtype != SVDX_OUT_BF16 && out_dtype != SVDX_OUT_F32))
     return svdx_fail(SVDX_E_BADARG, "gemv: bad arguments (M <= 8, K, lda, ldw multiples of 8, 16 B aligned, bf16 / fp32 output)");
+  if (short_ld(lda, K, M)) return svdx_fail(SVDX_E_BADARG, "gemv: lda < K");
+  if (short_ld(ldw, K, N)) return svdx_fail(SVDX_E_BADARG, "gemv: ldw < K");
+  if (short_ld(ldo, N, M)) return svdx_fail(SVDX_E_BADARG, "gemv: ldo < N");
   const unsigned blocks = (unsigned)(((long long)N * 32 + 255) / 256);
   const int f32 = out_dtype == SVDX_OUT_F32;
   const bf16* ap = reinterpret_cast<const bf16*>(a);
@@ -1454,6 +1468,9 @@ extern "C" int svdx_outer_accum(const void* dy, int64_t lddy, const void* x, int
   if (!dy || !x || !g || T <= 0 || T > 8 || O <= 0 || K <= 0 || K % 4 || ldx % 4 || ldg % 4 || (reinterpret_cast<uintptr_t>(x) & 7) ||
       (reinterpret_cast<uintptr_t>(g) & 15))
     return svdx_fail(SVDX_E_BADARG, "outer_accum: bad arguments (T <= 8, K, ldx, ldg multiples of 4, aligned)");
+  if (short_ld(lddy, O, T)) return svdx_fail(SVDX_E_BADARG, "outer_accum: lddy < O");
+  if (short_ld(ldx, K, T)) return svdx_fail(SVDX_E_BADARG, "outer_accum: ldx < K");
+  if (short_ld(ldg, K, O)) return svdx_fail(SVDX_E_BADARG, "outer_accum: ldg < K");
   outer_accum_kernel<<<nblocks((long long)O * (K / 4)), 256, 0, ST(stream)>>>(reinterpret_cast<const bf16*>(dy), lddy, reinterpret_cast<const bf16*>(x), ldx,
                                                                          T, O, K, scale, g, ldg);
   SVDX_CHECK_LAUNCH("outer_accum");
@@ -1684,6 +1701,7 @@ extern "C" int svdx_unprep_conv_grad(const float* src, float* dst, int32_t O, in
 
 extern "C" int svdx_dot_diff(const void* dy, const void* a, const void* b, int64_t n, float* out, void* stream) {
   if (!dy || !a || !b || !out || n <= 0 || n % 8) return svdx_fail(SVDX_E_BADARG, "dot_diff: bad arguments");
+  if (misaligned16(dy) || misaligned16(a) || misaligned16(b)) return svdx_fail(SVDX_E_BADARG, "dot_diff: dy, a and b must be 16-byte aligned");
   long long nvec = n / 8;
   unsigned grid = nblocks(nvec);
   const unsigned cap = 4u * (unsigned)svdx_num_sms();
@@ -1707,6 +1725,15 @@ extern "C" int svdx_splitk_epilogue(float* ws, int64_t ldw, void* out, int64_t l
   if (!ws || !out || rows <= 0 || cols <= 0 || cols % 8 || ldw % 4 || ldo % 8 || (res1 && ldr1 % 8) || (res2 && ldr2 % 8) ||
       (rowbias && rowbias_div <= 0))
     return svdx_fail(SVDX_E_BADARG, "splitk_epilogue: bad arguments");
+  if (misaligned16(ws)) return svdx_fail(SVDX_E_BADARG, "splitk_epilogue: ws must be 16-byte aligned");
+  if (misaligned16(out) || misaligned16(res1) || misaligned16(res2))
+    return svdx_fail(SVDX_E_BADARG, "splitk_epilogue: out, res1 and res2 must be 16-byte aligned");
+  if (short_ld(ldw, cols, rows)) return svdx_fail(SVDX_E_BADARG, "splitk_epilogue: ldw < cols");
+  if (short_ld(ldo, cols, rows)) return svdx_fail(SVDX_E_BADARG, "splitk_epilogue: ldo < cols");
+  if (res1 && short_ld(ldr1, cols, rows)) return svdx_fail(SVDX_E_BADARG, "splitk_epilogue: ldr1 < cols");
+  if (res2 && short_ld(ldr2, cols, rows)) return svdx_fail(SVDX_E_BADARG, "splitk_epilogue: ldr2 < cols");
+  if (rowbias && short_ld(ldrb, cols, (rows + rowbias_div - 1) / rowbias_div))
+    return svdx_fail(SVDX_E_BADARG, "splitk_epilogue: ldrb < cols");
   splitk_epilogue_kernel<<<nblocks(rows * (cols / 8)), 256, 0, ST(stream)>>>(ws, ldw, reinterpret_cast<bf16*>(out), ldo, rows, cols, bias, rowbias,
                                                                             rowbias_div, ldrb, reinterpret_cast<const bf16*>(res1), ldr1,
                                                                             reinterpret_cast<const bf16*>(res2), ldr2, scales);

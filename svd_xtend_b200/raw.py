@@ -820,24 +820,56 @@ def planes_to_space(src, dst, N, H, W, Cc):
     return dst
 
 
+def _flat_bf16(what: str, **ts) -> None:
+    """the concat / split / axpby kernels index their operands as flat bf16 arrays: anything else would be misread"""
+    for name, t in ts.items():
+        if t.dtype != bf16:
+            raise ValueError(f"{what}: {name} must be bfloat16, got {t.dtype}")
+        if not t.is_contiguous():
+            raise ValueError(f"{what}: {name} must be contiguous")
+
+
+def _channel_rows(what: str, **ts) -> int:
+    """the common row count of channels-last operands [..., C]"""
+    rows = {name: t.numel() // t.shape[-1] if t.dim() and t.shape[-1] else 0 for name, t in ts.items()}
+    if len(set(rows.values())) != 1:
+        raise ValueError(f"{what}: operands must have the same row count, got {rows}")
+    return next(iter(rows.values()))
+
+
 def concat_channels(a, b, dst):
+    _flat_bf16("concat_channels", a=a, b=b, dst=dst)
+    rows = _channel_rows("concat_channels", a=a, b=b, dst=dst)
+    if dst.shape[-1] != a.shape[-1] + b.shape[-1]:
+        raise ValueError(f"concat_channels: dst has {dst.shape[-1]} channels, a and b {a.shape[-1]} + {b.shape[-1]}")
     if _fam("elementwise", 0.0, 4.0 * dst.numel()):
         return dst
-    check(load().svdx_concat_channels(a.data_ptr(), a.shape[-1], b.data_ptr(), b.shape[-1], dst.data_ptr(), a.numel() // a.shape[-1],
-                                      _stream()), "concat_channels")
+    check(load().svdx_concat_channels(a.data_ptr(), a.shape[-1], b.data_ptr(), b.shape[-1], dst.data_ptr(), rows, _stream()),
+          "concat_channels")
     return dst
 
 
 def split_channels(src, a, b, accumulate_a=False):
+    """a = src[..., :Ca] (a += with accumulate_a, one bf16 rounding of the fp32 sum) and b = src[..., Ca:]; b None drops those channels"""
+    ops = dict(src=src, a=a) if b is None else dict(src=src, a=a, b=b)
+    _flat_bf16("split_channels", **ops)
+    rows = _channel_rows("split_channels", **ops)
     Ca = a.shape[-1]
     Cb = src.shape[-1] - Ca
+    if b is not None and b.shape[-1] != Cb:
+        raise ValueError(f"split_channels: src has {src.shape[-1]} channels, a and b {Ca} + {b.shape[-1]}")
     if _fam("elementwise", 0.0, 4.0 * src.numel()):
         return
-    check(load().svdx_split_channels(src.data_ptr(), a.data_ptr(), Ca, _ptr(b), Cb, src.numel() // src.shape[-1], int(accumulate_a),
-                                     _stream()), "split_channels")
+    check(load().svdx_split_channels(src.data_ptr(), a.data_ptr(), Ca, _ptr(b), Cb, rows, int(accumulate_a), _stream()), "split_channels")
 
 
 def axpby(a, b, y, scales=None):
+    """y = scales[0] * a + scales[1] * b over flat bf16 tensors (scales: device fp32 [2]; None = 1, 1)"""
+    _flat_bf16("axpby", a=a, b=b, y=y)
+    if not a.numel() == b.numel() == y.numel():
+        raise ValueError(f"axpby: a, b and y must have the same length, got {a.numel()}, {b.numel()}, {y.numel()}")
+    if scales is not None and (scales.dtype != torch.float32 or scales.numel() < 2):
+        raise ValueError("axpby: scales must be fp32 with at least 2 elements")
     if _fam("elementwise", 0.0, 6.0 * a.numel()):
         return y
     check(load().svdx_axpby_bf16(a.data_ptr(), b.data_ptr(), _ptr(scales), y.data_ptr(), a.numel(), _stream()), "axpby_bf16")
