@@ -457,6 +457,23 @@ int svdx_adamw8bit_mul(const void* jobs, const int32_t* block_prefix, int32_t nj
 int svdx_adamw8bit_ema_mul(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
                            const float* qmap2, float* state, float grad_scale, double* ema_state, const float* grad_mul, void* stream);
 
+/* Sharded block-wise 8-bit AdamW over NVLink peer memory (P2PShardedAdamW8bit): reduce-scatter + svdx_adamw8bit + all-gather as
+ * ONE kernel, replacing DistributedDataParallel's all-reduce + bitsandbytes.optim.AdamW8bit of train_svd.py:746-773,815-824,
+ * 1044-1049 at N > 1. jobs: DEVICE array of this rank's sub-jobs
+ *   {float* p; void* s1; void* s2; float* absmax1; float* absmax2; float* ema; int64 off; int64 n; int64 quant}
+ * each a whole number of 256-element blocks of one parameter (a parameter that straddles a shard boundary is split by block
+ * range; s1 / s2 / absmax1 / absmax2 / ema point at the sub-job's first block), p / state / EMA this rank's local buffers, and
+ * off the arena offset of p[0]. Per element the gradient is sum over r = 0 .. world-1, in rank order from 0, of grads[r][off + i]
+ * (the FULL gradient arenas, peer-mapped, as svdx_adamw_p2p sums), times grad_scale (= 1 / world) and grad_mul[0] when grad_mul
+ * is not NULL; the update is svdx_adamw8bit's, bit for bit (same roundings, block absmax and maps; no FMA, no atomics); the new
+ * bf16 value is stored to shadows[r][off + i] of every rank. tick != 0 first advances state (and ema_state when given) as
+ * svdx_adamw_p2p does. ema_state NULL: no EMA; otherwise every job's ema is advanced as in svdx_adamw8bit_ema. The caller
+ * orders the ranks around the launch as for svdx_adamw_p2p. grads[r] / shadows[r]: 16-byte aligned; world 1 .. 16. Two launches
+ * with tick, one without. */
+int svdx_adamw8bit_p2p(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
+                       const float* qmap2, const void* const* grads, void* const* shadows, int32_t world, float* state,
+                       float grad_scale, int32_t tick, double* ema_state, const float* grad_mul, void* stream);
+
 /* Batch assembly of a training step from video frames (train_svd.py:942-1017; svd_xtend_b200.video_train). Every operation is
  * rounded separately (no FMA), in the reference's order.
  * svdx_vae_frames_in: the VAE encoder's input rows, bf16 [(B*F + B) * H*W][c_pad] (token-major, channels >= 3 zero), as

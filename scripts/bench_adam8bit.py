@@ -2,6 +2,9 @@
 """8-bit AdamW benchmark (train_svd.py --use_8bit_adam) on the H100 path, one JSON line.
 
     python scripts/bench_adam8bit.py [--steps K] [--warmup W]
+    python scripts/bench_adam8bit.py --sharded nccl|p2p --world N
+
+--sharded times the sharded forms' update instead (see `sharded()` below); without it:
 
 Measured in one process on one GPU:
   1. the config-2 train step of bench.py (seeded default-init SVD UNet, as-scripted trainable set, one CUDA graph) captured
@@ -35,7 +38,11 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--sharded", choices=("nccl", "p2p"), default=None)
+    ap.add_argument("--world", type=int, default=1)
     args = ap.parse_args()
+    if args.sharded is not None:
+        return sharded(args.sharded, args.world)
 
     from svd_xtend_b200.optim8bit import AdamW8bit, state_bytes, update_bytes
     from svd_xtend_b200.train import FusedAdamW, FusedAdamW8bit, GraphedStep, ParamArena
@@ -172,6 +179,98 @@ def main():
             "power_limit_w": power_limit_w(0), "train_step": train_step, "optimizer_pass": opt_pass, "script_loop": script,
             "memory": memory}
     sys.stdout.flush()
+    print(json.dumps(line), flush=True)
+
+
+HBM_TBPS = 3.35     # H100 SXM data-sheet HBM3 bandwidth
+
+
+def sharded(form: str, world: int):
+    """One rank's optimizer update of ShardedAdamW8bit (form "nccl") or P2PShardedAdamW8bit ("p2p") at world size `world`, on the
+    config-2 arena (the as-scripted trainable set, 397,620,480 parameters) and on the whole UNet, CUDA events over many launches.
+
+    world 1 times the real optimizer's step(). At world N > 1 the N ranks are emulated on one device: rank 0's optimizer is built
+    over its own arena with torch.distributed stood in for, and the peer pointer lists point at local buffers, one gradient and
+    one shadow slice per rank (only the owned slice [lo, hi) of a peer arena is ever addressed, so each peer buffer covers just
+    that slice). These are LOCAL-HBM timings, not NVLink: the peers' gradient reads and shadow writes go to this card's memory.
+    "p2p" times the one-kernel step (tick + svdx_adamw8bit_p2p, the fences left out); "nccl" times the svdx_adamw8bit launch
+    over rank 0's sub-jobs only (tick + update; the reduce-scatter and the all-gather are not measured). Bytes are counted from
+    shapes (svd_xtend_b200.optim8bit.update_bytes: the local HBM traffic, the emulated peer traffic included)."""
+    from types import SimpleNamespace
+
+    import torch.distributed as dist
+
+    from oracle.svd_unet_oracle import SVD_CONFIG
+    from svd_xtend_b200 import train
+    from svd_xtend_b200.optim8bit import update_bytes
+    from svd_xtend_b200.unet import UNetSpatioTemporalConditionModel
+
+    if not torch.cuda.is_available():
+        raise RuntimeError("bench_adam8bit.py needs a CUDA device: the optimizer kernels have no CPU fallback")
+    if not 1 <= world <= 16:
+        raise ValueError("--world is 1 .. 16")
+    dev = torch.device("cuda", 0)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    cls = train.P2PShardedAdamW8bit if form == "p2p" else train.ShardedAdamW8bit
+    out = {}
+    for which in ("as_scripted", "whole_unet"):
+        with torch.device("meta"):
+            m = UNetSpatioTemporalConditionModel(**SVD_CONFIG)
+        shapes = [p.shape for n, p in m.named_parameters() if which == "whole_unet" or "temporal_transformer_block" in n]
+        net = torch.nn.Module()
+        net.ps = torch.nn.ParameterList([torch.nn.Parameter(torch.empty(s, device=dev).normal_(0, 0.02)) for s in shapes])
+        arena = train.ParamArena(net, pad_to=world * 256, block=256)
+        arena.grad.normal_()
+        peers = None
+        saved = train.dist, train.map_peer_buffers
+        if world > 1:
+            shard = arena.numel // world
+            peers = [(torch.empty(shard, device=dev).normal_(), torch.empty(shard, device=dev, dtype=torch.bfloat16))
+                     for _ in range(world - 1)]
+            train.dist = SimpleNamespace(is_initialized=lambda: True, get_world_size=lambda group=None: world,
+                                         get_rank=lambda group=None: 0, get_backend=lambda group=None: "nccl",
+                                         ReduceOp=dist.ReduceOp, all_reduce=lambda *a, **k: None)
+            # rank 0 owns [0, shard): a peer slice buffer is addressed from the peer arena's base, here its own start
+            train.map_peer_buffers = lambda t, group=None: [t.data_ptr()] + [(g if t.dtype == torch.float32 else s).data_ptr()
+                                                                              for g, s in peers]
+        try:
+            opt = cls(arena, lr=1e-5)
+            if form == "nccl" and world > 1:
+                def fn():
+                    opt._launch(1.0 / world, None)
+            else:
+                def fn():
+                    opt.step()
+            for _ in range(3):
+                fn()
+            launches = 20
+            times = []
+            for _ in range(3):
+                torch.cuda.synchronize()
+                e0.record()
+                for _ in range(launches):
+                    fn()
+                e1.record()
+                torch.cuda.synchronize()
+                times.append(e0.elapsed_time(e1) / launches)
+        finally:
+            train.dist, train.map_peer_buffers = saved
+        n8 = sum(n for _, _, n, q, _, _ in opt.subjobs if q)
+        n32 = sum(n for _, _, n, q, _, _ in opt.subjobs if not q)
+        nbytes = update_bytes(n8, n32, shadow=True, ema=False, world=world if form == "p2p" else 1)
+        ms = statistics.median(times)
+        out[which] = {"ms": ms, "ms_windows": times, "params": sum(p.numel() for p in arena.params), "rank_params": n8 + n32,
+                      "rank_params_8bit": n8, "bytes": nbytes, "gbps": nbytes / ms / 1e6,
+                      "share_of_hbm_peak": nbytes / ms / 1e6 / (HBM_TBPS * 1e3), "finite": bool(torch.isfinite(arena.data).all())}
+        del opt, arena, net, peers, m
+        gc.collect()
+        torch.cuda.empty_cache()
+    what = ("the optimizer's step()" if world == 1 else
+            "rank 0's launch of N emulated ranks on one card (LOCAL-HBM timing, not NVLink): "
+            + ("tick + svdx_adamw8bit_p2p" if form == "p2p" else "tick + svdx_adamw8bit over its sub-jobs, without the NCCL collectives"))
+    line = {"metric": f"sharded 8-bit AdamW ({form}) update, one rank of {world}", "value": out["as_scripted"]["ms"], "unit": "ms",
+            "higher_is_better": False, "form": form, "world": world, "what": what + ", CUDA events over 20 launches, medians of 3",
+            "hbm_peak_tbps": HBM_TBPS, "card": torch.cuda.get_device_name(dev), "power_limit_w": power_limit_w(0), **out}
     print(json.dumps(line), flush=True)
 
 

@@ -6,7 +6,10 @@
      fp32 masters everywhere;
  (3) the same step as ONE kernel over NVLink peer memory (P2PShardedAdamW), eager and replayed from a CUDA graph;
  (4) checkpoint and resume of ShardedAdamW: train at world N, state_dict() (collective), continue; a fresh optimizer that loads
-     the dict at world N continues bit for bit, and one at world N/2 (a subgroup) ends on masters within the tolerance of (2)."""
+     the dict at world N continues bit for bit, and one at world N/2 (a subgroup) ends on masters within the tolerance of (2);
+ (5) the sharded 8-bit forms (ShardedAdamW8bit, P2PShardedAdamW8bit) against FusedAdamW8bit.step(1/N) over the rank-order sum of
+     the ranks' gradients, three steps: the P2P form bit for bit, the NCCL form (whose reduce-scatter sums in its own order)
+     within the tolerance of (2); every rank's operands identical; state_dict() (collective) equal to FusedAdamW8bit's."""
 import os
 import sys
 
@@ -14,7 +17,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import torch.distributed as dist
 
-from svd_xtend_b200.train import FusedAdamW, GradReducer, P2PShardedAdamW, ParamArena, ShardedAdamW
+from svd_xtend_b200.train import (FusedAdamW, FusedAdamW8bit, GradReducer, P2PShardedAdamW, P2PShardedAdamW8bit, ParamArena,
+                                  ShardedAdamW, ShardedAdamW8bit)
 from svd_xtend_b200.unet import UNetSpatioTemporalConditionModel
 from svd_xtend_b200.workload import edm_loss, synthetic_batch
 
@@ -30,7 +34,7 @@ dev = torch.device("cuda", local)
 dist.init_process_group("nccl", device_id=dev)
 
 
-def build(pad_world=None):
+def build(pad_world=None, block=64):
     torch.manual_seed(0)
     unet = UNetSpatioTemporalConditionModel(**TINY).to(dev)
     unet.requires_grad_(False)
@@ -38,7 +42,7 @@ def build(pad_world=None):
         if "temporal_transformer_block" in n:
             p.requires_grad_(True)
     unet.train()
-    arena = ParamArena(unet, pad_to=(pad_world or world) * 64)
+    arena = ParamArena(unet, pad_to=(pad_world or world) * (256 if block == 256 else 64), block=block)
     unet.attach_arena(arena)
     return unet, arena
 
@@ -209,6 +213,50 @@ if half and rank < half:
     assert e_half < 1e-3 and opt_h.t == 6
 elif not half:
     print(f"[ddp_check] rank {rank}: world 1: no smaller world to resume at", flush=True)
+# ---- (5) the sharded 8-bit forms against FusedAdamW8bit on the rank-order sum of the gradients. Every rank draws every rank's
+# seeded gradients, so each can form the sum in rank order.
+def grads8(a, r, t):
+    g = torch.Generator(device=dev).manual_seed(1000 * t + r)
+    out = torch.zeros_like(a.grad)
+    for p in a.params:
+        o = a.offset_of[p]
+        out[o:o + p.numel()] = torch.randn(p.numel(), generator=g, device=dev) * 1e-2
+    return out
+
+
+for cls in (P2PShardedAdamW8bit, ShardedAdamW8bit):
+    _, a_ref = build(block=256)
+    _, a8 = build(block=256)
+    ref8 = FusedAdamW8bit(a_ref, lr=1e-3, weight_decay=1e-2, min_8bit_size=1024)
+    o8 = cls(a8, lr=1e-3, weight_decay=1e-2, min_8bit_size=1024)
+    w8 = a8.data.clone()
+    for t in range(3):
+        ref8.lr = o8.lr = 1e-3 / (1 + t)
+        gs = [grads8(a8, r, t) for r in range(world)]
+        total = torch.zeros_like(a8.grad)
+        for x in gs:
+            total += x
+        a_ref.grad.copy_(total)
+        a8.grad.copy_(gs[rank])
+        ref8.step(1.0 / world)
+        o8.step()
+    torch.cuda.synchronize()
+    lo, hi = o8.lo, o8.hi
+    if cls is P2PShardedAdamW8bit:
+        ok_own = torch.equal(a8.data[lo:hi], a_ref.data[lo:hi])
+    else:
+        ok_own = ((a8.data[lo:hi] - a_ref.data[lo:hi]).norm() / (a_ref.data[lo:hi] - w8[lo:hi]).norm()).item() < 1e-3
+    others = [torch.empty_like(a8.shadow) for _ in range(world)]
+    dist.all_gather(others, a8.shadow)
+    same8 = all(torch.equal(o, a8.shadow) for o in others)
+    sd8, sdr = o8.state_dict(), ref8.state_dict()
+    sd_equal = all(torch.equal(v, sdr["state"][i][k]) if isinstance(v, torch.Tensor) else v == sdr["state"][i][k]
+                   for i in sdr["state"] for k, v in sd8["state"][i].items())
+    exact = cls is P2PShardedAdamW8bit
+    print(f"[ddp_check] rank {rank}: {cls.__name__}: own masters vs FusedAdamW8bit on the rank-order sum "
+          f"({'bit for bit' if exact else 'rel-l2 of the update < 1e-3'}): {ok_own}, operands identical across ranks: {same8}, "
+          f"state_dict equal to FusedAdamW8bit's: {sd_equal if exact else 'not compared (other summation order)'}, t = {o8.t}", flush=True)
+    assert ok_own and same8 and o8.t == 3 and (sd_equal or not exact)
 dist.barrier()
 torch.cuda.synchronize()
 sys.stdout.flush()

@@ -131,6 +131,8 @@ _PROTOS = {
                                c_void_p, c_void_p, c_void_p, c_void_p],
     "svdx_adamw8bit_mul": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p],
     "svdx_adamw8bit_ema_mul": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p],
+    "svdx_adamw8bit_p2p": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_float, c_int,
+                           c_void_p, c_void_p, c_void_p],
     "svdx_multi_transpose": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p],
     "svdx_lora_merge": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p],
     "svdx_vae_frames_in": [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p],

@@ -792,8 +792,72 @@ struct Adam8Job {
   long long n;
   long long quant;
 };
+// A job of the peer-memory form (svdx_adamw8bit_p2p): one rank's share of a parameter, a whole number of its 256-element blocks
+// (s1 / s2 / absmax1 / absmax2 / ema already point at the share's first block). The gradient is the rank-order sum of every
+// rank's gradient arena at `off`, and the new bf16 value goes to every rank's shadow arena at `off`.
+struct Adam8P2PJob {
+  float* p;
+  void* s1;
+  void* s2;
+  float* absmax1;
+  float* absmax2;
+  float* ema;
+  long long off;        // arena offset of p[0]
+  long long n;
+  long long quant;
+};
+struct Adam8Peers {     // the peer arenas of the P2P form (AdamP2P's pointers and the rank count)
+  AdamP2P ptr;
+  int world;
+};
+struct Adam8NoPeers {};
+template <bool P2P> using Adam8JobT = std::conditional_t<P2P, Adam8P2PJob, Adam8Job>;
+template <bool P2P> using Adam8Src = std::conditional_t<P2P, Adam8Peers, Adam8NoPeers>;
+
 constexpr int A8_BLOCK = 256;
 constexpr int A8_WARPS = 8;       // 256 threads per CTA, one warp per block at a time
+
+// eight gradient elements at element `base` of the job: its own g, or (P2P) the rank-order sum of every rank's arena, summed
+// as adamw_p2p_kernel sums (from 0, up to four ranks' loads in flight)
+template <bool P2P>
+SVDX_DEVINL void a8_load_grad8(const Adam8JobT<P2P>& j, const Adam8Src<P2P>& src, long long base, float (&gg)[8]) {
+  if constexpr (!P2P) {
+    const float4 g0 = __ldg(reinterpret_cast<const float4*>(j.g + base)), g1 = __ldg(reinterpret_cast<const float4*>(j.g + base + 4));
+    gg[0] = g0.x; gg[1] = g0.y; gg[2] = g0.z; gg[3] = g0.w; gg[4] = g1.x; gg[5] = g1.y; gg[6] = g1.z; gg[7] = g1.w;
+  } else {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) gg[k] = 0.f;
+#pragma unroll 1
+    for (int r0 = 0; r0 < src.world; r0 += 4) {
+      float4 t[4][2];
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        if (r0 + q < src.world) {
+          const float* g = src.ptr.grad[r0 + q] + j.off + base;
+          t[q][0] = __ldcg(reinterpret_cast<const float4*>(g));
+          t[q][1] = __ldcg(reinterpret_cast<const float4*>(g + 4));
+        }
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        if (r0 + q < src.world) {
+          gg[0] = __fadd_rn(gg[0], t[q][0].x); gg[1] = __fadd_rn(gg[1], t[q][0].y);
+          gg[2] = __fadd_rn(gg[2], t[q][0].z); gg[3] = __fadd_rn(gg[3], t[q][0].w);
+          gg[4] = __fadd_rn(gg[4], t[q][1].x); gg[5] = __fadd_rn(gg[5], t[q][1].y);
+          gg[6] = __fadd_rn(gg[6], t[q][1].z); gg[7] = __fadd_rn(gg[7], t[q][1].w);
+        }
+    }
+  }
+}
+template <bool P2P>
+SVDX_DEVINL float a8_load_grad1(const Adam8JobT<P2P>& j, const Adam8Src<P2P>& src, long long i) {
+  if constexpr (!P2P) {
+    return j.g[i];
+  } else {
+    float g = 0.f;
+    for (int r = 0; r < src.world; ++r) g = __fadd_rn(g, __ldcg(src.ptr.grad[r] + j.off + i));
+    return g;
+  }
+}
 
 SVDX_DEVINL int a8_code(const float* mid, float x) {
   // #{k : mid[k] < x} over 255 sorted midpoints (mid[255] = +inf): a tie goes to the lower code
@@ -804,11 +868,14 @@ SVDX_DEVINL int a8_code(const float* mid, float x) {
   return c;
 }
 
-template <bool EMA>
-__global__ void __launch_bounds__(256) adamw8bit_kernel(const Adam8Job* __restrict__ jobs, const int* __restrict__ block_prefix, int njobs,
-                                                        int total_blocks, const float* __restrict__ qmap1, const float* __restrict__ qmap2,
-                                                        const float* __restrict__ state, float gscale, const double* __restrict__ ema_state,
-                                                        const float* __restrict__ gmul) {
+// P2P: the jobs are Adam8P2PJob; the gradient is loaded from every rank's arena and the shadow stored to every rank's (see
+// svdx_adamw8bit_p2p). The arithmetic is the same code in both forms.
+template <bool EMA, bool P2P = false>
+__global__ void __launch_bounds__(256) adamw8bit_kernel(const Adam8JobT<P2P>* __restrict__ jobs, const int* __restrict__ block_prefix,
+                                                        int njobs, int total_blocks, const float* __restrict__ qmap1,
+                                                        const float* __restrict__ qmap2, const float* __restrict__ state, float gscale,
+                                                        const double* __restrict__ ema_state, const float* __restrict__ gmul,
+                                                        const __grid_constant__ Adam8Src<P2P> src) {
   __shared__ float q1[256], q2[256], mid1[256], mid2[256];
   if (gmul) gscale = __fmul_rn(gscale, *gmul);
   for (int k = threadIdx.x; k < 256; k += blockDim.x) {
@@ -833,23 +900,23 @@ __global__ void __launch_bounds__(256) adamw8bit_kernel(const Adam8Job* __restri
       const int mid = (lo + hi + 1) >> 1;
       if (block_prefix[mid] <= b) lo = mid; else hi = mid - 1;
     }
-    const Adam8Job j = jobs[lo];
+    const Adam8JobT<P2P> j = jobs[lo];
     const int blk = b - block_prefix[lo];
     const long long base = (long long)blk * A8_BLOCK + lane * 8;
     const long long rem = j.n - base;
     const int cnt = rem >= 8 ? 8 : (rem > 0 ? (int)rem : 0);
     const bool quant = j.quant != 0;
-    const uintptr_t a16 = reinterpret_cast<uintptr_t>(j.p) | reinterpret_cast<uintptr_t>(j.g) |
-                          (j.shadow ? reinterpret_cast<uintptr_t>(j.shadow) : 0) | (EMA ? reinterpret_cast<uintptr_t>(j.ema) : 0) |
-                          (quant ? 0 : reinterpret_cast<uintptr_t>(j.s1) | reinterpret_cast<uintptr_t>(j.s2));
+    uintptr_t a16 = reinterpret_cast<uintptr_t>(j.p) | (EMA ? reinterpret_cast<uintptr_t>(j.ema) : 0) |
+                    (quant ? 0 : reinterpret_cast<uintptr_t>(j.s1) | reinterpret_cast<uintptr_t>(j.s2));
+    if constexpr (P2P) a16 |= (uintptr_t)(j.off * 2);     // the peer arenas are 16-byte aligned: g at 4 * off, shadow at 2 * off
+    else a16 |= reinterpret_cast<uintptr_t>(j.g) | (j.shadow ? reinterpret_cast<uintptr_t>(j.shadow) : 0);
     const bool vec = cnt == 8 && (a16 & 15) == 0 &&
                      (!quant || ((reinterpret_cast<uintptr_t>(j.s1) | reinterpret_cast<uintptr_t>(j.s2)) & 7) == 0);
     float pp[8], gg[8], mm[8], vv[8];
     if (vec) {
       const float4 p0 = *reinterpret_cast<const float4*>(j.p + base), p1 = *reinterpret_cast<const float4*>(j.p + base + 4);
-      const float4 g0 = __ldg(reinterpret_cast<const float4*>(j.g + base)), g1 = __ldg(reinterpret_cast<const float4*>(j.g + base + 4));
+      a8_load_grad8<P2P>(j, src, base, gg);
       pp[0] = p0.x; pp[1] = p0.y; pp[2] = p0.z; pp[3] = p0.w; pp[4] = p1.x; pp[5] = p1.y; pp[6] = p1.z; pp[7] = p1.w;
-      gg[0] = g0.x; gg[1] = g0.y; gg[2] = g0.z; gg[3] = g0.w; gg[4] = g1.x; gg[5] = g1.y; gg[6] = g1.z; gg[7] = g1.w;
       if (quant) {
         const uint2 c1 = *reinterpret_cast<const uint2*>(reinterpret_cast<const uint8_t*>(j.s1) + base);
         const uint2 c2 = *reinterpret_cast<const uint2*>(reinterpret_cast<const uint8_t*>(j.s2) + base);
@@ -875,7 +942,7 @@ __global__ void __launch_bounds__(256) adamw8bit_kernel(const Adam8Job* __restri
         pp[k] = gg[k] = mm[k] = vv[k] = 0.f;
         if (k < cnt) {
           pp[k] = j.p[base + k];
-          gg[k] = j.g[base + k];
+          gg[k] = a8_load_grad1<P2P>(j, src, base + k);
           if (quant) {
             mm[k] = __fmul_rn(q1[reinterpret_cast<const uint8_t*>(j.s1)[base + k]], a1);
             vv[k] = __fmul_rn(q2[reinterpret_cast<const uint8_t*>(j.s2)[base + k]], a2);
@@ -927,9 +994,13 @@ __global__ void __launch_bounds__(256) adamw8bit_kernel(const Adam8Job* __restri
         *reinterpret_cast<float4*>(v) = make_float4(vv[0], vv[1], vv[2], vv[3]);
         *reinterpret_cast<float4*>(v + 4) = make_float4(vv[4], vv[5], vv[6], vv[7]);
       }
-      if (j.shadow)
-        *reinterpret_cast<uint4*>(j.shadow + base) = make_uint4(pack_bf16x2(pp[0], pp[1]), pack_bf16x2(pp[2], pp[3]),
-                                                                pack_bf16x2(pp[4], pp[5]), pack_bf16x2(pp[6], pp[7]));
+      const uint4 sh = make_uint4(pack_bf16x2(pp[0], pp[1]), pack_bf16x2(pp[2], pp[3]), pack_bf16x2(pp[4], pp[5]),
+                                  pack_bf16x2(pp[6], pp[7]));
+      if constexpr (P2P) {
+        for (int r = 0; r < src.world; ++r) *reinterpret_cast<uint4*>(src.ptr.shadow[r] + j.off + base) = sh;
+      } else if (j.shadow) {
+        *reinterpret_cast<uint4*>(j.shadow + base) = sh;
+      }
       if constexpr (EMA) {
         const float4 e0 = *reinterpret_cast<float4*>(j.ema + base), e1 = *reinterpret_cast<float4*>(j.ema + base + 4);
         *reinterpret_cast<float4*>(j.ema + base) = ema_update4(e0, pp, omd);
@@ -948,7 +1019,11 @@ __global__ void __launch_bounds__(256) adamw8bit_kernel(const Adam8Job* __restri
             reinterpret_cast<float*>(j.s1)[base + k] = mm[k];
             reinterpret_cast<float*>(j.s2)[base + k] = vv[k];
           }
-          if (j.shadow) j.shadow[base + k] = __float2bfloat16_rn(pp[k]);
+          if constexpr (P2P) {
+            for (int r = 0; r < src.world; ++r) src.ptr.shadow[r][j.off + base + k] = __float2bfloat16_rn(pp[k]);
+          } else if (j.shadow) {
+            j.shadow[base + k] = __float2bfloat16_rn(pp[k]);
+          }
           if constexpr (EMA) j.ema[base + k] = ema_update(j.ema[base + k], pp[k], omd);
         }
       }
@@ -958,6 +1033,7 @@ __global__ void __launch_bounds__(256) adamw8bit_kernel(const Adam8Job* __restri
       j.absmax2[blk] = amax2;
     }
   }
+  if constexpr (P2P) __threadfence_system();     // the peer stores are performed system-wide before this kernel counts as complete
 }
 
 // row softmax of a bf16 score matrix, y[r][:] = softmax(scale * x[r][:]) (fp32 arithmetic, in place allowed): the single-head,
@@ -1547,11 +1623,11 @@ static int adamw8bit_launch(const void* jobs, const int32_t* block_prefix, int32
   if (ema) {
     adamw_ema_tick_kernel<<<1, 1, 0, ST(stream)>>>(state, ema_state);
     adamw8bit_kernel<true><<<(unsigned)blocks, 256, 0, ST(stream)>>>(j, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, ema_state,
-                                                                      grad_mul);
+                                                                      grad_mul, Adam8NoPeers{});
   } else {
     adamw_tick_kernel<<<1, 1, 0, ST(stream)>>>(state);
     adamw8bit_kernel<false><<<(unsigned)blocks, 256, 0, ST(stream)>>>(j, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, nullptr,
-                                                                       grad_mul);
+                                                                       grad_mul, Adam8NoPeers{});
   }
   SVDX_CHECK_LAUNCH(ema ? "adamw8bit_ema" : "adamw8bit");
   return SVDX_OK;
@@ -1576,6 +1652,41 @@ extern "C" int svdx_adamw8bit_ema_mul(const void* jobs, const int32_t* block_pre
                                       const float* qmap1, const float* qmap2, float* state, float grad_scale, double* ema_state,
                                       const float* grad_mul, void* stream) {
   return adamw8bit_launch(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, ema_state, true, grad_mul, stream);
+}
+
+extern "C" int svdx_adamw8bit_p2p(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
+                                  const float* qmap2, const void* const* grads, void* const* shadows, int32_t world, float* state,
+                                  float grad_scale, int32_t tick, double* ema_state, const float* grad_mul, void* stream) {
+  if (!jobs || !block_prefix || !qmap1 || !qmap2 || !grads || !shadows || !state || njobs <= 0 || total_blocks <= 0 || world < 1 ||
+      world > 16 || (reinterpret_cast<uintptr_t>(jobs) & 7) || (reinterpret_cast<uintptr_t>(block_prefix) & 3) ||
+      (reinterpret_cast<uintptr_t>(qmap1) & 3) || (reinterpret_cast<uintptr_t>(qmap2) & 3) || (reinterpret_cast<uintptr_t>(state) & 3) ||
+      (reinterpret_cast<uintptr_t>(ema_state) & 7) || (reinterpret_cast<uintptr_t>(grad_mul) & 3))
+    return svdx_fail(SVDX_E_BADARG, "adamw8bit_p2p: bad arguments (device job table, block prefix, maps, state[8], world 1..16, "
+                                    "8-byte aligned ema_state[9])");
+  Adam8Peers src{};
+  src.world = world;
+  for (int r = 0; r < world; ++r) {
+    if (!grads[r] || !shadows[r] || (reinterpret_cast<uintptr_t>(grads[r]) & 15) || (reinterpret_cast<uintptr_t>(shadows[r]) & 15))
+      return svdx_fail(SVDX_E_BADARG, "adamw8bit_p2p: null / misaligned peer arena (16-byte aligned gradient and shadow arenas)");
+    src.ptr.grad[r] = reinterpret_cast<const float*>(grads[r]);
+    src.ptr.shadow[r] = reinterpret_cast<bf16*>(shadows[r]);
+  }
+  if (tick) {
+    if (ema_state) adamw_ema_tick_kernel<<<1, 1, 0, ST(stream)>>>(state, ema_state);
+    else adamw_tick_kernel<<<1, 1, 0, ST(stream)>>>(state);
+  }
+  long long blocks = (total_blocks + A8_WARPS - 1) / A8_WARPS;
+  const long long cap = (long long)svdx_num_sms() * 8;
+  if (blocks > cap) blocks = cap;
+  const Adam8P2PJob* j = reinterpret_cast<const Adam8P2PJob*>(jobs);
+  if (ema_state)
+    adamw8bit_kernel<true, true><<<(unsigned)blocks, 256, 0, ST(stream)>>>(j, block_prefix, njobs, total_blocks, qmap1, qmap2, state,
+                                                                            grad_scale, ema_state, grad_mul, src);
+  else
+    adamw8bit_kernel<false, true><<<(unsigned)blocks, 256, 0, ST(stream)>>>(j, block_prefix, njobs, total_blocks, qmap1, qmap2, state,
+                                                                             grad_scale, nullptr, grad_mul, src);
+  SVDX_CHECK_LAUNCH("adamw8bit_p2p");
+  return SVDX_OK;
 }
 
 static int adamw_p2p_launch(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo, int64_t n,

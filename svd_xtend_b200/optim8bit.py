@@ -60,18 +60,21 @@ def state_bytes(numels, min_8bit_size: int = 4096) -> int:
     return total
 
 
-def update_bytes(n8: int, n32: int, shadow: bool, ema: bool) -> float:
-    """HBM bytes one update moves: p r/w, g, m and v r/w (1-byte codes + absmax, or fp32), the bf16 shadow, the EMA r/w"""
-    extra = (2.0 if shadow else 0.0) + (8.0 if ema else 0.0)
+def update_bytes(n8: int, n32: int, shadow: bool, ema: bool, world: int = 1) -> float:
+    """HBM bytes one update moves: p r/w, g, m and v r/w (1-byte codes + absmax, or fp32), the bf16 shadow, the EMA r/w; with
+    world > 1 (svdx_adamw8bit_p2p) also the other ranks' gradients read and shadows written, 6 bytes per element and peer"""
+    extra = (2.0 if shadow else 0.0) + (8.0 if ema else 0.0) + 6.0 * (world - 1)
     return (12.0 + extra) * (n8 + n32) + 4.0 * n8 + 16.0 * n8 / BLOCK + 16.0 * n32
 
 
 class JobTable:
     """device job table + block prefix of one svdx_adamw8bit launch. Rows are kept on the host as an int64 array; `set`
-    copies them to the device only when a pointer changed (e.g. gradients re-allocated by zero_grad(set_to_none=True))."""
+    copies them to the device only when a pointer changed (e.g. gradients re-allocated by zero_grad(set_to_none=True)).
+    n_field: the column of the job length (8 in svdx_adamw8bit's rows, 7 in svdx_adamw8bit_p2p's)."""
 
-    def __init__(self, device):
+    def __init__(self, device, n_field: int = 8):
         self.device = device
+        self.n_field = n_field
         self.rows = None
         self.dev = None
         self.prefix = None
@@ -80,7 +83,7 @@ class JobTable:
     def set(self, rows: np.ndarray):
         if self.rows is not None and self.rows.shape == rows.shape and np.array_equal(self.rows, rows):
             return
-        counts = [num_blocks(int(n)) for n in rows[:, 8]]
+        counts = [num_blocks(int(n)) for n in rows[:, self.n_field]]
         prefix = np.zeros(len(counts), dtype=np.int32)
         if len(counts) > 1:
             prefix[1:] = np.cumsum(counts[:-1])
@@ -99,6 +102,14 @@ class JobTable:
 
 def job_row(p: int, g: int, s1: int, s2: int, a1: int, a2: int, shadow: int, ema: int, n: int, quant: bool):
     return (p, g, s1, s2, a1, a2, shadow, ema, n, 1 if quant else 0)
+
+
+# job row of svdx_adamw8bit_p2p: p, s1, s2, absmax1, absmax2, ema, arena offset, n, quant (nine 8-byte fields)
+P2P_JOB_FIELDS = 9
+
+
+def p2p_job_row(p: int, s1: int, s2: int, a1: int, a2: int, ema: int, off: int, n: int, quant: bool):
+    return (p, s1, s2, a1, a2, ema, off, n, 1 if quant else 0)
 
 
 def check_param_state(st: dict, p: torch.Tensor, min_8bit_size: int, what: str) -> None:

@@ -33,7 +33,7 @@ _KERNELS_PER_CALL = {"svdx_groupnorm_apply_fused": 1, "svdx_attention_bwd": 3, "
                      "svdx_adamw_graph_ema": 2, "svdx_adamw_p2p_ema": 2, "svdx_ema_multi": 2, "svdx_adamw8bit": 2,
                      "svdx_adamw8bit_ema": 2, "svdx_adamw_graph_mul": 2, "svdx_adamw_graph_ema_mul": 2, "svdx_adamw8bit_mul": 2,
                      "svdx_adamw8bit_ema_mul": 2, "svdx_adamw_p2p_mul": 2, "svdx_adamw_p2p_ema_mul": 2, "svdx_grad_sumsq": 2,
-                     "svdx_grad_sumsq_p2p": 2}
+                     "svdx_grad_sumsq_p2p": 2, "svdx_adamw8bit_p2p": 2}
 
 
 def check(rc: int, what: str = "") -> None:
@@ -1057,6 +1057,31 @@ def adamw8bit(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad
         args += (ema_state.data_ptr(),)
     name = "svdx_adamw8bit" + ("_ema" if ema_state is not None else "") + ("_mul" if gm is not None else "")
     check(getattr(load(), name)(*args, *(() if gm is None else (gm,)), _stream()), name)
+
+
+def adamw8bit_p2p(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, peer_grads, peer_shadows, state, grad_scale, tick=True,
+                  ema_state=None, nbytes=0.0, grad_mul=None):
+    """sharded 8-bit AdamW over NVLink peer memory in one launch (svdx_adamw8bit_p2p; tick + update when `tick`): jobs is the
+    device table of this rank's sub-jobs (svd_xtend_b200.h), peer_grads / peer_shadows the FULL arenas of every rank as for
+    adamw_p2p. ema_state: advance every job's EMA too; grad_mul: the clip coefficient (device fp32). nbytes is for the byte
+    accounting only."""
+    if qmap1.dtype != torch.float32 or qmap2.dtype != torch.float32 or qmap1.numel() != 256 or qmap2.numel() != 256:
+        raise ValueError("adamw8bit_p2p: qmap1 / qmap2 are float32[256]")
+    if ema_state is not None and (ema_state.dtype != torch.float64 or ema_state.numel() < 9):
+        raise ValueError("adamw8bit_p2p: ema_state is float64[9] (svd_xtend_b200.h)")
+    if len(peer_grads) != len(peer_shadows):
+        raise ValueError("adamw8bit_p2p: one gradient and one shadow arena per rank")
+    gm = _grad_mul(grad_mul)
+    if _fam("adamw", 0.0, nbytes):
+        return
+    world = len(peer_grads)
+    ga = (C.c_void_p * world)(*[t if isinstance(t, int) else t.data_ptr() for t in peer_grads])
+    sa = (C.c_void_p * world)(*[t if isinstance(t, int) else t.data_ptr() for t in peer_shadows])
+    rc = load().svdx_adamw8bit_p2p(jobs.data_ptr(), block_prefix.data_ptr(), njobs, total_blocks, qmap1.data_ptr(), qmap2.data_ptr(),
+                                   ga, sa, world, state.data_ptr(), float(grad_scale), int(tick), _ptr(ema_state), gm, _stream())
+    if not tick:
+        LAUNCHES[0] -= 1          # check() counts the tick + update pair
+    check(rc, "svdx_adamw8bit_p2p")
 
 
 def multi_transpose(src_base, jobs, tile_prefix, njobs, total_tiles):

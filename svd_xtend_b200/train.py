@@ -28,8 +28,14 @@ class ParamArena:
     """Flattens the trainable parameters (in registration order) into one fp32 buffer; every parameter's
     `.data` becomes a view, and a same-shaped gradient arena provides `.grad` views."""
 
-    def __init__(self, module: torch.nn.Module, params: Optional[Iterable[torch.nn.Parameter]] = None, pad_to: int = 64):
-        """pad_to: the flat length is rounded up to a multiple of it (ShardedAdamW: world_size * 64, equal 256-byte aligned shards)"""
+    def __init__(self, module: torch.nn.Module, params: Optional[Iterable[torch.nn.Parameter]] = None, pad_to: int = 64,
+                 block: int = 64):
+        """pad_to: the flat length is rounded up to a multiple of it (ShardedAdamW: world_size * 64, equal 256-byte aligned shards).
+        block: every parameter starts at a multiple of it (a multiple of 64). The sharded 8-bit optimizers need
+        ParamArena(..., pad_to=world_size * 256, block=256): then every 256-element quantisation block, counted from its
+        parameter's first element, lies in one shard."""
+        if block <= 0 or block % 64:
+            raise ValueError(f"ParamArena: block must be a positive multiple of 64, got {block}")
         ps = [p for p in (params if params is not None else module.parameters()) if p.requires_grad]
         if not ps:
             raise ValueError("ParamArena: no trainable parameters")
@@ -37,12 +43,13 @@ class ParamArena:
         if any(p.dtype != F32 for p in ps):
             raise ValueError("ParamArena expects fp32 master parameters (train_svd.py loads the UNet in fp32)")
         self.params: List[torch.nn.Parameter] = ps
+        self.block = block
         # 64-element alignment keeps every view 256-byte aligned (vector loads, TMA-friendly)
         self.offsets: List[int] = []
         off = 0
         for p in ps:
             self.offsets.append(off)
-            off += (p.numel() + 63) // 64 * 64
+            off += (p.numel() + block - 1) // block * block
         off = (off + pad_to - 1) // pad_to * pad_to
         self.numel = off
         self.data = torch.zeros(off, device=dev, dtype=F32)
@@ -444,24 +451,25 @@ class FusedAdamW(_ArenaAdamW):
         self._set_hyper(load_adamw_state_dict(self.arena, sd, self.m, self.v))
 
 
-class FusedAdamW8bit(_ArenaAdamW):
-    """FusedAdamW with block-wise 8-bit moments (bitsandbytes' AdamW8bit, train_svd.py --use_8bit_adam; the update is stated in
-    oracle/svd_adam8bit_oracle.py): a parameter with at least `min_8bit_size` elements keeps m / v as uint8 codes plus one fp32
-    absmax per 256-element block counted from its own arena offset (arena padding belongs to no block); a smaller one keeps
-    fp32 m / v. ONE tick + ONE launch over every parameter (`svdx_adamw8bit`), with the same device `state` float[8] as
-    FusedAdamW, so a captured GraphedStep replays the right sequence. About 2.03 bytes of state per parameter instead of 8.
-    The update is deterministic, so under GradReducer every rank's replica stays identical."""
+_STATE_KEY = {"codes1": "state1", "codes2": "state2", "absmax1": "absmax1", "absmax2": "absmax2", "m32": "state1", "v32": "state2"}
+
+
+class _Arena8bit(_ArenaAdamW):
+    """The block-wise 8-bit state of FusedAdamW8bit and its sharded forms. `layout` is the unsharded one, per parameter
+    (param, arena offset, quant, state offset (codes / fp32 elements), absmax offset), into buffers laid out as FusedAdamW8bit
+    keeps them (one absmax per 256-element block counted from the parameter's first element). An optimizer that owns the arena
+    range [lo, hi) keeps only the part of those buffers its range covers: its sub-jobs (one per parameter it touches, a whole
+    number of blocks) cover a contiguous range of each unsharded buffer, [c0, c1) of the codes, [b0, b1) of the absmax and
+    [f0, f1) of the fp32 states, so the owned state of every rank is one slice of FusedAdamW8bit's buffers."""
 
     _moment_buffers = ("codes1", "codes2", "absmax1", "absmax2", "m32", "v32")
 
-    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, min_8bit_size: int = 4096,
-                 max_grad_norm: Optional[float] = None):
+    def _init_8bit(self, min_8bit_size: int, lo: int, hi: int):
         from .optim8bit import dynamic_map, num_blocks
-        super().__init__(arena, lr, betas, weight_decay, eps, max_grad_norm)
         self.min_8bit_size = int(min_8bit_size)
+        arena = self.arena
         dev = arena.data.device
         self.qmap1, self.qmap2 = dynamic_map(True).to(dev), dynamic_map(False).to(dev)
-        # per parameter: (param, arena offset, quant, state offset (codes / fp32 elements), absmax offset)
         self.layout: List[tuple] = []
         codes, blocks, f32 = 0, 0, 0
         for p in arena.params:
@@ -473,72 +481,120 @@ class FusedAdamW8bit(_ArenaAdamW):
             else:
                 self.layout.append((p, arena.offset_of[p], False, f32, 0))
                 f32 += (n + 63) // 64 * 64
-        self.codes1 = torch.zeros(codes, dtype=torch.uint8, device=dev)
-        self.codes2 = torch.zeros(codes, dtype=torch.uint8, device=dev)
-        self.absmax1 = torch.zeros(blocks, dtype=F32, device=dev)
-        self.absmax2 = torch.zeros(blocks, dtype=F32, device=dev)
-        self.m32 = torch.zeros(f32, dtype=F32, device=dev)
-        self.v32 = torch.zeros(f32, dtype=F32, device=dev)
-        self._table = None
         self._index = {p: i for i, (p, *_r) in enumerate(self.layout)}
+        self.subjobs, self.ranges = self._subjobs(lo, hi)
+        (c0, c1), (b0, b1), (f0, f1) = self.ranges
+        self.codes1 = torch.zeros(c1 - c0, dtype=torch.uint8, device=dev)
+        self.codes2 = torch.zeros(c1 - c0, dtype=torch.uint8, device=dev)
+        self.absmax1 = torch.zeros(b1 - b0, dtype=F32, device=dev)
+        self.absmax2 = torch.zeros(b1 - b0, dtype=F32, device=dev)
+        self.m32 = torch.zeros(f1 - f0, dtype=F32, device=dev)
+        self.v32 = torch.zeros(f1 - f0, dtype=F32, device=dev)
+        self._table = None
+
+    def _subjobs(self, lo: int, hi: int):
+        """the sub-jobs of the arena range [lo, hi): (param, arena offset a, length n, quant, state index, absmax index) with the
+        indices into the UNSHARDED buffers, and the ranges ((c0, c1), (b0, b1), (f0, f1)) of those buffers that they cover"""
+        from .optim8bit import num_blocks
+        jobs = []
+        rng = [[None, 0], [None, 0], [None, 0]]
+        for p, off, quant, so, bo in self.layout:
+            a, b = max(off, lo), min(off + p.numel(), hi)
+            if a >= b:
+                continue
+            d, n = a - off, b - a
+            if quant:
+                if d % 256:
+                    raise ValueError(f"{type(self).__name__}: a quantisation block of a parameter crosses the shard boundary {a}")
+                jobs.append((p, a, n, True, so + d, bo + d // 256))
+                ext = ((so + d, so + d + num_blocks(n) * 256), (bo + d // 256, bo + d // 256 + num_blocks(n)))
+                for r, (x, y) in zip(rng[:2], ext):
+                    r[0] = x if r[0] is None else r[0]
+                    r[1] = y
+            else:
+                jobs.append((p, a, n, False, so + d, 0))
+                r = rng[2]
+                r[0] = so + d if r[0] is None else r[0]
+                r[1] = so + d + (n + 63) // 64 * 64
+        return jobs, tuple((0, 0) if x is None else (x, y) for x, y in rng)
 
     def attach_ema(self, ema):
         super().attach_ema(ema)
         self._table = None          # the job table carries the EMA's addresses
 
-    def state_views(self, p: torch.nn.Parameter) -> Dict[str, torch.Tensor]:
-        """this parameter's optimizer state as views into the flat buffers (bitsandbytes' keys, without step)"""
-        _, _, quant, so, bo = self.layout[self._index[p]]
-        n = p.numel()
+    def _state_ptrs(self, quant: bool, si: int, bi: int):
+        """device addresses (s1, s2, absmax1, absmax2) of a sub-job whose unsharded state / absmax indices are si / bi"""
+        (c0, _), (b0, _), (f0, _) = self.ranges
         if quant:
-            nb = (n + 255) // 256
-            return {"state1": self.codes1[so:so + n].view(p.shape), "state2": self.codes2[so:so + n].view(p.shape),
-                    "qmap1": self.qmap1, "qmap2": self.qmap2, "absmax1": self.absmax1[bo:bo + nb], "absmax2": self.absmax2[bo:bo + nb]}
-        return {"state1": self.m32[so:so + n].view(p.shape), "state2": self.v32[so:so + n].view(p.shape)}
+            return (self.codes1.data_ptr() + si - c0, self.codes2.data_ptr() + si - c0, self.absmax1.data_ptr() + 4 * (bi - b0),
+                    self.absmax2.data_ptr() + 4 * (bi - b0))
+        return self.m32.data_ptr() + 4 * (si - f0), self.v32.data_ptr() + 4 * (si - f0), 0, 0
 
     def job_rows(self):
-        """the launch's job table as an int64 array [params, 10] (svd_xtend_b200.h, svdx_adamw8bit)"""
+        """the svdx_adamw8bit job table of this optimizer's sub-jobs as an int64 array [jobs, 10] (svd_xtend_b200.h)"""
         import numpy as np
         from .optim8bit import job_row
         a = self.arena
         pb, gb = a.data.data_ptr(), a.grad.data_ptr()
         sb = a.shadow.data_ptr() if a.shadow is not None else 0
         eb = self.ema._flat.data_ptr() if self.ema is not None else 0
-        rows = []
-        for p, off, quant, so, bo in self.layout:
-            if quant:
-                s1, s2 = self.codes1.data_ptr() + so, self.codes2.data_ptr() + so
-                a1, a2 = self.absmax1.data_ptr() + 4 * bo, self.absmax2.data_ptr() + 4 * bo
-            else:
-                s1, s2, a1, a2 = self.m32.data_ptr() + 4 * so, self.v32.data_ptr() + 4 * so, 0, 0
-            rows.append(job_row(pb + 4 * off, gb + 4 * off, s1, s2, a1, a2, sb + 2 * off if sb else 0, eb + 4 * off if eb else 0,
-                                p.numel(), quant))
+        rows = [job_row(pb + 4 * off, gb + 4 * off, *self._state_ptrs(quant, si, bi), sb + 2 * off if sb else 0,
+                        eb + 4 * off if eb else 0, n, quant)
+                for p, off, n, quant, si, bi in self.subjobs]
         return np.array(rows, dtype=np.int64).reshape(-1, 10)
 
-    def step(self, grad_scale: float = 1.0):
+    def _job_table(self, rows_fn, n_field: int, world: int = 1):
         from .optim8bit import JobTable, update_bytes
         if self._table is None:
-            self._table = JobTable(self.arena.data.device)
-            self._table.set(self.job_rows())
-            n8 = sum(p.numel() for p, _, q, _, _ in self.layout if q)
-            self._nbytes = update_bytes(n8, sum(p.numel() for p in self.arena.params) - n8, self.arena.shadow is not None, self.ema is not None)
-        tb = self._table
-        coef = None
-        if self._clip is not None:
-            raw.grad_sumsq(self.arena.grad, self._sumsq)
-            coef = self._clip_coef(grad_scale)
+            self._table = JobTable(self.arena.data.device, n_field)
+            self._table.set(rows_fn())
+            n8 = sum(n for _, _, n, q, _, _ in self.subjobs if q)
+            n32 = sum(n for _, _, n, q, _, _ in self.subjobs if not q)
+            self._nbytes = update_bytes(n8, n32, self.arena.shadow is not None, self.ema is not None, world)
+        return self._table
+
+    def _launch(self, grad_scale: float, coef: Optional[torch.Tensor]):
+        """tick + svdx_adamw8bit over this optimizer's sub-jobs, gradients read from the arena at the parameters' offsets"""
+        tb = self._job_table(self.job_rows, 8)
         raw.adamw8bit(tb.dev, tb.prefix, tb.njobs, tb.blocks, self.qmap1, self.qmap2, self.state, grad_scale,
                       ema_state=None if self.ema is None else self.ema._state, nbytes=self._nbytes, grad_mul=coef)
-        self._updated()
 
     # ---- checkpoints in bitsandbytes' per-parameter layout (svd_xtend_b200.optim8bit.AdamW8bit loads them too) ----
-    def state_dict(self) -> dict:
-        step = self.t
-        st = {}
-        for i, (p, *_r) in enumerate(self.layout):
-            d = {k: (v if k.startswith("qmap") else v.clone()) for k, v in self.state_views(p).items()}
+    def _param_view(self, i: int, name: str, flat: torch.Tensor) -> Optional[torch.Tensor]:
+        """parameter i's part of the UNSHARDED moment buffer `name` (flat), None if that buffer holds none of its state"""
+        p, _, quant, so, bo = self.layout[i]
+        n = p.numel()
+        if quant and name in ("codes1", "codes2"):
+            return flat[so:so + n].view(p.shape)
+        if quant and name in ("absmax1", "absmax2"):
+            return flat[bo:bo + (n + 255) // 256]
+        if not quant and name in ("m32", "v32"):
+            return flat[so:so + n].view(p.shape)
+        return None
+
+    def _param_states(self, bufs) -> Dict[int, dict]:
+        """per parameter index, a copy of its state in bitsandbytes' keys (without step) from (name, unsharded buffer) pairs; each
+        pair's slices are copied before the next pair is drawn, so an iterator may hand out one temporary after another"""
+        got: Dict[int, dict] = {i: {} for i in range(len(self.layout))}
+        for name, flat in bufs:
+            for i in got:
+                v = self._param_view(i, name, flat)
+                if v is not None:
+                    got[i][_STATE_KEY[name]] = v.clone()
+        return {i: self._ordered(i, d) for i, d in got.items()}
+
+    def _ordered(self, i: int, got: dict) -> dict:
+        """parameter i's state in FusedAdamW8bit's key order, the shared maps included"""
+        if not self.layout[i][2]:
+            return {k: got[k] for k in ("state1", "state2")}
+        return {"state1": got["state1"], "state2": got["state2"], "qmap1": self.qmap1, "qmap2": self.qmap2,
+                "absmax1": got["absmax1"], "absmax2": got["absmax2"]}
+
+    def _state_dict_of(self, bufs, step: int) -> dict:
+        """FusedAdamW8bit's state dict from (name, unsharded buffer) pairs (see _param_states)"""
+        st = self._param_states(bufs)
+        for d in st.values():
             d["step"] = step
-            st[i] = d
         group = {"lr": self._lr, "betas": tuple(self.betas), "eps": self.eps, "weight_decay": self.weight_decay, "amsgrad": False,
                  "optim_bits": 8, "min_8bit_size": self.min_8bit_size, "percentile_clipping": 100, "block_wise": True,
                  "is_paged": False, "params": list(range(len(self.layout)))}
@@ -546,96 +602,114 @@ class FusedAdamW8bit(_ArenaAdamW):
 
     @torch.no_grad()
     def load_state_dict(self, sd: dict) -> None:
+        """load a state dict of FusedAdamW8bit, of the drop-in AdamW8bit over the same parameters, or of a sharded form saved at any
+        world size; local (no collective): this optimizer copies the blocks it owns. Every check runs before anything is
+        written; ValueError if the dict does not fit."""
+        who = f"{type(self).__name__}.load_state_dict"
         groups = sd["param_groups"]
         if len(groups) != 1 or len(groups[0]["params"]) != len(self.layout):
-            raise ValueError("FusedAdamW8bit.load_state_dict: one group over the arena's parameters expected")
+            raise ValueError(f"{who}: one group over the arena's parameters expected")
         g = groups[0]
         if int(g.get("min_8bit_size", self.min_8bit_size)) != self.min_8bit_size:
-            raise ValueError("FusedAdamW8bit.load_state_dict: saved with a different min_8bit_size")
-        from .optim8bit import check_param_state
-        steps = set()
-        maps_done = False
+            raise ValueError(f"{who}: saved with a different min_8bit_size")
+        from .optim8bit import check_param_state, num_blocks
         missing = [i for i in g["params"] if i not in sd["state"]]
         if missing:
-            raise ValueError(f"FusedAdamW8bit.load_state_dict: no state for parameters {missing[:8]} (they never had a gradient in "
+            raise ValueError(f"{who}: no state for parameters {missing[:8]} (they never had a gradient in "
                              "the saved run); the fused form keeps one step count for all parameters and needs every one")
-        for (p, *_r), i in zip(self.layout, g["params"]):
+        steps, maps, srcs = set(), None, []
+        for (p, _, quant, _, _), i in zip(self.layout, g["params"]):
             src = {k: (v.contiguous() if isinstance(v, torch.Tensor) else v) for k, v in sd["state"][i].items()}
-            check_param_state(src, p, self.min_8bit_size, f"FusedAdamW8bit.load_state_dict: parameter {i}")
-            dst = self.state_views(p)
+            check_param_state(src, p, self.min_8bit_size, f"{who}: parameter {i}")
+            want = {"state1": (tuple(p.shape), torch.uint8 if quant else F32), "state2": (tuple(p.shape), torch.uint8 if quant else F32)}
+            if quant:
+                want.update(absmax1=((num_blocks(p.numel()),), F32), absmax2=((num_blocks(p.numel()),), F32))
             for k in ("state1", "state2", "absmax1", "absmax2"):
-                if (k in dst) != (k in src):
-                    raise ValueError(f"FusedAdamW8bit.load_state_dict: parameter {i} has a different state form")
-                if k in dst:
-                    if src[k].shape != dst[k].shape or src[k].dtype != dst[k].dtype:
-                        raise ValueError(f"FusedAdamW8bit.load_state_dict: {k} of parameter {i} has shape {tuple(src[k].shape)} "
-                                         f"{src[k].dtype}, expected {tuple(dst[k].shape)} {dst[k].dtype}")
-                    dst[k].copy_(src[k])
+                if (k in want) != (k in src):
+                    raise ValueError(f"{who}: parameter {i} has a different state form")
+                if k in want and (tuple(src[k].shape), src[k].dtype) != want[k]:
+                    raise ValueError(f"{who}: {k} of parameter {i} has shape {tuple(src[k].shape)} "
+                                     f"{src[k].dtype}, expected {want[k][0]} {want[k][1]}")
             if "qmap1" in src:
-                if not maps_done:
-                    self.qmap1.copy_(src["qmap1"])
-                    self.qmap2.copy_(src["qmap2"])
-                    maps_done = True
-                elif not (torch.equal(src["qmap1"].to(self.qmap1.device), self.qmap1) and torch.equal(src["qmap2"].to(self.qmap2.device), self.qmap2)):
-                    raise ValueError("FusedAdamW8bit.load_state_dict: parameters carry different quantisation maps")
+                if maps is None:
+                    maps = (src["qmap1"], src["qmap2"])
+                elif not (torch.equal(src["qmap1"].cpu(), maps[0].cpu()) and torch.equal(src["qmap2"].cpu(), maps[1].cpu())):
+                    raise ValueError(f"{who}: parameters carry different quantisation maps")
             steps.add(int(src.get("step", 0)))
+            srcs.append(src)
         if len(steps) > 1:
-            raise ValueError("FusedAdamW8bit.load_state_dict: parameters at different step counts (one device counter here)")
-        b1, b2 = g.get("betas", self.betas)
-        self._set_hyper({"lr": float(g.get("lr", self._lr)), "betas": (b1, b2), "eps": g.get("eps", self.eps),
-                         "weight_decay": g.get("weight_decay", self.weight_decay), "step": float(steps.pop() if steps else 0), "extra": {}})
+            raise ValueError(f"{who}: parameters at different step counts (one device counter here)")
+        if maps is not None:
+            self.qmap1.copy_(maps[0])
+            self.qmap2.copy_(maps[1])
+        (c0, c1), (b0, b1), (f0, f1) = self.ranges
+        for (p, _, quant, so, bo), src in zip(self.layout, srcs):
+            n = p.numel()
+            if quant:
+                parts = (("codes1", "state1", so, n, c0, c1), ("codes2", "state2", so, n, c0, c1),
+                         ("absmax1", "absmax1", bo, num_blocks(n), b0, b1), ("absmax2", "absmax2", bo, num_blocks(n), b0, b1))
+            else:
+                parts = (("m32", "state1", so, n, f0, f1), ("v32", "state2", so, n, f0, f1))
+            for buf, key, start, length, r0, r1 in parts:
+                x, y = max(start, r0), min(start + length, r1)
+                if x < y:
+                    getattr(self, buf)[x - r0:y - r0].copy_(src[key].reshape(-1)[x - start:y - start])
+        b1_, b2_ = g.get("betas", self.betas)
+        self._set_hyper({"lr": float(g.get("lr", self._lr)), "betas": (b1_, b2_), "eps": g.get("eps", self.eps),
+                         "weight_decay": g.get("weight_decay", self.weight_decay), "step": float(steps.pop() if steps else 0),
+                         "extra": {}})
 
 
-class ShardedAdamW(_ArenaAdamW):
-    """Data-parallel update with the optimizer state SHARDED over the ranks (ZeRO-1 on the flat arenas), all in NCCL
-    collectives that capture into the step's CUDA graph:
+class FusedAdamW8bit(_Arena8bit):
+    """FusedAdamW with block-wise 8-bit moments (bitsandbytes' AdamW8bit, train_svd.py --use_8bit_adam; the update is stated in
+    oracle/svd_adam8bit_oracle.py): a parameter with at least `min_8bit_size` elements keeps m / v as uint8 codes plus one fp32
+    absmax per 256-element block counted from its own arena offset (arena padding belongs to no block); a smaller one keeps
+    fp32 m / v. ONE tick + ONE launch over every parameter (`svdx_adamw8bit`), with the same device `state` float[8] as
+    FusedAdamW, so a captured GraphedStep replays the right sequence. About 2.03 bytes of state per parameter instead of 8.
+    The update is deterministic, so under GradReducer every rank's replica stays identical."""
 
-        reduce-scatter(sum) of the fp32 gradient arena   -> this rank's 1/N slice of the summed gradient   (in place)
-        fused AdamW on that slice (grad_scale = 1/N)       -> fp32 masters + moments of the slice, bf16 shadow of the slice
-        all-gather of the bf16 shadow                       -> every rank has all updated operand weights   (in place)
-
-    versus all-reduce + replicated AdamW this moves 0.75x the bytes over NVLink (1/2 for the reduce-scatter + 1/4 for the bf16
-    all-gather) and does 1/N of the optimizer's 30 B/parameter of HBM traffic per rank. The fp32 masters of slices a rank does
-    not own go stale on it (only their bf16 operand copies are kept current): call `gather_masters()` before saving a
-    checkpoint or reading `p.data` of arbitrary parameters. Semantics of the update itself = torch.optim.AdamW on the MEAN
-    gradient, as DistributedDataParallel + AdamW would give (train_svd.py:767-773, :815-824)."""
-
-    _moment_buffers = ("m", "v")
-    _ema_sharded = True
-
-    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, group=None,
+    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, min_8bit_size: int = 4096,
                  max_grad_norm: Optional[float] = None):
         super().__init__(arena, lr, betas, weight_decay, eps, max_grad_norm)
+        self._init_8bit(min_8bit_size, 0, arena.numel)
+
+    def _own(self):
+        return [(x, getattr(self, x)) for x in self._moment_buffers]
+
+    def state_views(self, p: torch.nn.Parameter) -> Dict[str, torch.Tensor]:
+        """this parameter's optimizer state as views into the flat buffers (bitsandbytes' keys, without step)"""
+        i = self._index[p]
+        views = ((x, self._param_view(i, x, f)) for x, f in self._own())
+        return self._ordered(i, {_STATE_KEY[x]: v for x, v in views if v is not None})
+
+    def step(self, grad_scale: float = 1.0):
+        coef = None
+        if self._clip is not None:
+            raw.grad_sumsq(self.arena.grad, self._sumsq)
+            coef = self._clip_coef(grad_scale)
+        self._launch(grad_scale, coef)
+        self._updated()
+
+    def state_dict(self) -> dict:
+        return self._state_dict_of(self._own(), self.t)
+
+
+class _Shards:
+    """The data-parallel sharding of the ZeRO-1 optimizers: rank r owns the arena slice [lo, hi) of length numel / world, the
+    gradient is summed into the owner's slice, and the owners' updated slices are gathered back. Needs `arena` and `ema`."""
+
+    _ema_sharded = True
+
+    def _shard(self, group, unit: int, hint: str):
+        """world, rank and [lo, hi) over `group`; ValueError naming `hint` (the ParamArena call to use) unless the arena splits
+        into `world` equal slices of a multiple of `unit` elements"""
         self.group = group
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
-        if arena.numel % (self.world * 64):
-            raise ValueError(f"ShardedAdamW: build the arena with ParamArena(..., pad_to={self.world * 64}) (equal, aligned shards)")
-        n = arena.numel // self.world
+        if self.arena.numel % (self.world * unit):
+            raise ValueError(f"{type(self).__name__}: build the arena with {hint}")
+        n = self.arena.numel // self.world
         self.lo, self.hi = self.rank * n, (self.rank + 1) * n
-        self.m = torch.zeros(n, device=arena.data.device, dtype=F32)
-        self.v = torch.zeros(n, device=arena.data.device, dtype=F32)
-
-    def state_dict(self) -> dict:
-        """COLLECTIVE: every rank calls it and gets the same full torch.optim.AdamW state dict (rank 0 saves it). m, then v, is
-        all-gathered into one temporary arena-length fp32 buffer and copied to the CPU before the next gather, so the peak
-        extra device memory is one arena (1.6 GB for the as-scripted temporal set, 6.1 GB for the whole UNet). Call
-        gather_masters() too before saving the weights."""
-        return adamw_state_dict(self.arena, self.t, self._hyper(), self._gathered_moments())
-
-    def _gathered_moments(self):
-        tmp = torch.empty_like(self.arena.data)
-        for mine in (self.m, self.v):
-            tmp[self.lo:self.hi].copy_(mine)
-            self.all_gather_(tmp)
-            yield tmp
-
-    @torch.no_grad()
-    def load_state_dict(self, sd: dict) -> None:
-        """local, no collective: this rank copies its [lo, hi) slice of the per-parameter moments. A dict saved at any world
-        size, or by FusedAdamW / torch.optim.AdamW over the same parameters, loads at any other. On resume every rank also loads
-        the full weights and calls arena.refresh_shadow()."""
-        self._set_hyper(load_adamw_state_dict(self.arena, sd, self.m, self.v, self.lo))
 
     def gather_ema(self):
         """make every slice of the attached EMA current on this rank (in-place all-gather, like gather_masters)"""
@@ -666,6 +740,62 @@ class ShardedAdamW(_ArenaAdamW):
         else:
             dist.all_gather_into_tensor(flat, flat[self.lo:self.hi], group=self.group)
 
+    def _gather_updated(self):
+        """after this rank's update of [lo, hi): every rank's bf16 operands (or, without a shadow, masters) current"""
+        a = self.arena
+        self.all_gather_(a.shadow if a.shadow is not None else a.data)
+
+    def gather_masters(self):
+        """make the fp32 masters of ALL slices current on this rank (before save_pretrained / state_dict)"""
+        self.all_gather_(self.arena.data)
+
+
+class ShardedAdamW(_Shards, _ArenaAdamW):
+    """Data-parallel update with the optimizer state SHARDED over the ranks (ZeRO-1 on the flat arenas), all in NCCL
+    collectives that capture into the step's CUDA graph:
+
+        reduce-scatter(sum) of the fp32 gradient arena   -> this rank's 1/N slice of the summed gradient   (in place)
+        fused AdamW on that slice (grad_scale = 1/N)       -> fp32 masters + moments of the slice, bf16 shadow of the slice
+        all-gather of the bf16 shadow                       -> every rank has all updated operand weights   (in place)
+
+    versus all-reduce + replicated AdamW this moves 0.75x the bytes over NVLink (1/2 for the reduce-scatter + 1/4 for the bf16
+    all-gather) and does 1/N of the optimizer's 30 B/parameter of HBM traffic per rank. The fp32 masters of slices a rank does
+    not own go stale on it (only their bf16 operand copies are kept current): call `gather_masters()` before saving a
+    checkpoint or reading `p.data` of arbitrary parameters. Semantics of the update itself = torch.optim.AdamW on the MEAN
+    gradient, as DistributedDataParallel + AdamW would give (train_svd.py:767-773, :815-824)."""
+
+    _moment_buffers = ("m", "v")
+
+    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, group=None,
+                 max_grad_norm: Optional[float] = None):
+        super().__init__(arena, lr, betas, weight_decay, eps, max_grad_norm)
+        world = dist.get_world_size(group) if dist.is_initialized() else 1
+        self._shard(group, 64, f"ParamArena(..., pad_to={world * 64}) (equal, aligned shards)")
+        n = self.hi - self.lo
+        self.m = torch.zeros(n, device=arena.data.device, dtype=F32)
+        self.v = torch.zeros(n, device=arena.data.device, dtype=F32)
+
+    def state_dict(self) -> dict:
+        """COLLECTIVE: every rank calls it and gets the same full torch.optim.AdamW state dict (rank 0 saves it). m, then v, is
+        all-gathered into one temporary arena-length fp32 buffer and copied to the CPU before the next gather, so the peak
+        extra device memory is one arena (1.6 GB for the as-scripted temporal set, 6.1 GB for the whole UNet). Call
+        gather_masters() too before saving the weights."""
+        return adamw_state_dict(self.arena, self.t, self._hyper(), self._gathered_moments())
+
+    def _gathered_moments(self):
+        tmp = torch.empty_like(self.arena.data)
+        for mine in (self.m, self.v):
+            tmp[self.lo:self.hi].copy_(mine)
+            self.all_gather_(tmp)
+            yield tmp
+
+    @torch.no_grad()
+    def load_state_dict(self, sd: dict) -> None:
+        """local, no collective: this rank copies its [lo, hi) slice of the per-parameter moments. A dict saved at any world
+        size, or by FusedAdamW / torch.optim.AdamW over the same parameters, loads at any other. On resume every rank also loads
+        the full weights and calls arena.refresh_shadow()."""
+        self._set_hyper(load_adamw_state_dict(self.arena, sd, self.m, self.v, self.lo))
+
     def step(self):
         a = self.arena
         g = self.reduce_scatter_grads()
@@ -676,15 +806,8 @@ class ShardedAdamW(_ArenaAdamW):
             coef = self._clip_coef(1.0 / self.world)
         raw.adamw_graph(a.data[self.lo:self.hi], g, self.m, self.v, self.state, 1.0 / self.world,
                         shadow=None if a.shadow is None else a.shadow[self.lo:self.hi], **self._ema_args(self.lo, self.hi), grad_mul=coef)
-        if a.shadow is not None:
-            self.all_gather_(a.shadow)
-        else:
-            self.all_gather_(a.data)
+        self._gather_updated()
         self._updated()
-
-    def gather_masters(self):
-        """make the fp32 masters of ALL slices current on this rank (before save_pretrained / state_dict)"""
-        self.all_gather_(self.arena.data)
 
 
 def map_peer_buffers(t: torch.Tensor, group=None) -> List[int]:
@@ -725,7 +848,37 @@ def map_peer_buffers(t: torch.Tensor, group=None) -> List[int]:
 _IPC_OPEN: Dict[bytes, int] = {}      # allocation handle -> base address of its mapping in this process
 
 
-class P2PShardedAdamW(ShardedAdamW):
+class _PeerShards:
+    """What the NVLink peer-memory forms add to a _Shards optimizer: every rank's gradient and shadow arena mapped into this
+    process (map_peer_buffers), and a fence that orders the ranks around the one-kernel exchange"""
+
+    def _map_peers(self):
+        arena, who = self.arena, type(self).__name__
+        if arena.shadow is None:
+            raise ValueError(f"{who} needs the arena's bf16 shadow (CUDA arena)")
+        if self.world > 16:
+            raise ValueError(f"{who}: at most 16 ranks (one NVSwitch domain)")
+        self._flag = torch.zeros(1, device=arena.data.device, dtype=F32)
+        if self.world > 1:
+            self.peer_grad = map_peer_buffers(arena.grad, self.group)
+            self.peer_shadow = map_peer_buffers(arena.shadow, self.group)
+        else:
+            self.peer_grad, self.peer_shadow = [arena.grad.data_ptr()], [arena.shadow.data_ptr()]
+
+    def _fence(self):
+        dist.all_reduce(self._flag, group=self.group)      # stream-ordered on every rank, captured into the step graph
+
+    def _peer_clip_coef(self) -> Optional[torch.Tensor]:
+        """the clip coefficient of the mean gradient: a pre-pass over the same peer slices (the gradient crosses NVLink twice
+        when clipping), then the rank sum of the partials; None without clipping"""
+        if self._clip is None:
+            return None
+        raw.grad_sumsq_p2p(self.peer_grad, self.lo, self.hi - self.lo, self._sumsq)
+        all_reduce_sumsq(self._sumsq[:1], self.world, self.group)
+        return self._clip_coef(1.0 / self.world)
+
+
+class P2PShardedAdamW(_PeerShards, ShardedAdamW):
     """ShardedAdamW with the three NCCL phases (reduce-scatter, 1/N AdamW, all-gather of the bf16 operands) replaced by ONE
     kernel over NVLink peer memory (`svdx_adamw_p2p`): every rank reads its slice of every rank's gradient arena directly,
     updates its masters / moments and stores the bf16 operands into every rank's shadow arena. Same bytes over the links, no
@@ -735,33 +888,122 @@ class P2PShardedAdamW(ShardedAdamW):
     def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, group=None,
                  max_grad_norm: Optional[float] = None):
         super().__init__(arena, lr=lr, betas=betas, weight_decay=weight_decay, eps=eps, group=group, max_grad_norm=max_grad_norm)
-        if arena.shadow is None:
-            raise ValueError("P2PShardedAdamW needs the arena's bf16 shadow (CUDA arena)")
-        if self.world > 16:
-            raise ValueError("P2PShardedAdamW: at most 16 ranks (one NVSwitch domain)")
-        self._flag = torch.zeros(1, device=arena.data.device, dtype=F32)
-        if self.world > 1:
-            self.peer_grad = map_peer_buffers(arena.grad, group)
-            self.peer_shadow = map_peer_buffers(arena.shadow, group)
-        else:
-            self.peer_grad, self.peer_shadow = [arena.grad.data_ptr()], [arena.shadow.data_ptr()]
-
-    def _fence(self):
-        dist.all_reduce(self._flag, group=self.group)      # stream-ordered on every rank, captured into the step graph
+        self._map_peers()
 
     def step(self):
         a = self.arena
         if self.world > 1:
             self._fence()                                   # every rank's gradients are final
-        coef = None
-        if self._clip is not None:
-            # a pre-pass over the same peer slices (the gradient crosses NVLink twice when clipping), then the rank sum of the
-            # partials: the norm of the mean gradient the update below applies
-            raw.grad_sumsq_p2p(self.peer_grad, self.lo, self.hi - self.lo, self._sumsq)
-            all_reduce_sumsq(self._sumsq[:1], self.world, self.group)
-            coef = self._clip_coef(1.0 / self.world)
+        coef = self._peer_clip_coef()
         raw.adamw_p2p(a.data[self.lo:self.hi], self.m, self.v, self.peer_grad, self.peer_shadow, self.lo, self.state, 1.0 / self.world,
                       **self._ema_args(self.lo, self.hi), grad_mul=coef)
+        if self.world > 1:
+            self._fence()                                   # every shadow is complete, nobody still reads this rank's gradients
+        self._updated()
+
+
+class ShardedAdamW8bit(_Shards, _Arena8bit):
+    """FusedAdamW8bit with its state SHARDED over the ranks, ShardedAdamW's exchange in NCCL collectives that capture into the
+    step's CUDA graph:
+
+        reduce-scatter(sum) of the fp32 gradient arena   -> this rank's 1/N slice of the summed gradient   (in place)
+        svdx_adamw8bit over this rank's sub-jobs (grad_scale = 1/N)   -> masters, codes, absmax, fp32 states, bf16 shadow
+        all-gather of the bf16 shadow                       -> every rank has all updated operand weights   (in place)
+
+    Each rank keeps the 8-bit state of its own blocks only, about 2.03 bytes per parameter / N. The arena must be built with
+    ParamArena(..., pad_to=world * 256, block=256), so that every 256-element quantisation block lies in one shard; a
+    parameter that straddles a shard boundary is split into per-rank sub-jobs by block range. The update is FusedAdamW8bit's
+    on the mean gradient, bit for bit, and state dicts are FusedAdamW8bit's. As with ShardedAdamW, the masters of slices this
+    rank does not own go stale: call gather_masters() before saving the weights, and gather_ema() before using an attached EMA."""
+
+    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, min_8bit_size: int = 4096,
+                 group=None, max_grad_norm: Optional[float] = None):
+        super().__init__(arena, lr, betas, weight_decay, eps, max_grad_norm)
+        world = dist.get_world_size(group) if dist.is_initialized() else 1
+        hint = f"ParamArena(..., pad_to={world * 256}, block=256) (every quantisation block in one shard)"
+        self._shard(group, 256, hint)
+        if arena.block % 256:
+            raise ValueError(f"{type(self).__name__}: build the arena with {hint}")
+        self._init_8bit(min_8bit_size, self.lo, self.hi)
+
+    def step(self):
+        g = self.reduce_scatter_grads()
+        coef = None
+        if self._clip is not None:
+            raw.grad_sumsq(g, self._sumsq)
+            all_reduce_sumsq(self._sumsq[:1], self.world, self.group)
+            coef = self._clip_coef(1.0 / self.world)
+        self._launch(1.0 / self.world, coef)
+        self._gather_updated()
+        self._updated()
+
+    def state_dict(self) -> dict:
+        """COLLECTIVE: every rank calls it and gets the same dict FusedAdamW8bit.state_dict() gives (bitsandbytes' per-parameter
+        keys, uint8 codes, absmax, step; on the device). The six state buffers are gathered one at a time into a temporary of
+        the unsharded size and sliced into the dict's tensors before the next, so the peak extra device memory is the returned
+        state (about 2.03 bytes per parameter, as FusedAdamW8bit's dict) plus two temporaries of the largest buffer (the codes,
+        1 byte per parameter, padded to an equal part per rank): about 4.1 bytes per parameter, 1.6 GB for the as-scripted
+        temporal set (397.6 M parameters)."""
+        return self._state_dict_of(self._gathered_buffers(), self.t)
+
+    def _gathered_buffers(self):
+        """(name, unsharded buffer) for the six state buffers, each all-gathered from every rank's owned range"""
+        per_rank = [self._subjobs(r * (self.arena.numel // self.world), (r + 1) * (self.arena.numel // self.world))[1]
+                    for r in range(self.world)]
+        for name in self._moment_buffers:
+            k = {"codes1": 0, "codes2": 0, "absmax1": 1, "absmax2": 1, "m32": 2, "v32": 2}[name]
+            mine = getattr(self, name)
+            spans = [rng[k] for rng in per_rank]
+            full = torch.zeros(max(y for _, y in spans), dtype=mine.dtype, device=mine.device)
+            if self.world == 1:
+                full.copy_(mine)
+            else:
+                width = max(y - x for x, y in spans)
+                src = torch.zeros(width, dtype=mine.dtype, device=mine.device)
+                src[:mine.numel()].copy_(mine)
+                if dist.get_backend(self.group) == "gloo":
+                    parts = [torch.empty_like(src) for _ in range(self.world)]
+                    dist.all_gather(parts, src, group=self.group)
+                else:
+                    tmp = torch.empty(width * self.world, dtype=mine.dtype, device=mine.device)
+                    dist.all_gather_into_tensor(tmp, src, group=self.group)
+                    parts = tmp.view(self.world, width)
+                for (x, y), part in zip(spans, parts):
+                    full[x:y].copy_(part[:y - x])
+                del parts, src
+            yield name, full
+            del full
+
+
+class P2PShardedAdamW8bit(_PeerShards, ShardedAdamW8bit):
+    """ShardedAdamW8bit with its three NCCL phases replaced by ONE kernel over NVLink peer memory (`svdx_adamw8bit_p2p`), with
+    P2PShardedAdamW's peer mappings and fences: each rank sums its blocks of every rank's gradient arena in rank order, applies
+    FusedAdamW8bit's update to its own state and stores the bf16 operands into every rank's shadow arena. Results are those of
+    FusedAdamW8bit.step(grad_scale=1/N) on the rank-order sum of the gradients, bit for bit."""
+
+    def __init__(self, arena: ParamArena, lr=1e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, min_8bit_size: int = 4096,
+                 group=None, max_grad_norm: Optional[float] = None):
+        super().__init__(arena, lr=lr, betas=betas, weight_decay=weight_decay, eps=eps, min_8bit_size=min_8bit_size, group=group,
+                         max_grad_norm=max_grad_norm)
+        self._map_peers()
+
+    def p2p_job_rows(self):
+        """the svdx_adamw8bit_p2p job table of this rank's sub-jobs as an int64 array [jobs, 9] (svd_xtend_b200.h)"""
+        import numpy as np
+        from .optim8bit import p2p_job_row
+        pb = self.arena.data.data_ptr()
+        eb = self.ema._flat.data_ptr() if self.ema is not None else 0
+        rows = [p2p_job_row(pb + 4 * off, *self._state_ptrs(quant, si, bi), eb + 4 * off if eb else 0, off, n, quant)
+                for p, off, n, quant, si, bi in self.subjobs]
+        return np.array(rows, dtype=np.int64).reshape(-1, 9)
+
+    def step(self):
+        if self.world > 1:
+            self._fence()                                   # every rank's gradients are final
+        coef = self._peer_clip_coef()
+        tb = self._job_table(self.p2p_job_rows, 7, self.world)
+        raw.adamw8bit_p2p(tb.dev, tb.prefix, tb.njobs, tb.blocks, self.qmap1, self.qmap2, self.peer_grad, self.peer_shadow, self.state,
+                          1.0 / self.world, ema_state=None if self.ema is None else self.ema._state, nbytes=self._nbytes, grad_mul=coef)
         if self.world > 1:
             self._fence()                                   # every shadow is complete, nobody still reads this rank's gradients
         self._updated()
