@@ -10,6 +10,7 @@
 #include "common.cuh"
 #include "../../include/svd_xtend_b200.h"
 #include "host_util.h"
+#include <stdio.h>
 #include <stdlib.h>
 
 namespace svdx {
@@ -969,6 +970,23 @@ static int gn_check(int C1, int C2, int64_t ldx, int64_t ldx2, const void* x, co
   return 0;
 }
 
+// a row stride shorter than the row overlaps the next row; one row has no stride to check (torch gives a size-1 dim any stride)
+static bool short_ld(long long ld, long long width, long long nrows) { return nrows > 1 && ld < width; }
+
+// the row strides of the one or two sources (the kernels address row r of slab n at (n * rows + r) * ld): the violated
+// constraint, or nullptr
+static const char* gn_ld_error(int C1, int C2, int64_t ldx, int64_t ldx2, long long nrows) {
+  if (short_ld(ldx, C1, nrows)) return "ldx < C1";
+  if (C2 > 0 && short_ld(ldx2, C2, nrows)) return "ldx2 < C2";
+  return nullptr;
+}
+
+static int norm_fail(const char* entry, const char* what) {
+  char msg[96];
+  snprintf(msg, sizeof(msg), "%s: %s", entry, what);
+  return svdx_fail(SVDX_E_BADARG, msg);
+}
+
 // at most 32 groups (the consumers' shared-memory group tables) of an even number of channels
 static int gn_groups_bad(int C, int G) { return G <= 0 || G > 32 || C % G || (C / G) % 2; }
 
@@ -977,6 +995,7 @@ extern "C" int svdx_groupnorm_sums(const void* x, int64_t ldx, int32_t C1, const
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
   if (gn_check(C1, C2, ldx, ldx2, x, x2) || outer <= 0 || rows <= 0 || !sums || (reinterpret_cast<uintptr_t>(sums) & 15) || ld < C1 + C2 || ld % 4)
     return svdx_fail(SVDX_E_BADARG, "groupnorm_sums: bad arguments");
+  if (const char* e = gn_ld_error(C1, C2, ldx, ldx2, (long long)outer * rows)) return norm_fail("groupnorm_sums", e);
   GnSrc s{reinterpret_cast<const bf16*>(x), ldx, C1, reinterpret_cast<const bf16*>(x2), ldx2, C2};
   int threads, rpc;
   gn_vec_config(C1 + C2, outer, rows, threads, rpc);
@@ -995,6 +1014,9 @@ extern "C" int svdx_groupnorm_apply_fused(const void* x, int64_t ldx, int32_t C1
       !rstd || !gamma || !beta || (reinterpret_cast<uintptr_t>(gamma) & 15) || (reinterpret_cast<uintptr_t>(beta) & 15) ||
       (ab_out && ((reinterpret_cast<uintptr_t>(ab_out) & 15))) || !csum1 || ldc1 < C1 || (C2 > 0 && (!csum2 || ldc2 < C2)) || outer <= 0 || rows <= 0)
     return svdx_fail(SVDX_E_BADARG, "groupnorm_apply_fused: bad arguments");
+  const long long M = (long long)outer * rows;
+  if (const char* e = gn_ld_error(C1, C2, ldx, ldx2, M)) return norm_fail("groupnorm_apply_fused", e);
+  if (short_ld(ldy, C1 + C2, M)) return norm_fail("groupnorm_apply_fused", "ldy < C1 + C2");
   GnSrc s{reinterpret_cast<const bf16*>(x), ldx, C1, reinterpret_cast<const bf16*>(x2), ldx2, C2};
   static bool attr[SVDX_MAX_DEVICES] = {false};
   gn_ring_attr(gn_apply_ring, attr);
@@ -1013,6 +1035,9 @@ extern "C" int svdx_groupnorm_bwd_sums(const void* x, int64_t ldx, int32_t C1, c
   if (gn_check(C1, C2, ldx, ldx2, x, x2) || !dy || lddy % 8 || (reinterpret_cast<uintptr_t>(dy) & 15) || (fuse_silu && !ab) || !sums ||
       (reinterpret_cast<uintptr_t>(sums) & 15) || outer <= 0 || rows <= 0)
     return svdx_fail(SVDX_E_BADARG, "groupnorm_bwd_sums: bad arguments");
+  const long long M = (long long)outer * rows;
+  if (const char* e = gn_ld_error(C1, C2, ldx, ldx2, M)) return norm_fail("groupnorm_bwd_sums", e);
+  if (short_ld(lddy, C1 + C2, M)) return norm_fail("groupnorm_bwd_sums", "lddy < C");
   GnSrc s{reinterpret_cast<const bf16*>(x), ldx, C1, reinterpret_cast<const bf16*>(x2), ldx2, C2};
   static bool attr[SVDX_MAX_DEVICES] = {false};
   gn_ring_attr(gn_bwd_sums_ring, attr);
@@ -1035,6 +1060,12 @@ extern "C" int svdx_groupnorm_bwd_fused(const void* x, int64_t ldx, int32_t C1, 
       (reinterpret_cast<uintptr_t>(dx) & 15) || (C2 > 0 && (!dx2 || lddx2 % 8 || (reinterpret_cast<uintptr_t>(dx2) & 15))) || !csum || !mean || !rstd ||
       !gamma || !beta || (dgamma && !dbeta) || (dres && (C2 > 0 || lddres % 8 || (reinterpret_cast<uintptr_t>(dres) & 15))) || outer <= 0 || rows <= 0)
     return svdx_fail(SVDX_E_BADARG, "groupnorm_bwd_fused: bad arguments");
+  const long long M = (long long)outer * rows;
+  if (const char* e = gn_ld_error(C1, C2, ldx, ldx2, M)) return norm_fail("groupnorm_bwd_fused", e);
+  if (short_ld(lddy, C1 + C2, M)) return norm_fail("groupnorm_bwd_fused", "lddy < C");
+  if (short_ld(lddx, C1, M)) return norm_fail("groupnorm_bwd_fused", "lddx < C1");
+  if (C2 > 0 && short_ld(lddx2, C2, M)) return norm_fail("groupnorm_bwd_fused", "lddx2 < C2");
+  if (dres && short_ld(lddres, C1 + C2, M)) return norm_fail("groupnorm_bwd_fused", "lddres < C");
   GnSrc s{reinterpret_cast<const bf16*>(x), ldx, C1, reinterpret_cast<const bf16*>(x2), ldx2, C2};
   static bool a1[SVDX_MAX_DEVICES] = {false}, a2[SVDX_MAX_DEVICES] = {false};
   gn_ring_attr(gn_bwd_fused_ring<true>, a1);
@@ -1123,6 +1154,9 @@ extern "C" int svdx_layernorm_fwd(const void* x, int64_t ldx, int32_t rows, int3
       (reinterpret_cast<uintptr_t>(beta) & 15) ||
       (addvec && (!xsum || add_div <= 0 || ldxs % 8 || (reinterpret_cast<uintptr_t>(addvec) & 15) || (reinterpret_cast<uintptr_t>(xsum) & 15))))
     return svdx_fail(SVDX_E_BADARG, "layernorm_fwd: bad arguments (C %% 8, C <= 2560, 16-byte aligned rows and vectors)");
+  if (short_ld(ldx, C, rows)) return norm_fail("layernorm_fwd", "ldx < C");
+  if (short_ld(ldy, C, rows)) return norm_fail("layernorm_fwd", "ldy < C");
+  if (addvec && short_ld(ldxs, C, rows)) return norm_fail("layernorm_fwd", "ldxs < C");
   const int nj = (C / 8 + 31) / 32;
   if (nj <= 5) {
     if (nj <= 1) ln_fwd_ring_launch<1>(x, ldx, rows, C, gamma, beta, eps, y, ldy, mean, rstd, addvec, add_div, xsum, ldxs, st);
@@ -1165,6 +1199,10 @@ extern "C" int svdx_layernorm_bwd(const void* x, int64_t ldx, const void* dy, in
   if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(dy) & 15) || (reinterpret_cast<uintptr_t>(dx) & 15) ||
       (dres && (reinterpret_cast<uintptr_t>(dres) & 15)))
     return svdx_fail(SVDX_E_BADARG, "layernorm_bwd: x / dy / dx / dres must be 16-byte aligned");
+  if (short_ld(ldx, C, rows)) return norm_fail("layernorm_bwd", "ldx < C");
+  if (short_ld(lddy, C, rows)) return norm_fail("layernorm_bwd", "lddy < C");
+  if (short_ld(lddx, C, rows)) return norm_fail("layernorm_bwd", "lddx < C");
+  if (dres && short_ld(lddres, C, rows)) return norm_fail("layernorm_bwd", "lddres < C");
   if (nj <= 5) {
     if (nj <= 1) ln_bwd_ring_launch<1>(x, ldx, dy, lddy, rows, C, gamma, mean, rstd, dx, lddx, dres, lddres, dgamma, dbeta, st);
     else if (nj <= 2) ln_bwd_ring_launch<2>(x, ldx, dy, lddy, rows, C, gamma, mean, rstd, dx, lddx, dres, lddres, dgamma, dbeta, st);

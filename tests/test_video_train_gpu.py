@@ -226,7 +226,7 @@ def test_graphed_step_matches_eager(optim):
 @pytest.mark.gpu
 def test_svd_config_graphed_step_matches_hand_composition():
     """14 x 320 x 512, B = 1, the as-scripted trainable set, FusedAdamW: the graphed step against the package's stages composed by
-    hand (eager assemble_train_batch + UNet + edm_loss + backward) on the same draws, within the spread of two eager runs"""
+    hand (eager assemble_train_batch + UNet + edm_loss + backward) on the same draws, within the spread of repeated eager runs"""
     from oracle.svd_clip_oracle import CLIP_CONFIG
     from svd_xtend_b200.video_train import assemble_train_batch
     from svd_xtend_b200.workload import SVD_CONFIG, edm_loss
@@ -244,18 +244,22 @@ def test_svd_config_graphed_step_matches_hand_composition():
     arena.data.copy_(w0)
     arena.refresh_shadow()
     u.refresh_trainable_operands(shadow_current=True)
+    # The GroupNorm channel sums are added across CTAs by atomics in a varying order, so the loss moves by ~3e-5 relative from
+    # run to run. One pair of eager runs is too small a sample of that spread: a graphed loss within the noise fell outside 4x one
+    # pair's difference about one time in ten. The loss spread is the largest difference over four eager reruns.
     hand = []
-    for _ in range(2):
+    for i in range(5):
         arena.zero_grad()
         b = assemble_train_batch(step.vae, step.image_encoder, u, x, seen[0], conditioning_dropout_prob=0.1)
         pred = u(b["sample"], b["timestep"], b["encoder_hidden_states"], added_time_ids=b["added_time_ids"]).sample
         lh = edm_loss(pred.float(), b["noisy"], b["latents"], b["sigmas"])
         lh.backward()
         torch.cuda.synchronize()
-        hand.append((lh.item(), arena.grad.clone()))
+        hand.append((lh.item(), arena.grad.clone() if i < 2 else None))
     spread = _rel(hand[1][1], hand[0][1])
     e = _rel(g_graph, hand[0][1])
-    print(f"SVD config: loss graphed {loss:.5f} hand {hand[0][0]:.5f} / {hand[1][0]:.5f}; grad rel-l2 {e:.3e} (eager spread {spread:.3e}); "
-          f"max memory {torch.cuda.max_memory_allocated() / 2**30:.1f} GiB")
+    spread_l = max(abs(h - hand[0][0]) for h, _ in hand[1:])
+    print(f"SVD config: loss graphed {loss:.5f} hand {' / '.join(f'{h:.5f}' for h, _ in hand)}; grad rel-l2 {e:.3e} (eager spread "
+          f"{spread:.3e}); max memory {torch.cuda.max_memory_allocated() / 2**30:.1f} GiB")
     assert e <= 4 * spread + 1e-6
-    assert abs(loss - hand[0][0]) <= 4 * abs(hand[1][0] - hand[0][0]) + 1e-5 * abs(hand[0][0])
+    assert abs(loss - hand[0][0]) <= 4 * spread_l + 1e-5 * abs(hand[0][0])
