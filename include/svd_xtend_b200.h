@@ -247,7 +247,12 @@ int svdx_layernorm_bwd(const void* x, int64_t ldx, const void* dy, int64_t lddy,
  * with seq_base(s) = (s / inner) * outer_stride + (s % inner) * inner_stride:
  *   spatial  (per frame over H*W):  inner = 1,  outer_stride = HW, tok_stride = 1
  *   temporal (per pixel over T):    inner = HW, outer_stride = T*HW, inner_stride = 1, tok_stride = HW
- * lse [nseq][heads][S] fp32 (natural-log sum-exp of the scaled scores) is saved for backward. */
+ * Rows that belong to no sequence are neither read nor written. Strided sequences (inner > 1) need S <= 128.
+ * lse fp32 (natural-log sum-exp of the scaled scores, saved for backward) and the backward's delta workspace are
+ * [token row][heads]: the value of token row r and head h is at [r * heads + h], so both must hold
+ * (largest token row + 1) * heads floats. Only the entries of token rows are written.
+ * Every ld is a multiple of 8 and at least heads*64; q / k / v / dout are 16-byte aligned, o / dq / dk / dv 4-byte
+ * aligned (16-byte aligned when inner > 1 and S <= 32). */
 typedef struct SvdxAttn {
   const void* q; const void* k; const void* v; void* o;
   int64_t ldq, ldk, ldv, ldo;
@@ -259,7 +264,7 @@ typedef struct SvdxAttn {
   /* backward only */
   const void* dout; int64_t lddo;
   void* dq; void* dk; void* dv; int64_t lddq, lddk, lddv;
-  float* delta;     /* workspace [nseq][heads][S] */
+  float* delta;     /* workspace [token row][heads], sized as lse */
 } SvdxAttn;
 int svdx_attention_fwd(const SvdxAttn* d, void* stream);
 int svdx_attention_bwd(const SvdxAttn* d, void* stream);

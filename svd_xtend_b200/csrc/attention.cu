@@ -416,18 +416,24 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_bwd_dkv_kernel(const __gri
                   ki[1].valid ? p.dk + ki[1].token * p.lddk + head * 64 : nullptr, dk, 1.f, 1.f, lane);
 }
 
-// delta[token][head] = sum_d dO * O   — one warp per (token, head)
-__global__ void attn_delta_kernel(const bf16* __restrict__ o, long long ldo, const bf16* __restrict__ dout, long long lddo, long long tokens,
-                                  int heads, float* __restrict__ delta) {
+// delta[token row][head] = sum_d dO * O   — one warp per (sequence, token, head); the token row follows the descriptor's
+// geometry as row_info does, so only the rows the backward kernels read are written
+__global__ void attn_delta_kernel(const bf16* __restrict__ o, long long ldo, const bf16* __restrict__ dout, long long lddo,
+                                  long long nseq, int S, int inner, long long outer_stride, long long inner_stride,
+                                  long long tok_stride, int heads, float* __restrict__ delta) {
   const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
-  if (w >= tokens * heads) return;
-  const long long tok = w / heads;
-  const int h = (int)(w - tok * heads);
+  if (w >= nseq * S * heads) return;
+  const long long st = w / heads;                    // sequence * S + token
+  const int h = (int)(w - st * heads);
+  const long long seq = st / S;
+  const long long t = st - seq * S;
+  const long long outer = seq / inner;
+  const long long tok = outer * outer_stride + (seq - outer * inner) * inner_stride + t * tok_stride;
   const float2 a = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(o + tok * ldo + h * 64 + 2 * lane));
   const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(dout + tok * lddo + h * 64 + 2 * lane));
   const float s = warp_sum(a.x * b.x + a.y * b.y);
-  if (lane == 0) delta[w] = s;
+  if (lane == 0) delta[tok * heads + h] = s;
 }
 
 }  // namespace svdx
@@ -447,6 +453,21 @@ static int attn_setup(const SvdxAttn* d, AttnKParams& p, bool bwd, dim3& grid) {
   if (!d || !d->q || !d->k || !d->v) return svdx_fail(SVDX_E_BADARG, "attention: null pointer");
   if (d->heads <= 0 || d->S <= 0 || d->nseq <= 0 || d->inner <= 0 || d->nseq % d->inner) return svdx_fail(SVDX_E_BADARG, "attention: bad sequence geometry");
   if ((d->ldq % 8) || (d->ldk % 8) || (d->ldv % 8)) return svdx_fail(SVDX_E_BADARG, "attention: leading dims must be multiples of 8");
+  const int64_t cols = (int64_t)d->heads * 64;
+  if (d->ldq < cols || d->ldk < cols || d->ldv < cols) return svdx_fail(SVDX_E_BADARG, "attention: ldq / ldk / ldv < heads * 64");
+  if (bwd) {
+    if (!d->dout || !d->dq || !d->dk || !d->dv || !d->lse || !d->delta || !d->o) return svdx_fail(SVDX_E_BADARG, "attention_bwd: null pointer");
+    if ((d->lddo % 8) || (d->lddq % 8) || (d->lddk % 8) || (d->lddv % 8) || (d->ldo % 8)) return svdx_fail(SVDX_E_BADARG, "attention_bwd: leading dims");
+    if (d->lddo < cols || d->lddq < cols || d->lddk < cols || d->lddv < cols || d->ldo < cols)
+      return svdx_fail(SVDX_E_BADARG, "attention_bwd: ldo / lddo / lddq / lddk / lddv < heads * 64");
+  } else {
+    if (!d->o || (d->ldo % 8)) return svdx_fail(SVDX_E_BADARG, "attention_fwd: output");
+    if (d->ldo < cols) return svdx_fail(SVDX_E_BADARG, "attention_fwd: ldo < heads * 64");
+  }
+  // o / dq / dk / dv are written as 4-byte column pairs (store_frag_rows), and o is read so by the delta kernel
+  const uintptr_t out_al = reinterpret_cast<uintptr_t>(d->o) | (bwd ? reinterpret_cast<uintptr_t>(d->dq) | reinterpret_cast<uintptr_t>(d->dk) |
+                                                                        reinterpret_cast<uintptr_t>(d->dv) : 0);
+  if (out_al & 3) return svdx_fail(SVDX_E_BADARG, "attention: o / dq / dk / dv must be 4 B aligned");
   memset(&p, 0, sizeof(p));
   int G = 1;
   if (d->inner > 1) {
@@ -463,26 +484,20 @@ static int attn_setup(const SvdxAttn* d, AttnKParams& p, bool bwd, dim3& grid) {
   p.tiles = (d->S + RT - 1) / RT;
   p.outer_stride = d->outer_stride; p.inner_stride = d->inner_stride; p.tok_stride = d->tok_stride;
   p.scale = d->scale;
-  const int cols = d->heads * 64;
-  int rc;
-  if ((rc = attn_make_map(&p.tq, d->q, d->ldq, cols, d, G, RT))) return rc;
-  if ((rc = attn_make_map(&p.tk, d->k, d->ldk, cols, d, G, RT))) return rc;
-  if ((rc = attn_make_map(&p.tv, d->v, d->ldv, cols, d, G, RT))) return rc;
-  if (bwd) {
-    if (!d->dout || !d->dq || !d->dk || !d->dv || !d->lse || !d->delta || !d->o) return svdx_fail(SVDX_E_BADARG, "attention_bwd: null pointer");
-    if ((d->lddo % 8) || (d->lddq % 8) || (d->lddk % 8) || (d->lddv % 8) || (d->ldo % 8)) return svdx_fail(SVDX_E_BADARG, "attention_bwd: leading dims");
-    if ((rc = attn_make_map(&p.tdo, d->dout, d->lddo, cols, d, G, RT))) return rc;
-  } else {
-    if (!d->o || (d->ldo % 8)) return svdx_fail(SVDX_E_BADARG, "attention_fwd: output");
-  }
+  const long long gz = (long long)(d->nseq / d->inner) * p.inner_groups;
+  if (gz > 65535 || d->heads > 65535) return svdx_fail(SVDX_E_BADARG, "attention: grid too large");
+  grid = dim3(p.tiles, d->heads, (unsigned)gz);
   p.o = reinterpret_cast<bf16*>(d->o); p.ldo = d->ldo;
   p.lse = d->lse; p.delta = d->delta;
   p.dq = reinterpret_cast<bf16*>(d->dq); p.lddq = d->lddq;
   p.dk = reinterpret_cast<bf16*>(d->dk); p.lddk = d->lddk;
   p.dv = reinterpret_cast<bf16*>(d->dv); p.lddv = d->lddv;
-  const long long gz = (long long)(d->nseq / d->inner) * p.inner_groups;
-  if (gz > 65535 || d->heads > 65535) return svdx_fail(SVDX_E_BADARG, "attention: grid too large");
-  grid = dim3(p.tiles, d->heads, (unsigned)gz);
+  // every argument check is above: the tensor maps need the driver
+  int rc;
+  if ((rc = attn_make_map(&p.tq, d->q, d->ldq, (int)cols, d, G, RT))) return rc;
+  if ((rc = attn_make_map(&p.tk, d->k, d->ldk, (int)cols, d, G, RT))) return rc;
+  if ((rc = attn_make_map(&p.tv, d->v, d->ldv, (int)cols, d, G, RT))) return rc;
+  if (bwd && (rc = attn_make_map(&p.tdo, d->dout, d->lddo, (int)cols, d, G, RT))) return rc;
   return 0;
 }
 
@@ -525,11 +540,10 @@ extern "C" int svdx_attention_bwd(const SvdxAttn* d, void* stream_v) {
     if (e != cudaSuccess) return svdx_fail_cuda(e, "attention_bwd: smem attribute");
     attr[slot] = true;
   }
-  // tokens covered = nseq * S (dense token-major matrices)
-  const long long tokens = (long long)d->nseq * d->S;
-  const long long warps = tokens * d->heads;
-  attn_delta_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>(reinterpret_cast<const bf16*>(d->o), d->ldo,
-                                                                         reinterpret_cast<const bf16*>(d->dout), d->lddo, tokens, d->heads, d->delta);
+  const long long warps = (long long)d->nseq * d->S * d->heads;
+  attn_delta_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>(
+      reinterpret_cast<const bf16*>(d->o), d->ldo, reinterpret_cast<const bf16*>(d->dout), d->lddo, d->nseq, d->S, d->inner,
+      d->outer_stride, d->inner_stride, d->tok_stride, d->heads, d->delta);
   attn_bwd_dq_kernel<<<grid, AT_THREADS, BDQ_SMEM, st>>>(p);
   attn_bwd_dkv_kernel<<<grid, AT_THREADS, BKV_SMEM, st>>>(p);
   SVDX_CHECK_LAUNCH("attention_bwd");

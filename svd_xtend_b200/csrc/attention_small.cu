@@ -364,6 +364,9 @@ static int small_fill(const SvdxAttn* d, SmallAttnP& p, bool bwd) {
   if (!d->q || !d->k || !d->v || !d->o) return svdx_fail(SVDX_E_BADARG, "attention(small): null pointer");
   if (d->heads <= 0 || d->nseq <= 0 || d->inner <= 0 || d->nseq % d->inner) return svdx_fail(SVDX_E_BADARG, "attention(small): bad sequence geometry");
   if ((d->ldq % 8) || (d->ldk % 8) || (d->ldv % 8) || (d->ldo % 8)) return svdx_fail(SVDX_E_BADARG, "attention(small): leading dims must be multiples of 8");
+  const int64_t cols = (int64_t)d->heads * 64;
+  if (d->ldq < cols || d->ldk < cols || d->ldv < cols || d->ldo < cols)
+    return svdx_fail(SVDX_E_BADARG, "attention(small): ldq / ldk / ldv / ldo < heads * 64");
   const uintptr_t al = reinterpret_cast<uintptr_t>(d->q) | reinterpret_cast<uintptr_t>(d->k) | reinterpret_cast<uintptr_t>(d->v) | reinterpret_cast<uintptr_t>(d->o);
   if (al & 15) return svdx_fail(SVDX_E_BADARG, "attention(small): operands must be 16 B aligned");
   memset(&p, 0, sizeof(p));
@@ -376,6 +379,8 @@ static int small_fill(const SvdxAttn* d, SmallAttnP& p, bool bwd) {
   if (bwd) {
     if (!d->dout || !d->dq || !d->dk || !d->dv) return svdx_fail(SVDX_E_BADARG, "attention_bwd(small): null pointer");
     if ((d->lddo % 8) || (d->lddq % 8) || (d->lddk % 8) || (d->lddv % 8)) return svdx_fail(SVDX_E_BADARG, "attention_bwd(small): leading dims");
+    if (d->lddo < cols || d->lddq < cols || d->lddk < cols || d->lddv < cols)
+      return svdx_fail(SVDX_E_BADARG, "attention_bwd(small): lddo / lddq / lddk / lddv < heads * 64");
     const uintptr_t a2 = reinterpret_cast<uintptr_t>(d->dout) | reinterpret_cast<uintptr_t>(d->dq) | reinterpret_cast<uintptr_t>(d->dk) | reinterpret_cast<uintptr_t>(d->dv);
     if (a2 & 15) return svdx_fail(SVDX_E_BADARG, "attention_bwd(small): operands must be 16 B aligned");
     p.dout = reinterpret_cast<const bf16*>(d->dout); p.lddo = d->lddo;

@@ -313,7 +313,7 @@ extern "C" int svdx_attention_hd80_fwd(const void* q, int64_t ldq, const void* k
   if (!q || !k || !v || !o || nseq <= 0 || heads <= 0 || S <= 0 || nseq > 65535 || heads > 65535)
     return svdx_fail(SVDX_E_BADARG, "attention_hd80_fwd: null pointer or bad geometry");
   if ((ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 2) || ldq < heads * 80 || ldk < heads * 80 || ldv < heads * 80 || ldo < heads * 80)
-    return svdx_fail(SVDX_E_BADARG, "attention_hd80_fwd: q/k/v rows need ld %% 8 == 0 and ld >= heads * 80, o rows ld even");
+    return svdx_fail(SVDX_E_BADARG, "attention_hd80_fwd: q/k/v rows need ld % 8 == 0 and ld >= heads * 80, o rows ld even");
   const uintptr_t al = reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v);
   if ((al & 15) || (reinterpret_cast<uintptr_t>(o) & 3)) return svdx_fail(SVDX_E_BADARG, "attention_hd80_fwd: q/k/v 16 B and o 4 B aligned");
   Attn80P p;
