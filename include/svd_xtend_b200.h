@@ -174,7 +174,7 @@ int svdx_splitk_epilogue(float* ws, int64_t ldw, void* out, int64_t ldo, int64_t
 
 /* number of SMs the persistent kernels size their grids to (queried once) */
 int svdx_num_sms(void);
-/* enable peer access from the current device to peer_device (needed before svdx_adamw_p2p dereferences arenas that live on,
+/* enable peer access from the current device to peer_device (needed before svdx_adamw_step_p2p dereferences arenas that live on,
  * or were IPC-mapped from, that GPU); idempotent; fails when the GPUs have no P2P path */
 int svdx_enable_peer_access(int32_t peer_device);
 /* CUDA IPC of a device buffer between the processes of one node (one process per GPU). export: the 64-byte handle of the
@@ -371,19 +371,30 @@ int svdx_blend_scales(const float* mix_factor, float* out16, void* stream);
  * step-varying scalar is in DEVICE memory, so that the update can be captured in a CUDA graph and replayed:
  * state = float[8] {lr, beta1, beta2, eps, weight_decay, step, 1-beta1^step, 1-beta2^step}. The call first advances
  * step and the bias corrections on the device (a 1-thread kernel), then updates; the host changes the learning rate by
- * writing state[0] (lr scheduler of train_svd.py:790-796). Two launches. */
-int svdx_adamw_graph(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
-                     void* shadow_bf16, void* stream);
+ * writing state[0] (lr scheduler of train_svd.py:790-796). Two launches. Optional arguments, NULL for none:
+ *   ema, ema_state: the update also advances the fp32 EMA buffer ema[0 .. n) (16-byte aligned) at the same flat offsets from
+ *     the freshly updated masters, and the tick also advances ema_state (the EMA state below, 8-byte aligned). Pass both or
+ *     neither: one without the other is SVDX_E_BADARG.
+ *   grad_mul: a DEVICE float (4-byte aligned) the gradient is also scaled by, read by the update kernel, so the applied gradient
+ *     is g * (grad_scale * grad_mul[0]); at grad_scale = 1 that is g * grad_mul[0], the product torch's in-place g.mul_(coef)
+ *     gives. Gradient clipping passes out + 1 of svdx_clip_coef, so the clip is decided on the device and a captured step
+ *     needs no host sync.
+ * With all three NULL the update is plain AdamW. */
+int svdx_adamw_step(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale, void* shadow_bf16,
+                    float* ema, double* ema_state, const float* grad_mul, void* stream);
 /* Data-parallel optimizer step over NVLink peer memory (one process per GPU, every rank's gradient and bf16 operand arenas
  * mapped into every process with CUDA IPC): reduce-scatter + AdamW + all-gather as ONE kernel. This rank owns [lo, lo + n):
  * it loads that slice of grads[r] (r = 0 .. world-1, the FULL arenas, peer-mapped), sums in rank order, applies AdamW with
  * grad_scale (= 1 / world) to its local p / m / v slices (length n) and stores the bf16 value to shadows[r][lo + i] of every
  * rank. The caller provides the cross-rank ordering: all gradients final before the launch, no rank reads its shadow or
  * clears its gradients until every rank's launch has completed. tick != 0 also advances the device step count / bias
- * corrections in state[5..7] (svdx_adamw_graph's state layout). Replaces DistributedDataParallel's all-reduce +
- * torch.optim.AdamW of train_svd.py:767-773,815-824,1044-1049 at N > 1. */
-int svdx_adamw_p2p(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world,
-                   int64_t lo, int64_t n, float* state, float grad_scale, int32_t tick, void* stream);
+ * corrections in state[5..7] (svdx_adamw_step's state layout), and ema_state with an EMA. grads[r]: 16-byte aligned,
+ * shadows[r]: 8-byte aligned. ema (this rank's slice: length n, 16-byte aligned, no peer traffic), ema_state and grad_mul as in
+ * svdx_adamw_step. Two launches with tick, one without. Replaces DistributedDataParallel's all-reduce + torch.optim.AdamW of
+ * train_svd.py:767-773,815-824,1044-1049 at N > 1. */
+int svdx_adamw_step_p2p(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo,
+                        int64_t n, float* state, float grad_scale, int32_t tick, float* ema, double* ema_state,
+                        const float* grad_mul, void* stream);
 
 /* Global gradient norm for clipping (torch.nn.utils.clip_grad_norm_ with norm type 2: train_svd.py's --max_grad_norm,
  * :468-470, :1044-1049), computed and applied on the device so that a captured step clips without a host sync.
@@ -391,9 +402,9 @@ int svdx_adamw_p2p(float* p, float* m, float* v, const void* const* grads, void*
  * svdx_grad_sumsq: sumsq[0] = sum over i < n of (double)g[i]^2 (g 16-byte aligned: the gradient arena or a slice of it). The
  * partition over blocks depends on n only, the partials are fp64 and a second one-block kernel sums them in index order:
  * identical bits for the same input, launch after launch and replay after replay. Two launches, no host access.
- * svdx_grad_sumsq_p2p: the same over the slice [lo, lo + n) of the rank-order sum of grads[0 .. world) (svdx_adamw_p2p's
+ * svdx_grad_sumsq_p2p: the same over the slice [lo, lo + n) of the rank-order sum of grads[0 .. world) (svdx_adamw_step_p2p's
  * peer-mapped arenas, summed exactly as that kernel sums them, up to four ranks' loads in flight), so the norm is that of the
- * gradient svdx_adamw_p2p applies. lo and n multiples of 4. Two launches.
+ * gradient svdx_adamw_step_p2p applies. lo and n multiples of 4. Two launches.
  * svdx_clip_coef: one thread. From sumsq[0], a DEVICE max_norm and the host scale (1 / world under the sharded optimizers, so
  * the norm is that of the mean gradient), writes the DEVICE pair out = {total_norm, coef}:
  *   total_norm = fl(fl(sqrt(sumsq[0])) * scale),  coef = min(max_norm / (total_norm + 1e-6f), 1)
@@ -407,20 +418,12 @@ int svdx_clip_coef(const double* sumsq, const float* max_norm, float scale, floa
  * -> [D] diffusers.training_utils.EMAModel.step: get_decay on the host, then per parameter tensor
  * s.sub_((1 - d) * (s - p)) if p.requires_grad else s.copy_(p)).
  * ema_state = double[9] in DEVICE memory: {optimization_step, decay, min_decay, update_after_step, use_ema_warmup (0/1),
- * inv_gamma, power, cur_decay_value, 1 - cur_decay_value}. Every entry point below first advances the step and evaluates
- * EMAModel.get_decay in fp64 on the device (a 1-thread kernel, capturable in a CUDA graph), then applies
- * e = e - (float)(1 - d) * (e - p) with three separately rounded fp32 operations: bit-identical to the torch ops.
+ * inv_gamma, power, cur_decay_value, 1 - cur_decay_value}. Every entry point that takes it (the AdamW updates given an
+ * ema_state, and svdx_ema_multi) first advances the step and evaluates EMAModel.get_decay in fp64 on the device (a 1-thread
+ * kernel, capturable in a CUDA graph), then applies e = e - (float)(1 - d) * (e - p) with three separately rounded fp32
+ * operations: bit-identical to the torch ops.
  *
- * svdx_adamw_graph_ema: svdx_adamw_graph whose update also advances the fp32 EMA buffer ema[0 .. n) at the same flat
- * offsets from the freshly updated masters (16-byte aligned). Two launches. */
-int svdx_adamw_graph_ema(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
-                         void* shadow_bf16, float* ema, double* ema_state, void* stream);
-/* svdx_adamw_p2p plus the EMA of this rank's slice: ema points at the local slice (length n, 16-byte aligned), no peer
- * traffic. tick != 0 advances both the AdamW state and ema_state. */
-int svdx_adamw_p2p_ema(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world,
-                       int64_t lo, int64_t n, float* state, float grad_scale, int32_t tick, float* ema, double* ema_state,
-                       void* stream);
-/* the EMA update over many tensors in one launch (EMAModel.step over parameters outside a fused optimizer).
+ * svdx_ema_multi: the EMA update over many tensors in one launch (EMAModel.step over parameters outside a fused optimizer).
  * jobs: device array of {float* shadow; const float* param; int64 n}; block_prefix[j] = first 4096-element block of job j,
  * total_blocks = sum of ceil(n_j / 4096). Two launches (tick + update). */
 int svdx_ema_multi(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, double* ema_state,
@@ -433,48 +436,27 @@ int svdx_ema_multi(const void* jobs, const int32_t* block_prefix, int32_t njobs,
  * one fp32 absmax per 256-element block and moment (absmax[ceil(n / 256)]); blocks start at the parameter's first element.
  * quant == 0: s1 / s2 are fp32 m / v [n] (parameters below min_8bit_size). shadow (optional): bf16 copy of the new p.
  * block_prefix[j] = first 256-element block of job j, total_blocks = sum of ceil(n_j / 256). qmap1 / qmap2: DEVICE float[256],
- * sorted, shared by every job of the launch. state = svdx_adamw_graph's float[8] (device, advanced by a 1-thread tick first), so
+ * sorted, shared by every job of the launch. state = svdx_adamw_step's float[8] (device, advanced by a 1-thread tick first), so
  * the pair can be captured in a CUDA graph and replayed. Every operation is rounded separately (no FMA); no atomics. Aligned
- * jobs (p, g, fp32 states, shadow, EMA 16-byte; codes 8-byte) take 16-byte loads, others a scalar path. Two launches. */
-int svdx_adamw8bit(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
-                   const float* qmap2, float* state, float grad_scale, void* stream);
-/* svdx_adamw8bit whose update also advances every job's fp32 EMA buffer (job.ema, required) from the new p
- * (svdx_adamw_graph_ema's rule; the tick also advances ema_state). Two launches. */
-int svdx_adamw8bit_ema(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
-                       const float* qmap2, float* state, float grad_scale, double* ema_state, void* stream);
+ * jobs (p, g, fp32 states, shadow, EMA 16-byte; codes 8-byte) take 16-byte loads, others a scalar path. ema_state (optional,
+ * 8-byte aligned): the update also advances every job's fp32 EMA buffer job.ema from the new p, by svdx_adamw_step's rule, and
+ * the tick advances ema_state; NULL: no EMA, job.ema is ignored. grad_mul (optional) as in svdx_adamw_step. Two launches. */
+int svdx_adamw8bit_step(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
+                        const float* qmap2, float* state, float grad_scale, double* ema_state, const float* grad_mul, void* stream);
 
-/* The six update entry points above with one more, trailing argument grad_mul (before the stream): a DEVICE float the
- * gradient is also scaled by, read by the update kernel, so the applied gradient is g * (grad_scale * grad_mul[0]); at
- * grad_scale = 1 that is g * grad_mul[0], the product torch's in-place g.mul_(coef) gives. grad_mul NULL is the entry point
- * without the suffix, bit for bit. Gradient clipping passes out + 1 of svdx_clip_coef, so the clip is decided on the device and
- * a captured step needs no host sync. Every other argument and the launches are those of the form without the suffix. */
-int svdx_adamw_graph_mul(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
-                         void* shadow_bf16, const float* grad_mul, void* stream);
-int svdx_adamw_graph_ema_mul(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
-                             void* shadow_bf16, float* ema, double* ema_state, const float* grad_mul, void* stream);
-int svdx_adamw_p2p_mul(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world,
-                       int64_t lo, int64_t n, float* state, float grad_scale, int32_t tick, const float* grad_mul, void* stream);
-int svdx_adamw_p2p_ema_mul(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world,
-                           int64_t lo, int64_t n, float* state, float grad_scale, int32_t tick, float* ema, double* ema_state,
-                           const float* grad_mul, void* stream);
-int svdx_adamw8bit_mul(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
-                       const float* qmap2, float* state, float grad_scale, const float* grad_mul, void* stream);
-int svdx_adamw8bit_ema_mul(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
-                           const float* qmap2, float* state, float grad_scale, double* ema_state, const float* grad_mul, void* stream);
-
-/* Sharded block-wise 8-bit AdamW over NVLink peer memory (P2PShardedAdamW8bit): reduce-scatter + svdx_adamw8bit + all-gather as
- * ONE kernel, replacing DistributedDataParallel's all-reduce + bitsandbytes.optim.AdamW8bit of train_svd.py:746-773,815-824,
- * 1044-1049 at N > 1. jobs: DEVICE array of this rank's sub-jobs
+/* Sharded block-wise 8-bit AdamW over NVLink peer memory (P2PShardedAdamW8bit): reduce-scatter + svdx_adamw8bit_step +
+ * all-gather as ONE kernel, replacing DistributedDataParallel's all-reduce + bitsandbytes.optim.AdamW8bit of
+ * train_svd.py:746-773,815-824,1044-1049 at N > 1. jobs: DEVICE array of this rank's sub-jobs
  *   {float* p; void* s1; void* s2; float* absmax1; float* absmax2; float* ema; int64 off; int64 n; int64 quant}
  * each a whole number of 256-element blocks of one parameter (a parameter that straddles a shard boundary is split by block
  * range; s1 / s2 / absmax1 / absmax2 / ema point at the sub-job's first block), p / state / EMA this rank's local buffers, and
  * off the arena offset of p[0]. Per element the gradient is sum over r = 0 .. world-1, in rank order from 0, of grads[r][off + i]
- * (the FULL gradient arenas, peer-mapped, as svdx_adamw_p2p sums), times grad_scale (= 1 / world) and grad_mul[0] when grad_mul
- * is not NULL; the update is svdx_adamw8bit's, bit for bit (same roundings, block absmax and maps; no FMA, no atomics); the new
- * bf16 value is stored to shadows[r][off + i] of every rank. tick != 0 first advances state (and ema_state when given) as
- * svdx_adamw_p2p does. ema_state NULL: no EMA; otherwise every job's ema is advanced as in svdx_adamw8bit_ema. The caller
- * orders the ranks around the launch as for svdx_adamw_p2p. grads[r] / shadows[r]: 16-byte aligned; world 1 .. 16. Two launches
- * with tick, one without. */
+ * (the FULL gradient arenas, peer-mapped, as svdx_adamw_step_p2p sums), times grad_scale (= 1 / world) and grad_mul[0] when
+ * grad_mul is not NULL; the update is svdx_adamw8bit_step's, bit for bit (same roundings, block absmax and maps; no FMA, no
+ * atomics); the new bf16 value is stored to shadows[r][off + i] of every rank. tick != 0 first advances state (and ema_state
+ * when given) as svdx_adamw_step_p2p does. ema_state NULL: no EMA; otherwise every job's ema is advanced as in
+ * svdx_adamw8bit_step. The caller orders the ranks around the launch as for svdx_adamw_step_p2p. grads[r] / shadows[r]: 16-byte
+ * aligned; world 1 .. 16. Two launches with tick, one without. */
 int svdx_adamw8bit_p2p(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
                        const float* qmap2, const void* const* grads, void* const* shadows, int32_t world, float* state,
                        float grad_scale, int32_t tick, double* ema_state, const float* grad_mul, void* stream);

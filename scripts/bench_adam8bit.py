@@ -193,7 +193,7 @@ def sharded(form: str, world: int):
     over its own arena with torch.distributed stood in for, and the peer pointer lists point at local buffers, one gradient and
     one shadow slice per rank (only the owned slice [lo, hi) of a peer arena is ever addressed, so each peer buffer covers just
     that slice). These are LOCAL-HBM timings, not NVLink: the peers' gradient reads and shadow writes go to this card's memory.
-    "p2p" times the one-kernel step (tick + svdx_adamw8bit_p2p, the fences left out); "nccl" times the svdx_adamw8bit launch
+    "p2p" times the one-kernel step (tick + svdx_adamw8bit_p2p, the fences left out); "nccl" times the svdx_adamw8bit_step launch
     over rank 0's sub-jobs only (tick + update; the reduce-scatter and the all-gather are not measured). Bytes are counted from
     shapes (svd_xtend_b200.optim8bit.update_bytes: the local HBM traffic, the emulated peer traffic included)."""
     from types import SimpleNamespace
@@ -267,7 +267,7 @@ def sharded(form: str, world: int):
         torch.cuda.empty_cache()
     what = ("the optimizer's step()" if world == 1 else
             "rank 0's launch of N emulated ranks on one card (LOCAL-HBM timing, not NVLink): "
-            + ("tick + svdx_adamw8bit_p2p" if form == "p2p" else "tick + svdx_adamw8bit over its sub-jobs, without the NCCL collectives"))
+            + ("tick + svdx_adamw8bit_p2p" if form == "p2p" else "tick + svdx_adamw8bit_step over its sub-jobs, without the NCCL collectives"))
     line = {"metric": f"sharded 8-bit AdamW ({form}) update, one rank of {world}", "value": out["as_scripted"]["ms"], "unit": "ms",
             "higher_is_better": False, "form": form, "world": world, "what": what + ", CUDA events over 20 launches, medians of 3",
             "hbm_peak_tbps": HBM_TBPS, "card": torch.cuda.get_device_name(dev), "power_limit_w": power_limit_w(0), **out}

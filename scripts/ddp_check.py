@@ -107,7 +107,7 @@ print(f"[ddp_check] rank {rank}: sharded path: bf16 operand update vs all-reduce
 assert e_shadow < 2e-2 and same_shadow and own < 1e-3 and e_masters < 1e-3 and opt.t == 1
 shadow_nccl, data_nccl = arena.shadow.clone(), arena.data.clone()
 
-# ---- (3) the same step as ONE kernel over NVLink peer memory (svdx_adamw_p2p) vs the NCCL sharded step; then three more steps
+# ---- (3) the same step as ONE kernel over NVLink peer memory (svdx_adamw_step_p2p) vs the NCCL sharded step; then three more steps
 # captured in a CUDA graph (fences + kernel replayed) against the eager NCCL optimizer fed the same gradients
 arena.data.copy_(w0)
 arena.refresh_shadow()

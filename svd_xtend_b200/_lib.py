@@ -111,26 +111,15 @@ _PROTOS = {
     "svdx_gemv": [c_void_p, c_i64, c_void_p, c_i64, c_int, c_int, c_int, c_void_p, c_void_p, c_i64, c_int, c_float, c_int, c_void_p],
     "svdx_outer_accum": [c_void_p, c_i64, c_void_p, c_i64, c_int, c_int, c_int, c_void_p, c_void_p, c_i64, c_void_p],
     "svdx_blend_scales": [c_void_p, c_void_p, c_void_p],
-    "svdx_adamw_graph": [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_float, c_void_p, c_void_p],
-    "svdx_adamw_p2p": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_i64, c_i64, c_void_p, c_float, c_int, c_void_p],
+    "svdx_adamw_step": [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
+                        c_void_p],
+    "svdx_adamw_step_p2p": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_i64, c_i64, c_void_p, c_float, c_int,
+                            c_void_p, c_void_p, c_void_p, c_void_p],
     "svdx_grad_sumsq": [c_void_p, c_i64, c_void_p, c_void_p],
     "svdx_grad_sumsq_p2p": [c_void_p, c_int, c_i64, c_i64, c_void_p, c_void_p],
     "svdx_clip_coef": [c_void_p, c_void_p, c_float, c_void_p, c_void_p],
-    "svdx_adamw_graph_ema": [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p],
-    "svdx_adamw_p2p_ema": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_i64, c_i64, c_void_p, c_float, c_int, c_void_p,
-                           c_void_p, c_void_p],
     "svdx_ema_multi": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p],
-    "svdx_adamw8bit": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p],
-    "svdx_adamw8bit_ema": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p],
-    "svdx_adamw_graph_mul": [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_float, c_void_p, c_void_p, c_void_p],
-    "svdx_adamw_graph_ema_mul": [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_float, c_void_p, c_void_p, c_void_p,
-                                 c_void_p, c_void_p],
-    "svdx_adamw_p2p_mul": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_i64, c_i64, c_void_p, c_float, c_int, c_void_p,
-                           c_void_p],
-    "svdx_adamw_p2p_ema_mul": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_i64, c_i64, c_void_p, c_float, c_int,
-                               c_void_p, c_void_p, c_void_p, c_void_p],
-    "svdx_adamw8bit_mul": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p],
-    "svdx_adamw8bit_ema_mul": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p],
+    "svdx_adamw8bit_step": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p],
     "svdx_adamw8bit_p2p": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_float, c_int,
                            c_void_p, c_void_p, c_void_p],
     "svdx_multi_transpose": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p],

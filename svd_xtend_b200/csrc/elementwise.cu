@@ -1560,41 +1560,52 @@ extern "C" int svdx_blend_scales(const float* mix_factor, float* out3, void* str
   return SVDX_OK;
 }
 
-extern "C" int svdx_adamw_graph_mul(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
-                                    void* shadow_bf16, const float* grad_mul, void* stream) {
-  if (!p || !g || !m || !v || !state || n <= 0 || (reinterpret_cast<uintptr_t>(p) & 15) || (reinterpret_cast<uintptr_t>(g) & 15) ||
-      (reinterpret_cast<uintptr_t>(m) & 15) || (reinterpret_cast<uintptr_t>(v) & 15) || (reinterpret_cast<uintptr_t>(shadow_bf16) & 7))
-    return svdx_fail(SVDX_E_BADARG, "adamw_graph: bad arguments (16-byte aligned flat buffers, device state[8])");
-  adamw_tick_kernel<<<1, 1, 0, ST(stream)>>>(state);
+// The optional arguments of the AdamW entry points: ema (16-byte aligned) and ema_state (8-byte aligned) together or not at
+// all, grad_mul 4-byte aligned. NULL passes every alignment test.
+static bool adamw_options_ok(const float* ema, const double* ema_state, const float* grad_mul) {
+  return !ema == !ema_state && !misaligned16(ema) && !(reinterpret_cast<uintptr_t>(ema_state) & 7) &&
+         !(reinterpret_cast<uintptr_t>(grad_mul) & 3);
+}
+
+// The 1-thread tick before an update: the AdamW step and bias corrections, and with an EMA also its decay.
+static void adamw_tick(float* state, double* ema_state, void* stream) {
+  if (ema_state) adamw_ema_tick_kernel<<<1, 1, 0, ST(stream)>>>(state, ema_state);
+  else adamw_tick_kernel<<<1, 1, 0, ST(stream)>>>(state);
+}
+
+// Grid of a grid-stride optimizer kernel: `blocks` CTAs, at most 8 per SM.
+static unsigned capped_grid(long long blocks) {
+  const long long cap = (long long)svdx_num_sms() * 8;
+  return (unsigned)(blocks < cap ? blocks : cap);
+}
+
+// Checks the peer arenas of a p2p launch and copies them to grad[0 .. world) and, unless shadows is NULL, shadow[0 .. world):
+// every gradient arena 16-byte aligned, every shadow arena aligned to shadow_align bytes.
+static bool peer_arenas(const void* const* grads, void* const* shadows, int world, uintptr_t shadow_align, const float** grad,
+                        bf16** shadow) {
+  for (int r = 0; r < world; ++r) {
+    if (!grads[r] || misaligned16(grads[r])) return false;
+    grad[r] = reinterpret_cast<const float*>(grads[r]);
+    if (!shadows) continue;
+    if (!shadows[r] || (reinterpret_cast<uintptr_t>(shadows[r]) & (shadow_align - 1))) return false;
+    shadow[r] = reinterpret_cast<bf16*>(shadows[r]);
+  }
+  return true;
+}
+
+extern "C" int svdx_adamw_step(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale, void* shadow_bf16,
+                               float* ema, double* ema_state, const float* grad_mul, void* stream) {
+  if (!p || !g || !m || !v || !state || n <= 0 || misaligned16(p) || misaligned16(g) || misaligned16(m) || misaligned16(v) ||
+      (reinterpret_cast<uintptr_t>(shadow_bf16) & 7) || !adamw_options_ok(ema, ema_state, grad_mul))
+    return svdx_fail(SVDX_E_BADARG, "adamw_step: bad arguments (16-byte aligned flat buffers and EMA, device state[8], ema and "
+                                    "ema_state[9] together, 4-byte aligned grad_mul)");
+  adamw_tick(state, ema_state, stream);
   const long long n4 = (n + 3) / 4;
-  adamw_state_kernel<false><<<nblocks(n4), 256, 0, ST(stream)>>>(p, g, m, v, n4, n, state, grad_scale, reinterpret_cast<bf16*>(shadow_bf16),
-                                                                 nullptr, nullptr, grad_mul);
-  SVDX_CHECK_LAUNCH("adamw_graph");
+  auto kernel = ema ? adamw_state_kernel<true> : adamw_state_kernel<false>;
+  kernel<<<nblocks(n4), 256, 0, ST(stream)>>>(p, g, m, v, n4, n, state, grad_scale, reinterpret_cast<bf16*>(shadow_bf16), ema, ema_state,
+                                              grad_mul);
+  SVDX_CHECK_LAUNCH("adamw_step");
   return SVDX_OK;
-}
-
-extern "C" int svdx_adamw_graph(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
-                                void* shadow_bf16, void* stream) {
-  return svdx_adamw_graph_mul(p, g, m, v, n, state, grad_scale, shadow_bf16, nullptr, stream);
-}
-
-extern "C" int svdx_adamw_graph_ema_mul(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
-                                        void* shadow_bf16, float* ema, double* ema_state, const float* grad_mul, void* stream) {
-  if (!p || !g || !m || !v || !state || !ema || !ema_state || n <= 0 || (reinterpret_cast<uintptr_t>(p) & 15) ||
-      (reinterpret_cast<uintptr_t>(g) & 15) || (reinterpret_cast<uintptr_t>(m) & 15) || (reinterpret_cast<uintptr_t>(v) & 15) ||
-      (reinterpret_cast<uintptr_t>(ema) & 15) || (reinterpret_cast<uintptr_t>(ema_state) & 7) || (reinterpret_cast<uintptr_t>(shadow_bf16) & 7))
-    return svdx_fail(SVDX_E_BADARG, "adamw_graph_ema: bad arguments (16-byte aligned flat buffers and EMA, device state[8], ema_state[9])");
-  adamw_ema_tick_kernel<<<1, 1, 0, ST(stream)>>>(state, ema_state);
-  const long long n4 = (n + 3) / 4;
-  adamw_state_kernel<true><<<nblocks(n4), 256, 0, ST(stream)>>>(p, g, m, v, n4, n, state, grad_scale, reinterpret_cast<bf16*>(shadow_bf16),
-                                                                ema, ema_state, grad_mul);
-  SVDX_CHECK_LAUNCH("adamw_graph_ema");
-  return SVDX_OK;
-}
-
-extern "C" int svdx_adamw_graph_ema(float* p, const float* g, float* m, float* v, int64_t n, float* state, float grad_scale,
-                                    void* shadow_bf16, float* ema, double* ema_state, void* stream) {
-  return svdx_adamw_graph_ema_mul(p, g, m, v, n, state, grad_scale, shadow_bf16, ema, ema_state, nullptr, stream);
 }
 
 extern "C" int svdx_ema_multi(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, double* ema_state,
@@ -1607,140 +1618,69 @@ extern "C" int svdx_ema_multi(const void* jobs, const int32_t* block_prefix, int
   return SVDX_OK;
 }
 
-static int adamw8bit_launch(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
-                            const float* qmap2, float* state, float grad_scale, double* ema_state, bool ema, const float* grad_mul,
-                            void* stream) {
-  if (!jobs || !block_prefix || !qmap1 || !qmap2 || !state || njobs <= 0 || total_blocks <= 0 || (reinterpret_cast<uintptr_t>(jobs) & 7) ||
-      (reinterpret_cast<uintptr_t>(block_prefix) & 3) || (reinterpret_cast<uintptr_t>(qmap1) & 3) ||
-      (reinterpret_cast<uintptr_t>(qmap2) & 3) || (reinterpret_cast<uintptr_t>(state) & 3) ||
-      (ema && (!ema_state || (reinterpret_cast<uintptr_t>(ema_state) & 7))))
-    return svdx_fail(SVDX_E_BADARG, ema ? "adamw8bit_ema: bad arguments (device job table, block prefix, maps, state[8], ema_state[9])"
-                                        : "adamw8bit: bad arguments (device job table, block prefix, maps, state[8])");
-  long long blocks = (total_blocks + A8_WARPS - 1) / A8_WARPS;
-  const long long cap = (long long)svdx_num_sms() * 8;      // grid-stride: the maps are staged in shared memory once per CTA
-  if (blocks > cap) blocks = cap;
-  const Adam8Job* j = reinterpret_cast<const Adam8Job*>(jobs);
-  if (ema) {
-    adamw_ema_tick_kernel<<<1, 1, 0, ST(stream)>>>(state, ema_state);
-    adamw8bit_kernel<true><<<(unsigned)blocks, 256, 0, ST(stream)>>>(j, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, ema_state,
-                                                                      grad_mul, Adam8NoPeers{});
-  } else {
-    adamw_tick_kernel<<<1, 1, 0, ST(stream)>>>(state);
-    adamw8bit_kernel<false><<<(unsigned)blocks, 256, 0, ST(stream)>>>(j, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, nullptr,
-                                                                       grad_mul, Adam8NoPeers{});
-  }
-  SVDX_CHECK_LAUNCH(ema ? "adamw8bit_ema" : "adamw8bit");
+// The arguments the two 8-bit entry points share: the job table (8-byte aligned), the block prefix, the maps and state[8]
+// (4-byte aligned), and the optional ema_state (8-byte aligned) and grad_mul (4-byte aligned).
+static bool adamw8bit_args_ok(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
+                              const float* qmap2, const float* state, const double* ema_state, const float* grad_mul) {
+  return jobs && block_prefix && qmap1 && qmap2 && state && njobs > 0 && total_blocks > 0 && !(reinterpret_cast<uintptr_t>(jobs) & 7) &&
+         !(reinterpret_cast<uintptr_t>(block_prefix) & 3) && !(reinterpret_cast<uintptr_t>(qmap1) & 3) &&
+         !(reinterpret_cast<uintptr_t>(qmap2) & 3) && !(reinterpret_cast<uintptr_t>(state) & 3) &&
+         !(reinterpret_cast<uintptr_t>(ema_state) & 7) && !(reinterpret_cast<uintptr_t>(grad_mul) & 3);
+}
+
+extern "C" int svdx_adamw8bit_step(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
+                                   const float* qmap2, float* state, float grad_scale, double* ema_state, const float* grad_mul,
+                                   void* stream) {
+  if (!adamw8bit_args_ok(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, ema_state, grad_mul))
+    return svdx_fail(SVDX_E_BADARG, "adamw8bit_step: bad arguments (device job table, block prefix, maps, state[8], 8-byte aligned "
+                                    "ema_state[9], 4-byte aligned grad_mul)");
+  adamw_tick(state, ema_state, stream);
+  // grid-stride: the maps are staged in shared memory once per CTA
+  auto kernel = ema_state ? adamw8bit_kernel<true> : adamw8bit_kernel<false>;
+  kernel<<<capped_grid((total_blocks + A8_WARPS - 1) / A8_WARPS), 256, 0, ST(stream)>>>(
+      reinterpret_cast<const Adam8Job*>(jobs), block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, ema_state, grad_mul,
+      Adam8NoPeers{});
+  SVDX_CHECK_LAUNCH("adamw8bit_step");
   return SVDX_OK;
-}
-
-extern "C" int svdx_adamw8bit(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
-                              const float* qmap2, float* state, float grad_scale, void* stream) {
-  return adamw8bit_launch(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, nullptr, false, nullptr, stream);
-}
-
-extern "C" int svdx_adamw8bit_mul(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
-                                  const float* qmap2, float* state, float grad_scale, const float* grad_mul, void* stream) {
-  return adamw8bit_launch(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, nullptr, false, grad_mul, stream);
-}
-
-extern "C" int svdx_adamw8bit_ema(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
-                                  const float* qmap2, float* state, float grad_scale, double* ema_state, void* stream) {
-  return adamw8bit_launch(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, ema_state, true, nullptr, stream);
-}
-
-extern "C" int svdx_adamw8bit_ema_mul(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks,
-                                      const float* qmap1, const float* qmap2, float* state, float grad_scale, double* ema_state,
-                                      const float* grad_mul, void* stream) {
-  return adamw8bit_launch(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, ema_state, true, grad_mul, stream);
 }
 
 extern "C" int svdx_adamw8bit_p2p(const void* jobs, const int32_t* block_prefix, int32_t njobs, int32_t total_blocks, const float* qmap1,
                                   const float* qmap2, const void* const* grads, void* const* shadows, int32_t world, float* state,
                                   float grad_scale, int32_t tick, double* ema_state, const float* grad_mul, void* stream) {
-  if (!jobs || !block_prefix || !qmap1 || !qmap2 || !grads || !shadows || !state || njobs <= 0 || total_blocks <= 0 || world < 1 ||
-      world > 16 || (reinterpret_cast<uintptr_t>(jobs) & 7) || (reinterpret_cast<uintptr_t>(block_prefix) & 3) ||
-      (reinterpret_cast<uintptr_t>(qmap1) & 3) || (reinterpret_cast<uintptr_t>(qmap2) & 3) || (reinterpret_cast<uintptr_t>(state) & 3) ||
-      (reinterpret_cast<uintptr_t>(ema_state) & 7) || (reinterpret_cast<uintptr_t>(grad_mul) & 3))
+  if (!adamw8bit_args_ok(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, ema_state, grad_mul) || !grads || !shadows ||
+      world < 1 || world > 16)
     return svdx_fail(SVDX_E_BADARG, "adamw8bit_p2p: bad arguments (device job table, block prefix, maps, state[8], world 1..16, "
                                     "8-byte aligned ema_state[9])");
   Adam8Peers src{};
   src.world = world;
-  for (int r = 0; r < world; ++r) {
-    if (!grads[r] || !shadows[r] || (reinterpret_cast<uintptr_t>(grads[r]) & 15) || (reinterpret_cast<uintptr_t>(shadows[r]) & 15))
-      return svdx_fail(SVDX_E_BADARG, "adamw8bit_p2p: null / misaligned peer arena (16-byte aligned gradient and shadow arenas)");
-    src.ptr.grad[r] = reinterpret_cast<const float*>(grads[r]);
-    src.ptr.shadow[r] = reinterpret_cast<bf16*>(shadows[r]);
-  }
-  if (tick) {
-    if (ema_state) adamw_ema_tick_kernel<<<1, 1, 0, ST(stream)>>>(state, ema_state);
-    else adamw_tick_kernel<<<1, 1, 0, ST(stream)>>>(state);
-  }
-  long long blocks = (total_blocks + A8_WARPS - 1) / A8_WARPS;
-  const long long cap = (long long)svdx_num_sms() * 8;
-  if (blocks > cap) blocks = cap;
-  const Adam8P2PJob* j = reinterpret_cast<const Adam8P2PJob*>(jobs);
-  if (ema_state)
-    adamw8bit_kernel<true, true><<<(unsigned)blocks, 256, 0, ST(stream)>>>(j, block_prefix, njobs, total_blocks, qmap1, qmap2, state,
-                                                                            grad_scale, ema_state, grad_mul, src);
-  else
-    adamw8bit_kernel<false, true><<<(unsigned)blocks, 256, 0, ST(stream)>>>(j, block_prefix, njobs, total_blocks, qmap1, qmap2, state,
-                                                                             grad_scale, nullptr, grad_mul, src);
+  if (!peer_arenas(grads, shadows, world, 16, src.ptr.grad, src.ptr.shadow))
+    return svdx_fail(SVDX_E_BADARG, "adamw8bit_p2p: null / misaligned peer arena (16-byte aligned gradient and shadow arenas)");
+  if (tick) adamw_tick(state, ema_state, stream);
+  auto kernel = ema_state ? adamw8bit_kernel<true, true> : adamw8bit_kernel<false, true>;
+  kernel<<<capped_grid((total_blocks + A8_WARPS - 1) / A8_WARPS), 256, 0, ST(stream)>>>(
+      reinterpret_cast<const Adam8P2PJob*>(jobs), block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale, ema_state, grad_mul,
+      src);
   SVDX_CHECK_LAUNCH("adamw8bit_p2p");
   return SVDX_OK;
 }
 
-static int adamw_p2p_launch(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo, int64_t n,
-                            float* state, float grad_scale, int32_t tick, float* ema, double* ema_state, const float* grad_mul,
-                            void* stream) {
-  if (!p || !m || !v || !grads || !shadows || !state || world < 1 || world > 16 || n <= 0 || n % 4 || lo % 4 ||
-      (reinterpret_cast<uintptr_t>(p) & 15) || (reinterpret_cast<uintptr_t>(m) & 15) || (reinterpret_cast<uintptr_t>(v) & 15))
-    return svdx_fail(SVDX_E_BADARG, "adamw_p2p: bad arguments (world <= 16, slice offset / length multiples of 4, 16-byte aligned buffers)");
-  AdamP2P ptr;
-  for (int r = 0; r < 16; ++r) { ptr.grad[r] = nullptr; ptr.shadow[r] = nullptr; }
-  for (int r = 0; r < world; ++r) {
-    if (!grads[r] || !shadows[r] || (reinterpret_cast<uintptr_t>(grads[r]) & 15) || (reinterpret_cast<uintptr_t>(shadows[r]) & 7))
-      return svdx_fail(SVDX_E_BADARG, "adamw_p2p: null / misaligned peer arena");
-    ptr.grad[r] = reinterpret_cast<const float*>(grads[r]);
-    ptr.shadow[r] = reinterpret_cast<bf16*>(shadows[r]);
-  }
-  if (tick) {
-    if (ema) adamw_ema_tick_kernel<<<1, 1, 0, ST(stream)>>>(state, ema_state);
-    else adamw_tick_kernel<<<1, 1, 0, ST(stream)>>>(state);
-  }
+extern "C" int svdx_adamw_step_p2p(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo,
+                                   int64_t n, float* state, float grad_scale, int32_t tick, float* ema, double* ema_state,
+                                   const float* grad_mul, void* stream) {
+  if (!p || !m || !v || !grads || !shadows || !state || world < 1 || world > 16 || n <= 0 || n % 4 || lo % 4 || misaligned16(p) ||
+      misaligned16(m) || misaligned16(v) || !adamw_options_ok(ema, ema_state, grad_mul))
+    return svdx_fail(SVDX_E_BADARG, "adamw_step_p2p: bad arguments (world <= 16, slice offset / length multiples of 4, 16-byte aligned "
+                                    "buffers and EMA slice, ema and ema_state[9] together, 4-byte aligned grad_mul)");
+  AdamP2P ptr{};
+  if (!peer_arenas(grads, shadows, world, 8, ptr.grad, ptr.shadow))
+    return svdx_fail(SVDX_E_BADARG, "adamw_step_p2p: null / misaligned peer arena");
+  if (tick) adamw_tick(state, ema_state, stream);
   const long long n4 = n / 4;
   // a few resident CTAs per SM, grid-stride: enough 16-byte loads in flight to cover the NVLink round trip
-  long long blocks = (n4 + 255) / 256;
-  const long long cap = (long long)svdx_num_sms() * 8;
-  if (blocks > cap) blocks = cap;
-  if (ema) adamw_p2p_kernel<true><<<(unsigned)blocks, 256, 0, ST(stream)>>>(p, m, v, ptr, world, lo, n4, state, grad_scale, ema, ema_state,
-                                                                                  grad_mul);
-  else adamw_p2p_kernel<false><<<(unsigned)blocks, 256, 0, ST(stream)>>>(p, m, v, ptr, world, lo, n4, state, grad_scale, nullptr,
-                                                                                   nullptr, grad_mul);
-  SVDX_CHECK_LAUNCH("adamw_p2p");
+  auto kernel = ema ? adamw_p2p_kernel<true> : adamw_p2p_kernel<false>;
+  kernel<<<capped_grid((n4 + 255) / 256), 256, 0, ST(stream)>>>(p, m, v, ptr, world, lo, n4, state, grad_scale, ema, ema_state, grad_mul);
+  SVDX_CHECK_LAUNCH("adamw_step_p2p");
   return SVDX_OK;
-}
-
-extern "C" int svdx_adamw_p2p(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo, int64_t n,
-                              float* state, float grad_scale, int32_t tick, void* stream) {
-  return adamw_p2p_launch(p, m, v, grads, shadows, world, lo, n, state, grad_scale, tick, nullptr, nullptr, nullptr, stream);
-}
-
-extern "C" int svdx_adamw_p2p_mul(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo,
-                                  int64_t n, float* state, float grad_scale, int32_t tick, const float* grad_mul, void* stream) {
-  return adamw_p2p_launch(p, m, v, grads, shadows, world, lo, n, state, grad_scale, tick, nullptr, nullptr, grad_mul, stream);
-}
-
-extern "C" int svdx_adamw_p2p_ema_mul(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world,
-                                      int64_t lo, int64_t n, float* state, float grad_scale, int32_t tick, float* ema, double* ema_state,
-                                      const float* grad_mul, void* stream) {
-  if (!ema || !ema_state || (reinterpret_cast<uintptr_t>(ema) & 15) || (reinterpret_cast<uintptr_t>(ema_state) & 7))
-    return svdx_fail(SVDX_E_BADARG, "adamw_p2p_ema: null / misaligned EMA slice or ema_state[9]");
-  return adamw_p2p_launch(p, m, v, grads, shadows, world, lo, n, state, grad_scale, tick, ema, ema_state, grad_mul, stream);
-}
-
-extern "C" int svdx_adamw_p2p_ema(float* p, float* m, float* v, const void* const* grads, void* const* shadows, int32_t world, int64_t lo,
-                                  int64_t n, float* state, float grad_scale, int32_t tick, float* ema, double* ema_state, void* stream) {
-  return svdx_adamw_p2p_ema_mul(p, m, v, grads, shadows, world, lo, n, state, grad_scale, tick, ema, ema_state, nullptr, stream);
 }
 
 static int grad_sumsq_launch(const GradSrc& src, bool p2p, long long n4, int tail, double* sumsq, void* stream) {
@@ -1765,10 +1705,8 @@ extern "C" int svdx_grad_sumsq_p2p(const void* const* grads, int32_t world, int6
   if (!grads || !sumsq || world < 1 || world > 16 || n <= 0 || n % 4 || lo < 0 || lo % 4 || (reinterpret_cast<uintptr_t>(sumsq) & 7))
     return svdx_fail(SVDX_E_BADARG, "grad_sumsq_p2p: bad arguments (world <= 16, slice offset / length multiples of 4, double[1025])");
   GradSrc src{};
-  for (int r = 0; r < world; ++r) {
-    if (!grads[r] || (reinterpret_cast<uintptr_t>(grads[r]) & 15)) return svdx_fail(SVDX_E_BADARG, "grad_sumsq_p2p: null / misaligned peer arena");
-    src.grad[r] = reinterpret_cast<const float*>(grads[r]);
-  }
+  if (!peer_arenas(grads, nullptr, world, 1, src.grad, nullptr))
+    return svdx_fail(SVDX_E_BADARG, "grad_sumsq_p2p: null / misaligned peer arena");
   src.world = world;
   src.lo = lo;
   return grad_sumsq_launch(src, true, n / 4, 0, sumsq, stream);

@@ -26,7 +26,7 @@ from . import raw
 
 F32, U8 = torch.float32, torch.uint8
 BLOCK = raw.A8_BLOCK
-# job row of svdx_adamw8bit: p, g, s1, s2, absmax1, absmax2, shadow, ema, n, quant (ten 8-byte fields)
+# job row of svdx_adamw8bit_step: p, g, s1, s2, absmax1, absmax2, shadow, ema, n, quant (ten 8-byte fields)
 JOB_FIELDS = 10
 
 
@@ -68,9 +68,9 @@ def update_bytes(n8: int, n32: int, shadow: bool, ema: bool, world: int = 1) -> 
 
 
 class JobTable:
-    """device job table + block prefix of one svdx_adamw8bit launch. Rows are kept on the host as an int64 array; `set`
+    """device job table + block prefix of one svdx_adamw8bit_step launch. Rows are kept on the host as an int64 array; `set`
     copies them to the device only when a pointer changed (e.g. gradients re-allocated by zero_grad(set_to_none=True)).
-    n_field: the column of the job length (8 in svdx_adamw8bit's rows, 7 in svdx_adamw8bit_p2p's)."""
+    n_field: the column of the job length (8 in svdx_adamw8bit_step's rows, 7 in svdx_adamw8bit_p2p's)."""
 
     def __init__(self, device, n_field: int = 8):
         self.device = device
@@ -151,7 +151,7 @@ def _check_fp32_cuda(t: torch.Tensor, what: str):
 
 
 class AdamW8bit(torch.optim.Optimizer):
-    """bitsandbytes.optim.AdamW8bit's constructor and state dict, on svdx_adamw8bit (see the module docstring)"""
+    """bitsandbytes.optim.AdamW8bit's constructor and state dict, on svdx_adamw8bit_step (see the module docstring)"""
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, amsgrad=False, optim_bits=32, args=None,
                  min_8bit_size=4096, percentile_clipping=100, block_wise=True, is_paged=False):

@@ -29,15 +29,14 @@ def dtype_code(t: torch.Tensor, what: str) -> int:
 
 # number of kernels launched through the C ABI since import (each wrapper adds what its entry point launches)
 LAUNCHES = [0]
-_KERNELS_PER_CALL = {"svdx_groupnorm_apply_fused": 1, "svdx_attention_bwd": 3, "svdx_adamw_graph": 2, "svdx_adamw_p2p": 2,
-                     "svdx_adamw_graph_ema": 2, "svdx_adamw_p2p_ema": 2, "svdx_ema_multi": 2, "svdx_adamw8bit": 2,
-                     "svdx_adamw8bit_ema": 2, "svdx_adamw_graph_mul": 2, "svdx_adamw_graph_ema_mul": 2, "svdx_adamw8bit_mul": 2,
-                     "svdx_adamw8bit_ema_mul": 2, "svdx_adamw_p2p_mul": 2, "svdx_adamw_p2p_ema_mul": 2, "svdx_grad_sumsq": 2,
-                     "svdx_grad_sumsq_p2p": 2, "svdx_adamw8bit_p2p": 2}
+_KERNELS_PER_CALL = {"svdx_groupnorm_apply_fused": 1, "svdx_attention_bwd": 3, "svdx_adamw_step": 2, "svdx_ema_multi": 2,
+                     "svdx_adamw8bit_step": 2, "svdx_grad_sumsq": 2, "svdx_grad_sumsq_p2p": 2}
 
 
-def check(rc: int, what: str = "") -> None:
-    LAUNCHES[0] += _KERNELS_PER_CALL.get(what, 1)
+def check(rc: int, what: str = "", kernels: Optional[int] = None) -> None:
+    """count the call's kernels (`kernels` when the count depends on an argument, else _KERNELS_PER_CALL or 1) and raise
+    when it failed"""
+    LAUNCHES[0] += _KERNELS_PER_CALL.get(what, 1) if kernels is None else kernels
     _lib.check(rc, what)
 
 
@@ -942,7 +941,7 @@ def _ema_args(ema, ema_state, n):
 
 
 def _grad_mul(grad_mul) -> Optional[int]:
-    """device address of the update's gradient multiplier (svd_xtend_b200.h, the *_mul entry points), None without one"""
+    """device address of the update's gradient multiplier (grad_mul in svd_xtend_b200.h), None without one"""
     if grad_mul is None:
         return None
     if grad_mul.dtype != torch.float32 or grad_mul.numel() < 1 or not grad_mul.is_cuda:
@@ -950,41 +949,39 @@ def _grad_mul(grad_mul) -> Optional[int]:
     return grad_mul.data_ptr()
 
 
+def _peer_ptrs(arenas) -> C.Array:
+    """the C array of every rank's arena address; arenas are tensors or already mapped device addresses"""
+    return (C.c_void_p * len(arenas))(*[t if isinstance(t, int) else t.data_ptr() for t in arenas])
+
+
 def adamw_p2p(p, m, v, peer_grads, peer_shadows, lo, state, grad_scale, tick=True, ema=None, ema_state=None, grad_mul=None):
-    """reduce-scatter + AdamW + all-gather in one kernel over NVLink peer memory (svdx_adamw_p2p): p / m / v are this rank's
-    slices, peer_grads / peer_shadows the FULL arenas of every rank (this rank's own included) as tensors mapped into this
-    process (train.map_peer_buffers). With `ema` (this rank's fp32 EMA slice) and `ema_state` the same launch also advances
-    the EMA of the updated masters (svdx_adamw_p2p_ema). grad_mul: a device fp32 scalar the gradient is also multiplied by
-    (the clip coefficient; svdx_adamw_p2p_mul / svdx_adamw_p2p_ema_mul)."""
+    """reduce-scatter + AdamW + all-gather in one kernel over NVLink peer memory (svdx_adamw_step_p2p; tick + update when
+    `tick`): p / m / v are this rank's slices, peer_grads / peer_shadows the FULL arenas of every rank (this rank's own
+    included) as tensors mapped into this process (train.map_peer_buffers). With `ema` (this rank's fp32 EMA slice) and
+    `ema_state` the same launch also advances the EMA of the updated masters. grad_mul: a device fp32 scalar the gradient is
+    also multiplied by (the clip coefficient)."""
     world = len(peer_grads)
     n = p.numel()
     _ema_args(ema, ema_state, n)
     gm = _grad_mul(grad_mul)
     if _fam("adamw", 0.0, (4.0 * world + 28.0 + 2.0 * world + (8.0 if ema is not None else 0.0)) * n):
         return
-    ga = (C.c_void_p * world)(*[t if isinstance(t, int) else t.data_ptr() for t in peer_grads])       # tensors or mapped addresses
-    sa = (C.c_void_p * world)(*[t if isinstance(t, int) else t.data_ptr() for t in peer_shadows])
-    args = (p.data_ptr(), m.data_ptr(), v.data_ptr(), ga, sa, world, lo, n, state.data_ptr(), float(grad_scale), int(tick))
-    if ema is not None:
-        args += (ema.data_ptr(), ema_state.data_ptr())
-    name = "svdx_adamw_p2p" + ("_ema" if ema is not None else "") + ("_mul" if gm is not None else "")
-    check(getattr(load(), name)(*args, *(() if gm is None else (gm,)), _stream()), name)
+    check(load().svdx_adamw_step_p2p(p.data_ptr(), m.data_ptr(), v.data_ptr(), _peer_ptrs(peer_grads), _peer_ptrs(peer_shadows), world,
+                                     lo, n, state.data_ptr(), float(grad_scale), int(tick), _ptr(ema), _ptr(ema_state), gm, _stream()),
+          "svdx_adamw_step_p2p", kernels=2 if tick else 1)
 
 
 def adamw_graph(p, g, m, v, state, grad_scale=1.0, shadow=None, ema=None, ema_state=None, grad_mul=None):
-    """CUDA-graph-safe AdamW: lr / betas / eps / weight decay / step / bias corrections live in the device float[8] `state`.
-    With `ema` (fp32, same length as p) and `ema_state` (device float64[9]) the update also advances the EMA of the new
-    masters at the same offsets (svdx_adamw_graph_ema). grad_mul: a device fp32 scalar the gradient is also multiplied by
-    (the clip coefficient; svdx_adamw_graph_mul / svdx_adamw_graph_ema_mul)."""
+    """CUDA-graph-safe AdamW (svdx_adamw_step): lr / betas / eps / weight decay / step / bias corrections live in the device
+    float[8] `state`. With `ema` (fp32, same length as p) and `ema_state` (device float64[9]) the update also advances the EMA
+    of the new masters at the same offsets. grad_mul: a device fp32 scalar the gradient is also multiplied by (the clip
+    coefficient)."""
     _ema_args(ema, ema_state, p.numel())
     gm = _grad_mul(grad_mul)
     if _fam("adamw", 0.0, ((30.0 if shadow is not None else 28.0) + (8.0 if ema is not None else 0.0)) * p.numel()):
         return
-    args = (p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(), state.data_ptr(), grad_scale, _ptr(shadow))
-    if ema is not None:
-        args += (ema.data_ptr(), ema_state.data_ptr())
-    name = "svdx_adamw_graph" + ("_ema" if ema is not None else "") + ("_mul" if gm is not None else "")
-    check(getattr(load(), name)(*args, *(() if gm is None else (gm,)), _stream()), name)
+    check(load().svdx_adamw_step(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(), state.data_ptr(), grad_scale,
+                                 _ptr(shadow), _ptr(ema), _ptr(ema_state), gm, _stream()), "svdx_adamw_step")
 
 
 SUMSQ_PARTIALS = 1024   # per-block partials of svdx_grad_sumsq: its sumsq buffer is float64[1 + SUMSQ_PARTIALS]
@@ -1012,8 +1009,7 @@ def grad_sumsq_p2p(peer_grads, lo, n, sumsq):
     world = len(peer_grads)
     if _fam("adamw", 0.0, 4.0 * world * n):
         return
-    ga = (C.c_void_p * world)(*[t if isinstance(t, int) else t.data_ptr() for t in peer_grads])
-    check(load().svdx_grad_sumsq_p2p(ga, world, lo, n, sumsq.data_ptr(), _stream()), "svdx_grad_sumsq_p2p")
+    check(load().svdx_grad_sumsq_p2p(_peer_ptrs(peer_grads), world, lo, n, sumsq.data_ptr(), _stream()), "svdx_grad_sumsq_p2p")
 
 
 def clip_coef(sumsq, max_norm, scale, out):
@@ -1039,24 +1035,24 @@ def ema_multi(jobs, block_prefix, njobs, total_blocks, ema_state, nelem):
 A8_BLOCK = 256       # elements per quantisation block of adamw8bit_kernel (one warp)
 
 
-def adamw8bit(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale=1.0, ema_state=None, nbytes=0.0, grad_mul=None):
-    """tick + block-wise 8-bit AdamW over many parameters in one launch (svdx_adamw8bit, svdx_adamw8bit_ema with `ema_state`).
-    jobs: device bytes of the job table (svd_xtend_b200.h); qmap1 / qmap2: device float[256]; state: device float[8];
-    nbytes (the HBM bytes the update moves) is for the byte accounting only. grad_mul: a device fp32 scalar the gradient is
-    also multiplied by (the clip coefficient; the *_mul entry points)."""
+def _adamw8bit_args(what, qmap1, qmap2, ema_state):
     if qmap1.dtype != torch.float32 or qmap2.dtype != torch.float32 or qmap1.numel() != 256 or qmap2.numel() != 256:
-        raise ValueError("adamw8bit: qmap1 / qmap2 are float32[256]")
-    gm = _grad_mul(grad_mul)
+        raise ValueError(f"{what}: qmap1 / qmap2 are float32[256]")
     if ema_state is not None and (ema_state.dtype != torch.float64 or ema_state.numel() < 9):
-        raise ValueError("adamw8bit: ema_state is float64[9] (svd_xtend_b200.h)")
+        raise ValueError(f"{what}: ema_state is float64[9] (svd_xtend_b200.h)")
+
+
+def adamw8bit(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, state, grad_scale=1.0, ema_state=None, nbytes=0.0, grad_mul=None):
+    """tick + block-wise 8-bit AdamW over many parameters in one launch (svdx_adamw8bit_step; every job's EMA advanced too
+    with `ema_state`). jobs: device bytes of the job table (svd_xtend_b200.h); qmap1 / qmap2: device float[256]; state:
+    device float[8]; nbytes (the HBM bytes the update moves) is for the byte accounting only. grad_mul: a device fp32 scalar
+    the gradient is also multiplied by (the clip coefficient)."""
+    _adamw8bit_args("adamw8bit", qmap1, qmap2, ema_state)
+    gm = _grad_mul(grad_mul)
     if _fam("adamw", 0.0, nbytes):
         return
-    args = (jobs.data_ptr(), block_prefix.data_ptr(), njobs, total_blocks, qmap1.data_ptr(), qmap2.data_ptr(), state.data_ptr(),
-            float(grad_scale))
-    if ema_state is not None:
-        args += (ema_state.data_ptr(),)
-    name = "svdx_adamw8bit" + ("_ema" if ema_state is not None else "") + ("_mul" if gm is not None else "")
-    check(getattr(load(), name)(*args, *(() if gm is None else (gm,)), _stream()), name)
+    check(load().svdx_adamw8bit_step(jobs.data_ptr(), block_prefix.data_ptr(), njobs, total_blocks, qmap1.data_ptr(), qmap2.data_ptr(),
+                                     state.data_ptr(), float(grad_scale), _ptr(ema_state), gm, _stream()), "svdx_adamw8bit_step")
 
 
 def adamw8bit_p2p(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, peer_grads, peer_shadows, state, grad_scale, tick=True,
@@ -1065,23 +1061,16 @@ def adamw8bit_p2p(jobs, block_prefix, njobs, total_blocks, qmap1, qmap2, peer_gr
     device table of this rank's sub-jobs (svd_xtend_b200.h), peer_grads / peer_shadows the FULL arenas of every rank as for
     adamw_p2p. ema_state: advance every job's EMA too; grad_mul: the clip coefficient (device fp32). nbytes is for the byte
     accounting only."""
-    if qmap1.dtype != torch.float32 or qmap2.dtype != torch.float32 or qmap1.numel() != 256 or qmap2.numel() != 256:
-        raise ValueError("adamw8bit_p2p: qmap1 / qmap2 are float32[256]")
-    if ema_state is not None and (ema_state.dtype != torch.float64 or ema_state.numel() < 9):
-        raise ValueError("adamw8bit_p2p: ema_state is float64[9] (svd_xtend_b200.h)")
+    _adamw8bit_args("adamw8bit_p2p", qmap1, qmap2, ema_state)
     if len(peer_grads) != len(peer_shadows):
         raise ValueError("adamw8bit_p2p: one gradient and one shadow arena per rank")
     gm = _grad_mul(grad_mul)
     if _fam("adamw", 0.0, nbytes):
         return
-    world = len(peer_grads)
-    ga = (C.c_void_p * world)(*[t if isinstance(t, int) else t.data_ptr() for t in peer_grads])
-    sa = (C.c_void_p * world)(*[t if isinstance(t, int) else t.data_ptr() for t in peer_shadows])
-    rc = load().svdx_adamw8bit_p2p(jobs.data_ptr(), block_prefix.data_ptr(), njobs, total_blocks, qmap1.data_ptr(), qmap2.data_ptr(),
-                                   ga, sa, world, state.data_ptr(), float(grad_scale), int(tick), _ptr(ema_state), gm, _stream())
-    if not tick:
-        LAUNCHES[0] -= 1          # check() counts the tick + update pair
-    check(rc, "svdx_adamw8bit_p2p")
+    check(load().svdx_adamw8bit_p2p(jobs.data_ptr(), block_prefix.data_ptr(), njobs, total_blocks, qmap1.data_ptr(), qmap2.data_ptr(),
+                                    _peer_ptrs(peer_grads), _peer_ptrs(peer_shadows), len(peer_grads), state.data_ptr(),
+                                    float(grad_scale), int(tick), _ptr(ema_state), gm, _stream()),
+          "svdx_adamw8bit_p2p", kernels=2 if tick else 1)
 
 
 def multi_transpose(src_base, jobs, tile_prefix, njobs, total_tiles):

@@ -531,7 +531,7 @@ class _Arena8bit(_ArenaAdamW):
         return self.m32.data_ptr() + 4 * (si - f0), self.v32.data_ptr() + 4 * (si - f0), 0, 0
 
     def job_rows(self):
-        """the svdx_adamw8bit job table of this optimizer's sub-jobs as an int64 array [jobs, 10] (svd_xtend_b200.h)"""
+        """the svdx_adamw8bit_step job table of this optimizer's sub-jobs as an int64 array [jobs, 10] (svd_xtend_b200.h)"""
         import numpy as np
         from .optim8bit import job_row
         a = self.arena
@@ -554,7 +554,7 @@ class _Arena8bit(_ArenaAdamW):
         return self._table
 
     def _launch(self, grad_scale: float, coef: Optional[torch.Tensor]):
-        """tick + svdx_adamw8bit over this optimizer's sub-jobs, gradients read from the arena at the parameters' offsets"""
+        """tick + svdx_adamw8bit_step over this optimizer's sub-jobs, gradients read from the arena at the parameters' offsets"""
         tb = self._job_table(self.job_rows, 8)
         raw.adamw8bit(tb.dev, tb.prefix, tb.njobs, tb.blocks, self.qmap1, self.qmap2, self.state, grad_scale,
                       ema_state=None if self.ema is None else self.ema._state, nbytes=self._nbytes, grad_mul=coef)
@@ -664,7 +664,7 @@ class FusedAdamW8bit(_Arena8bit):
     """FusedAdamW with block-wise 8-bit moments (bitsandbytes' AdamW8bit, train_svd.py --use_8bit_adam; the update is stated in
     oracle/svd_adam8bit_oracle.py): a parameter with at least `min_8bit_size` elements keeps m / v as uint8 codes plus one fp32
     absmax per 256-element block counted from its own arena offset (arena padding belongs to no block); a smaller one keeps
-    fp32 m / v. ONE tick + ONE launch over every parameter (`svdx_adamw8bit`), with the same device `state` float[8] as
+    fp32 m / v. ONE tick + ONE launch over every parameter (`svdx_adamw8bit_step`), with the same device `state` float[8] as
     FusedAdamW, so a captured GraphedStep replays the right sequence. About 2.03 bytes of state per parameter instead of 8.
     The update is deterministic, so under GradReducer every rank's replica stays identical."""
 
@@ -880,7 +880,7 @@ class _PeerShards:
 
 class P2PShardedAdamW(_PeerShards, ShardedAdamW):
     """ShardedAdamW with the three NCCL phases (reduce-scatter, 1/N AdamW, all-gather of the bf16 operands) replaced by ONE
-    kernel over NVLink peer memory (`svdx_adamw_p2p`): every rank reads its slice of every rank's gradient arena directly,
+    kernel over NVLink peer memory (`svdx_adamw_step_p2p`): every rank reads its slice of every rank's gradient arena directly,
     updates its masters / moments and stores the bf16 operands into every rank's shadow arena. Same bytes over the links, no
     intermediate HBM passes, one launch; two tiny all-reduces (captured with the step) order the ranks around it. Results are
     those of ShardedAdamW (bit-identical at world 2; at larger worlds the gradient sum runs in rank order on the owner)."""
@@ -907,7 +907,7 @@ class ShardedAdamW8bit(_Shards, _Arena8bit):
     step's CUDA graph:
 
         reduce-scatter(sum) of the fp32 gradient arena   -> this rank's 1/N slice of the summed gradient   (in place)
-        svdx_adamw8bit over this rank's sub-jobs (grad_scale = 1/N)   -> masters, codes, absmax, fp32 states, bf16 shadow
+        svdx_adamw8bit_step over this rank's sub-jobs (grad_scale = 1/N) -> masters, codes, absmax, fp32 states, bf16 shadow
         all-gather of the bf16 shadow                       -> every rank has all updated operand weights   (in place)
 
     Each rank keeps the 8-bit state of its own blocks only, about 2.03 bytes per parameter / N. The arena must be built with

@@ -414,16 +414,16 @@ def test_missing_parameter_state_is_reported():
 
 
 # ------------------------------------------------------------------------------------------------------------- ABI
-def test_abi_rejects_null_and_misaligned_buffers():
+def test_adamw8bit_step_rejects_null_and_misaligned_buffers():
     from svd_xtend_b200 import build
     build.build()
     from svd_xtend_b200 import _lib
     lib = _lib.load()
-    assert lib.svdx_adamw8bit(None, None, 1, 1, None, None, None, 1.0, None) == -1
+    assert lib.svdx_adamw8bit_step(None, None, 1, 1, None, None, None, 1.0, None, None, None) == -1
     assert b"adamw8bit" in lib.svdx_last_error()
     buf = (ctypes.c_double * 64)()
     a = ctypes.addressof(buf)
-    assert lib.svdx_adamw8bit(a + 4, a, 1, 1, a, a, a, 1.0, None) == -1          # job table not 8-byte aligned
-    assert lib.svdx_adamw8bit(a, a, 0, 1, a, a, a, 1.0, None) == -1              # no jobs
-    assert lib.svdx_adamw8bit_ema(a, a, 1, 1, a, a, a, 1.0, None, None) == -1    # EMA form without ema_state
-    assert lib.svdx_adamw8bit_ema(a, a, 1, 1, a, a, a, 1.0, a + 4, None) == -1   # misaligned ema_state
+    assert lib.svdx_adamw8bit_step(a + 4, a, 1, 1, a, a, a, 1.0, None, None, None) == -1     # job table not 8-byte aligned
+    assert lib.svdx_adamw8bit_step(a, a, 0, 1, a, a, a, 1.0, None, None, None) == -1         # no jobs
+    assert lib.svdx_adamw8bit_step(a, a, 1, 1, a, a, a, 1.0, a + 4, None, None) == -1        # misaligned ema_state
+    assert lib.svdx_adamw8bit_step(a, a, 1, 1, a, a, a, 1.0, None, a + 2, None) == -1        # misaligned grad_mul

@@ -1,4 +1,4 @@
-"""GPU tests of the block-wise 8-bit AdamW: svdx_adamw8bit against oracle/svd_adam8bit_oracle.py BIT FOR BIT (codes, absmax,
+"""GPU tests of the block-wise 8-bit AdamW: svdx_adamw8bit_step against oracle/svd_adam8bit_oracle.py BIT FOR BIT (codes, absmax,
 masters, bf16 shadow, fp32 small-parameter states) through FusedAdamW8bit and the drop-in AdamW8bit, on the config-2 arena of
 the SVD UNet, under CUDA-graph replay, with an attached EMA, across the two front ends, and in the unchanged script's loop."""
 import pytest

@@ -194,20 +194,34 @@ def test_attach_rules_on_cpu_arena():
         ema.step(net.parameters())
 
 
-def test_abi_rejects_bad_ema_arguments():
+def test_adamw_step_abi_rejects_bad_ema_arguments():
     from svd_xtend_b200 import build
     build.build()
     from svd_xtend_b200 import _lib
     lib = _lib.load()
     assert lib.svdx_ema_multi(None, None, 0, 0, None, None) == -1
     assert b"ema_multi" in lib.svdx_last_error()
-    assert lib.svdx_adamw_graph_ema(None, None, None, None, 0, None, 1.0, None, None, None, None) == -1
+    assert lib.svdx_adamw_step(None, None, None, None, 0, None, 1.0, None, None, None, None, None) == -1
     buf = (ctypes.c_double * 16)()
     misaligned = ctypes.addressof(buf) + 4
-    assert lib.svdx_adamw_p2p_ema(None, None, None, None, None, 1, 0, 4, None, 1.0, 1, None, misaligned, None) == -1
-    assert b"adamw_p2p_ema" in lib.svdx_last_error()
-    for name in ("svdx_adamw_graph_ema", "svdx_adamw_p2p_ema", "svdx_ema_multi"):
+    assert lib.svdx_adamw_step_p2p(None, None, None, None, None, 1, 0, 4, None, 1.0, 1, None, misaligned, None, None) == -1
+    assert b"adamw_step_p2p" in lib.svdx_last_error()
+    # every other argument valid: an EMA buffer without its state, or the state without a buffer, is refused
+    a = (ctypes.addressof(buf) + 15) & ~15
+    arenas = (ctypes.c_void_p * 1)(a)
+    for ema, ema_state in ((a, None), (None, a)):
+        assert lib.svdx_adamw_step(a, a, a, a, 4, a, 1.0, None, ema, ema_state, None, None) == -1
+        assert b"adamw_step: bad arguments" in lib.svdx_last_error()
+        assert lib.svdx_adamw_step_p2p(a, a, a, arenas, arenas, 1, 0, 4, a, 1.0, 1, ema, ema_state, None, None) == -1
+        assert b"adamw_step_p2p: bad arguments" in lib.svdx_last_error()
+    for name in ("svdx_adamw_step", "svdx_adamw_step_p2p", "svdx_ema_multi"):
         assert name in _lib._PROTOS
+    # the per-option entry points that svdx_adamw_step / _step_p2p / svdx_adamw8bit_step replace are not exported, so a binding
+    # written for them fails on a missing symbol rather than dropping the EMA or the clip
+    for name in ("svdx_adamw_graph", "svdx_adamw_graph_ema", "svdx_adamw_graph_mul", "svdx_adamw_graph_ema_mul", "svdx_adamw_p2p",
+                 "svdx_adamw_p2p_ema", "svdx_adamw_p2p_mul", "svdx_adamw_p2p_ema_mul", "svdx_adamw8bit", "svdx_adamw8bit_ema",
+                 "svdx_adamw8bit_mul", "svdx_adamw8bit_ema_mul"):
+        assert not hasattr(lib, name), name
 
 
 def test_bench_ema_counts_bytes_from_shapes():

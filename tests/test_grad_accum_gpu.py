@@ -57,7 +57,7 @@ def test_grad_sumsq_matches_fp64_and_repeats_bit_for_bit(n):
 
 @pytest.mark.parametrize("world,rank", [(1, 0), (2, 1), (5, 3)])
 def test_grad_sumsq_p2p_is_the_sumsq_of_the_rank_order_sum(world, rank):
-    """one device, the 'peer' arenas local tensors (as the svdx_adamw_p2p test does)"""
+    """one device, the 'peer' arenas local tensors (as the svdx_adamw_step_p2p test does)"""
     from svd_xtend_b200 import raw
     n_total = 8192 * world
     n = n_total // world

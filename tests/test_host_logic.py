@@ -170,8 +170,8 @@ def test_groupnorm_backward_fusion_is_decided_per_launch():
     assert y.gnb_sums is None
 
 
-def test_peer_memory_optimizer_api_exists():
+def test_peer_memory_optimizer_step_api_exists():
     from svd_xtend_b200 import _lib, train
     assert issubclass(train.P2PShardedAdamW, train.ShardedAdamW)
-    for name in ("svdx_adamw_p2p", "svdx_ipc_export", "svdx_ipc_import", "svdx_enable_peer_access"):
+    for name in ("svdx_adamw_step_p2p", "svdx_ipc_export", "svdx_ipc_import", "svdx_enable_peer_access"):
         assert name in _lib._PROTOS

@@ -384,8 +384,8 @@ def test_groupnorm_fwd_bwd_from_given_channel_sums(raw, outer, rows, C1, C2, sil
 
 @pytest.mark.parametrize("world,rank", [(1, 0), (2, 1), (3, 1), (8, 5)])
 def test_adamw_p2p_kernel_matches_reduce_scatter_adamw_all_gather(raw, world, rank):
-    """svdx_adamw_p2p on one device (the 'peer' arenas are local tensors): slice [lo, hi) of the summed gradients goes through
-    AdamW and lands as bf16 in EVERY shadow arena; everything outside the slice stays untouched. Reference: svdx_adamw_graph on
+    """svdx_adamw_step_p2p on one device (the 'peer' arenas are local tensors): slice [lo, hi) of the summed gradients goes through
+    AdamW and lands as bf16 in EVERY shadow arena; everything outside the slice stays untouched. Reference: svdx_adamw_step on
     the summed gradient slice (what reduce-scatter -> AdamW -> all-gather computes)."""
     n_total = 4096 * world
     n = n_total // world
@@ -411,3 +411,10 @@ def test_adamw_p2p_kernel_matches_reduce_scatter_adamw_all_gather(raw, world, ra
         assert torch.equal(shadows[r][lo:lo + n], sh_ref)
         rest = torch.cat([shadows[r][:lo], shadows[r][lo + n:]])
         assert bool((rest == 7.0).all())
+    # launch accounting: tick + update, or the update alone
+    counts = []
+    for tick in (True, False):
+        l0 = raw.LAUNCHES[0]
+        raw.adamw_p2p(p, m, v, grads, shadows, lo, state, 1.0 / world, tick=tick)
+        counts.append(raw.LAUNCHES[0] - l0)
+    assert counts == [2, 1]

@@ -107,9 +107,9 @@ def test_dicts_interchange_between_the_fused_forms(src, dst):
     assert torch.equal(o1.m, o2.m) and torch.equal(o1.v, o2.v) and torch.equal(o1.state[:6], o2.state[:6])
     _steps(o1, a1, range(3, 5))
     _steps(o2, a2, range(3, 5))
-    if "p2p" not in (src, dst):                      # the same kernel (svdx_adamw_graph) on both sides
+    if "p2p" not in (src, dst):                      # the same kernel (svdx_adamw_step) on both sides
         _assert_same(o1.snapshot_tensors(), o2.snapshot_tensors())
-    else:                                            # svdx_adamw_p2p: the same arithmetic in another kernel
+    else:                                            # svdx_adamw_step_p2p: the same arithmetic in another kernel
         d = (a1.data - a2.data).abs().max().item()
         assert d <= 1e-6 * a1.data.abs().max().item(), d
         assert o1.t == o2.t == 5
